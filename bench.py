@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py - NAR train interactions/s on B200 (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py - NAR train interactions/s on H100 (BASELINE.json metric), one JSON line on rank 0.
 
   python bench.py --gpus N --steps K --warmup W            # this repo (CUDA)
   python bench.py --impl reference --gpus N --steps K --warmup W   # reference CPU path (oracle port)
+  python bench.py --steps K --warmup W --dump-outputs DIR         # + what the last timed step computed, as DIR/*.npy
 
 A "step" = one pass of the NAR training hot path over one batch of synthetic G1-shaped sessions
 (sampler -> feature gather -> CAR -> UGRNN -> FC -> scorer -> softmax-CE -> backward -> TF-Adam).
@@ -10,7 +11,8 @@ A "step" = one pass of the NAR training hot path over one batch of synthetic G1-
   e2e   : the same metric through the reference-facing API (Estimator.train: model_fn / input_fn /
           ItemsStateUpdaterHook) with HOST numpy batches: per step one pinned H2D copy of the inputs,
           the host ClickedItemsState update and a D2H read of the loss, all inside the timed region
-  roofline        : the dominant kernel (CAR GEMM, tensor bound) timed alone, vs MEASURED_PEAKS.json
+  roofline        : the dominant kernel (CAR GEMM, tensor bound) timed alone, vs MEASURED_PEAKS.json if present,
+                    else the H100 SXM data sheet
   roofline_gather : the embedding-gather kernel (HBM bound; the kernel north_star names)
   cpu_baseline    : the oracle (torch-CPU restatement of the TF1.12 graph) on the same workload
 Data parallel (N > 1, torchrun): weak scaling, per-GPU batch fixed, global batch = N x batch;
@@ -48,15 +50,15 @@ def _peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get('hbm_gbs', 6650.0), d.get('bf16_tflops', 1590.0), d.get('bf16_tflops_sustained', 1400.0), 'measured'
-    return 6650.0, 1590.0, 1400.0, 'fallback'
+        return d.get('hbm_gbs', 3350.0), d.get('bf16_tflops', 989.0), d.get('bf16_tflops_sustained', 989.0), 'measured'
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16
+    return 3350.0, 989.0, 989.0, 'H100 SXM data sheet'
 
 
 class ClockSampler:
-    """SM clock / throttle reasons DURING the timed region (B200_PROFILING.md recipe).  Sampled in-process through
-    NVML (the library nvidia-smi itself calls) from a thread, every 10 ms: spawning `nvidia-smi -lms` inside the
-    timed region enumerates every GPU of the box and stalled kernel launches on an 8-GPU node for tens of ms
-    (measured: 4.4 instead of 2.7 ms per step at N=8).  Falls back to an nvidia-smi subprocess started BEFORE the
+    """SM clock / throttle reasons DURING the timed region.  Sampled in-process through NVML (the library nvidia-smi
+    itself calls) from a thread, every 10 ms: spawning `nvidia-smi -lms` inside the timed region enumerates every GPU
+    of the box and can stall kernel launches on an 8-GPU node for tens of ms.  Falls back to an nvidia-smi subprocess started BEFORE the
     warm-up (only its rows from the timed region are used) when pynvml is missing."""
 
     REASONS = [(0x8, 'hw_slowdown'), (0x40, 'hw_thermal_slowdown'), (0x20, 'sw_thermal_slowdown'), (0x4, 'sw_power_cap')]
@@ -196,8 +198,7 @@ def time_oracle(pb, batches, warmup, steps, state=None):
     backward + TF-Adam -> hook.after_run (ClickedItemsState update, numpy like the reference), all timed."""
     import torch
     from oracle import sampler_ref
-    # measured on the GPU box (128 logical CPUs): 8 -> 148, 16 -> 185, 32 -> 177, 64 -> 134, 128 -> 10 interactions/s;
-    # more threads than ~16 only add synchronisation cost to these GEMM sizes, so the baseline runs at its best setting
+    # 16 threads by default (NAR_CPU_THREADS): at these GEMM sizes more threads mostly add synchronisation cost
     torch.set_num_threads(min(os.cpu_count() or 1, int(os.environ.get('NAR_CPU_THREADS', '16'))))
     hp = pb.hp
     o = oracle_for(pb)
@@ -269,7 +270,7 @@ def workload_config(pb, args, gb):
             'sharding': ('contiguous session shards of the global batch, boundaries balanced by valid positions (per-GPU mean '
                          '%d sessions)' % hp.batch_size) if args.gpus > 1 and os.environ.get('NAR_DP_BALANCE', '1') == '1'
                         else 'contiguous session shards, equal counts',
-            'l2_policy': 'no explicit flush: the per-step working set (X,H1,E,dE,PD activations) exceeds the 126 MB L2'}
+            'l2_policy': 'no explicit flush: the per-step working set (X,H1,E,dE,PD activations) exceeds the 50 MB L2'}
 
 
 def run_ours(args):
@@ -319,11 +320,13 @@ def run_ours(args):
 
     side = eng.side_stream()
 
+    last_out = {}
+
     def dev_step(i):
         """step i on the main stream; the weight-independent front of step i+1 (sampler, row lists, statistics)
         is queued on the side stream right behind it (the reference prefetches its next batch the same way)"""
         st = staged[i]
-        eng.step(st, train=True)             # ONE C call: forward + backward, every launch sequenced in libnar_b200
+        last_out['step'] = eng.step(st, train=True)     # ONE C call: forward + backward, every launch sequenced in libnar_b200
         eng.apply_gradients(st)              # (NCCL sum of the gradients when world > 1) + TF-Adam
         if eng.use_side_stream and i + 1 < len(staged):
             eng.prepare(staged[i + 1], eng.global_step + 1, stream=side)
@@ -375,6 +378,8 @@ def run_ours(args):
     n_int = sum(st['L_global'] for st in staged[args.warmup:])
     value = n_int / (ms_total * 1e-3)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:       # before anything below runs the engine again
+        dump_outputs(args.dump_outputs, eng, last_out['step'])
 
     # ------------------------------------------------------------------ BASELINE configs[3]: G1-shaped, GLOBAL batch 4096 on 8 GPUs
     # (512 sessions per GPU).  The scaling series keeps the per-GPU batch of configs[1] (weak scaling, 256 per GPU);
@@ -472,7 +477,7 @@ def run_ours(args):
 
     line = {'metric': 'NAR train interactions/sec', 'value': value, 'unit': 'interactions/s', 'n_gpus': world,
             'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': ms_total / args.steps, 'higher_is_better': True,
-            'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32 (tcgen05: %s forward, single-pass TF32 backward; fp32 accumulate)' % ('bf16x3 (kind::f16, error-compensated)' if eng.fwd_prec == 4 else '3xTF32'), 'dedup_car_layer1': bool(eng.dedup),
+            'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32 (wgmma: %s forward, %s backward; fp32 accumulate)' % ('bf16x3 (error-compensated)' if eng.fwd_prec == 4 else '3xTF32', '3xTF32' if eng.bwd_prec == 3 else 'single-pass TF32'), 'dedup_car_layer1': bool(eng.dedup),
             'data': 'synthetic', 'config': workload_config(pb, args, gb),
             'interactions_per_step': n_int / args.steps,
             'e2e': {'value': e2e_value, 'unit': 'interactions/s', 'h2d_bytes_per_step': h2d_bytes, 'd2h_bytes_per_step': 16,
@@ -494,15 +499,30 @@ def run_ours(args):
     return 0
 
 
-def _ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture
-    (profiles/ncu_traffic.json, written by tools/summarize_ncu.py); None when there is no capture of that kernel."""
-    p = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    try:
-        with open(p) as f:
-            return json.load(f).get(kernel)
-    except Exception:  # noqa: BLE001
-        return None
+DUMP_BUDGET_BYTES = 64 * 1024 * 1024 - 64 * 1024     # all .npy files of one dump, headers included
+
+
+def dump_outputs(out_dir, eng, out):
+    """What the last timed step handed its caller, as out_dir/<name>.npy: the loss accumulators, the logits, the sampled
+    negatives and the parameters after the Adam update.  Every array gets an equal share of DUMP_BUDGET_BYTES; one that
+    does not fit its share is replaced by its entries at a fixed seeded set of flat indices, stored next to it as
+    <name>_index.npy (float64), so that the whole dump stays within the budget."""
+    import torch
+    torch.cuda.synchronize()
+    arrays = {'loss': out['loss'].detach().float().cpu().numpy()[:3],          # xe, l2 regulariser, novelty regulariser
+              'negatives': out['negatives'].detach().cpu().numpy().astype(np.float64),
+              'params': eng.params.detach().cpu().numpy()}
+    if out['logits'] is not None:
+        arrays['logits'] = out['logits'].detach().float().cpu().numpy()
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BUDGET_BYTES // len(arrays)
+    for name, a in arrays.items():
+        if a.nbytes > share:
+            k = share // (a.itemsize + 8)                   # sampled values + their float64 indices
+            idx = np.sort(np.random.RandomState(0).choice(a.size, k, replace=False))
+            np.save(os.path.join(out_dir, name + '_index.npy'), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
 
 
 def kernel_rooflines(eng, st, hbm_peak, tf_peak, peak_src):
@@ -544,9 +564,8 @@ def kernel_rooflines(eng, st, hbm_peak, tf_peak, peak_src):
     # SURVEY.md 8(d): per interaction (2+K)*(E+Di)*4 read + same written + (2+K)*8 index bytes
     gbytes = L * ((2 + K) * (E + Di) * 4 * 2 + (2 + K) * 8)
     actual = R * plan.Fp * 4 + R * (E + Di) * 4 + R * 12
-    traffic = _ncu_traffic('gather_features_kernel')
     roof_g = {'kernel': 'gather_features_kernel', 'bound': 'hbm', 'achieved': gbytes / (ms_g * 1e-3) / 1e9, 'peak': hbm_peak,
-              'unit': 'GB/s', 'frac': gbytes / (ms_g * 1e-3) / 1e9 / hbm_peak, 'traffic': traffic, 'peak_source': peak_src,
+              'unit': 'GB/s', 'frac': gbytes / (ms_g * 1e-3) / 1e9 / hbm_peak, 'peak_source': peak_src,
               'rows': R, 'us': ms_g * 1e3, 'algorithmic_bytes': gbytes, 'bytes_moved_incl_all_feature_columns': actual,
               'achieved_incl_all_columns': actual / (ms_g * 1e-3) / 1e9,
               'event_pair_overhead_us': ms_0 * 1e3,
@@ -556,10 +575,9 @@ def kernel_rooflines(eng, st, hbm_peak, tf_peak, peak_src):
                       'event-pair overhead reported next to it; algorithmic bytes count only the ACR + item-embedding rows, '
                       'the kernel also writes the %d context / metadata / recency / novelty / padding columns of every row'
                       % (plan.Fp - E - Di)}
-    # (c) the embedding gather where the HBM roofline actually applies: the G1 tables (46 MB ACR + 22 MB item embeddings) and
-    # the <= 1.5 K distinct rows a step touches live in the 126 MB L2, so (a) and (b) never see HBM.  Same row shape (250
-    # floats, ld 252), but a table far larger than L2 and distinct random ids: every row comes from HBM once and is written
-    # once (nar_gather_rows_f32, the kernel behind tf.nn.embedding_lookup nar_model.py:948); plus its gradient scatter-add.
+    # (c) the embedding gather with the table in HBM: a step touches <= 1.5 K distinct rows of the G1 tables, which L2
+    # largely keeps between launches.  Same row shape (250 floats, ld 252), but a table far larger than the 50 MB L2 and
+    # distinct random ids: every row comes from HBM once and is written once (nar_gather_rows_f32, the kernel behind tf.nn.embedding_lookup nar_model.py:948); plus its gradient scatter-add.
     try:
         Vb, nb_rows = 1 << 20, 1 << 18
         tab = torch.randn(Vb, 252, device='cuda')
@@ -576,8 +594,7 @@ def kernel_rooflines(eng, st, hbm_peak, tf_peak, peak_src):
             'scatter_add': {'kernel': 'scatter_add_rows_kernel', 'us': ms_s * 1e3,
                             'achieved': nb_rows * (250 * 4 * 3 + 8) / (ms_s * 1e-3) / 1e9,      # read src + read-modify-write of the row
                             'frac': nb_rows * (250 * 4 * 3 + 8) / (ms_s * 1e-3) / 1e9 / hbm_peak},
-            'note': '1 Mi x 252 fp32 table (1 GB, 8x the L2), 256 Ki distinct random ids: the only form of this gather that is HBM '
-                    'bound; at G1 size the tables are L2 resident'}
+            'note': '1 Mi x 252 fp32 table (1 GB, 20x the L2), 256 Ki distinct random ids: every row comes from HBM'}
         roof_g['frac_hbm_resident_form'] = roof_g['hbm_resident_form']['frac']
         del tab, gtab, outb, ids
     except Exception as ex:  # noqa: BLE001
@@ -613,16 +630,14 @@ def kernel_rooflines(eng, st, hbm_peak, tf_peak, peak_src):
     ms_1 = timeit(lambda: car2(1), iters=10)
     used = eng.fwd_prec
     ms_m = ms_4 if used == 4 else ms_3
-    # operand bytes each SM pulls into shared memory per 128x128 output tile and 32-k tile, times the tiles: the forward
-    # GEMMs are bound by that L2 -> shared-memory ingest, not by the tensor pipe (DESIGN.md section 4)
+    # operand bytes TMA brings into shared memory per 128x128 output tile and 32-k tile, times the tiles
     tiles = ((R + 127) // 128) * ((eng.C + 127) // 128) * ((eng.C + 31) // 32)
-    roof = {'kernel': ('gemm_tf32_kernel<MODE 4: bf16x3, A split into packed bf16 pairs in tensor memory, pre-split bf16 weight plane>'
-                       if used == 4 else 'gemm_tf32_kernel<MODE 3: 3xTF32 with the A split kept in tensor memory>') +
+    roof = {'kernel': ('gemm_kernel<MODE 4: bf16x3, A split in registers, pre-split bf16 weight plane>'
+                       if used == 4 else 'gemm_kernel<MODE 2: 3xTF32, A split in registers, B_lo plane from HBM>') +
                       ' (CAR_representation layer 2 forward)', 'bound': 'tensor',
             'achieved': flops / (ms_m * 1e-3) / 1e12, 'peak': tf_peak, 'unit': 'TFLOP/s',
             'frac': flops / (ms_m * 1e-3) / 1e12 / tf_peak,
-            'traffic': _ncu_traffic('gemm_tf32_kernel<0,0,4,1,1>' if used == 4 else 'gemm_tf32_kernel<0,1,3,1,1>'),
-            'peak_source': peak_src + ' cuBLAS bf16 (burst)',
+            'peak_source': peak_src,
             'issued_mma_flops_frac_of_peak': (3.0 * flops / (ms_m * 1e-3) / 1e12) / (tf_peak if used == 4 else tf_peak / 2.0),
             'shape': [R, eng.C, eng.C], 'us': ms_m * 1e3, 'forward_precision': used,
             'smem_ingest_GBps': tiles * (32768 if used == 4 else 49152) / (ms_m * 1e-3) / 1e9,
@@ -646,6 +661,8 @@ def main():
     ap.add_argument('--state-warmup', type=int, default=100)
     ap.add_argument('--cpu-steps', type=int, default=5)
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy')
     ap.add_argument('--global-batch', type=int, default=0,
                     help='sessions per step over ALL ranks (per-GPU batch = this / world); 0 = the workload batch per GPU (weak scaling)')
     args = ap.parse_args()
@@ -657,6 +674,8 @@ def main():
     if args.warmup < 3 and args.impl == 'ours':
         args.warmup = 3
     if args.impl == 'reference':
+        if args.dump_outputs:
+            ap.error('--dump-outputs writes what the CUDA path computed; it does not apply to --impl reference')
         args.warmup = max(1, args.warmup)
         return run_reference(args)
     return run_ours(args)

@@ -1,5 +1,5 @@
 """ctypes binding of libnar_b200.so (include/nar_b200.h).  There is no fallback: if the
-library is missing or no sm_100 device is present, loading / ctx creation raises."""
+library is missing or no sm_90 device is present, loading / ctx creation raises."""
 from __future__ import annotations
 
 import ctypes as C
@@ -175,7 +175,7 @@ def check(rc: int, what: str = ''):
 
 
 class Context:
-    """Owns a nar_ctx for one device.  Raises when no sm_100 device is available."""
+    """Owns a nar_ctx for one device.  Raises when no sm_90 device is available."""
 
     def __init__(self, device: int = 0):
         lib = load()

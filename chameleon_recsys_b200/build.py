@@ -1,4 +1,4 @@
-"""Build libnar_b200.so (sm_100a only) in-tree with nvcc.  No torch extension machinery:
+"""Build libnar_b200.so (sm_90a only) in-tree with nvcc.  No torch extension machinery:
 the product is a plain C-ABI shared library (include/nar_b200.h) loaded with ctypes."""
 from __future__ import annotations
 
@@ -10,9 +10,9 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnar_b200.so')
-SOURCES = ['gemm_tcgen05.cu', 'features.cu', 'sampler.cu', 'rnn.cu', 'loss.cu', 'misc.cu', 'host_state.cu', 'state.cu', 'car.cu',
+SOURCES = ['gemm_wgmma.cu', 'features.cu', 'sampler.cu', 'rnn.cu', 'loss.cu', 'misc.cu', 'host_state.cu', 'state.cu', 'car.cu',
            'gru.cu', 'engine.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-diag-suppress', '128',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-diag-suppress', '128',
               '-Xcompiler', '-fPIC']
 
 
@@ -53,7 +53,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
         list(ex.map(run, jobs))
     objs = [os.path.join(objdir, s.replace('.cu', '.o')) for s in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        run([nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'])
+        run([nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'])
     return LIB
 
 

@@ -1,4 +1,4 @@
-// Shared device helpers for libnar_b200 (sm_100a only).
+// Shared device helpers for libnar_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>
@@ -27,6 +27,8 @@ struct nar_ctx {
   int gather_key_valid;
 };
 #define NAR_GATHER_DESC_BYTES (2 * 512 * 16 + 64)
+// grid-stride kernels launched without a nar_ctx cap their grid at a few blocks per SM of an H100 SXM (132 SMs)
+#define NAR_GRID_SMS 132
 
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 

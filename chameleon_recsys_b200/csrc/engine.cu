@@ -56,7 +56,7 @@ struct StepBufs {
 
 }  // namespace
 
-// bf16x3 planes of the forward weights (fwd_precision 4; see gemm_tcgen05.cu MODE 4): one entry per (weight block, K) a
+// bf16x3 planes of the forward weights (fwd_precision 4; see gemm_wgmma.cu MODE 4): one entry per (weight block, K) a
 // forward GEMM uses; refreshed by one nar_pack_bf16x3 launch after every optimiser step / weight load
 constexpr int MAX_PLANES = 32;
 struct PlaneSet {

@@ -582,7 +582,7 @@ extern "C" int nar_build_base_rows(const int32_t* pos_idx, int64_t L, const int6
   if (L <= 0) return NAR_OK;
   NAR_CHECK_CUDA(cudaMemsetAsync(Mt, 0, (size_t)U * (size_t)ld_mt * sizeof(uint16_t), as_stream(stream)));
   const int64_t total = 2 * L + U + L * K;
-  int64_t g = (total + 255) / 256; if (g > 148 * 8) g = 148 * 8;
+  int64_t g = (total + 255) / 256; if (g > NAR_GRID_SMS * 8) g = NAR_GRID_SMS * 8;
   nar::feat::build_base_rows_kernel<<<(unsigned)g, 256, 0, as_stream(stream)>>>(pos_idx, L, item_clicked, label_next_item,
                                                                               unique_items, n_unique, U, neg_uidx, K,
                                                                               base_pos, base_item, Mt, ld_mt);
@@ -595,7 +595,7 @@ extern "C" int nar_build_rows(const int32_t* pos_idx, int64_t L, const int64_t* 
   if (!pos_idx || !item_clicked || !label_next_item || !negatives || !row_pos || !row_item || K < 0) return NAR_ERR_INVALID;
   if (L <= 0) return NAR_OK;
   const int64_t total = L * (K + 2);
-  int64_t g = (total + 255) / 256; if (g > 148 * 8) g = 148 * 8;
+  int64_t g = (total + 255) / 256; if (g > NAR_GRID_SMS * 8) g = NAR_GRID_SMS * 8;
   nar::feat::build_rows_kernel<<<(unsigned)g, 256, 0, as_stream(stream)>>>(pos_idx, L, item_clicked, label_next_item, negatives, K, row_pos, row_item);
   NAR_LAUNCH_CHECK();
   return NAR_OK;

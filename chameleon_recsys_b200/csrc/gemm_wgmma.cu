@@ -1,0 +1,589 @@
+// TMA-fed wgmma GEMM (sm_90a) with fused epilogues for the NAR dense layers.
+//
+//   D[M,N] = epilogue( sum_k A(m,k) * B(n,k) )
+//
+// Replaces every tf.layers.Dense of the reference graph (nar_model.py:375-473) and the UGRNN
+// input projection (:1317); forward, dgrad and wgrad all go through this one kernel by
+// choosing operand majors (no transposed copies of activations are ever made):
+//   fwd   Y  = X  * W        A = X  (K-major)   B = W   (MN-major: W is [in,out]) or W^T (K-major)
+//   dgrad dX = dY * W^T      A = dY (K-major)   B = W   (K-major)
+//   wgrad dW = X^T * dY      A = X  (MN-major)  B = dY  (MN-major), split-K + red.add
+//
+// CTA = 256 threads = two warpgroups, one 128 x 128 output tile, k-tiles of 32 (32 fp32 = one 128-byte swizzle row):
+//   thread 0     keeps STAGES k-tiles of A and B in flight (cp.async.bulk.tensor.2d, 128-byte swizzle, one mbarrier
+//                per stage) and refills a stage as soon as every thread is done with it;
+//   warpgroup w  multiplies rows [64w, 64w + 64) of the tile with wgmma.m64n128: A from registers, B from shared
+//                memory.  A is read from the swizzled TMA tile straight into the register fragment whatever its major,
+//                and that is also where 3xTF32 splits it.  wgmma reads 32-bit B operands only K-major, so a B tile that
+//                arrives MN-major (the forward weights W [in,out], the wgrad dY) is first transposed in shared memory
+//                by all 256 threads; the same pass writes B's lo part for 3xTF32.
+//   epilogue     accumulators -> shared memory -> row-contiguous bias / activation / activation-derivative and
+//                st.global.v4, or red.global.add.v4 for split-K.
+//
+// 3xTF32: hi = x with the low 13 mantissa bits cleared, lo = x - hi; D += Alo*Bhi + Ahi*Blo + Ahi*Bhi restores ~fp32
+// accuracy (the reference is fp32 end to end and logits are divided by temperature 0.1 before exp).
+//   MODE 0: single pass.   MODE 1: 3x, B_lo computed in-kernel.   MODE 2: 3x, B_lo read from HBM (nar_adam_tf keeps it).
+//   MODE 4: bf16x3 - the same error compensation with bf16 pieces on the bf16 tensor path, which runs at twice the tf32
+//           rate: x = hi + lo with hi = bf16(x), lo = bf16(x - hi) (16 mantissa bits kept).  A: fp32 K-major tile by
+//           TMA, split in registers.  B: a pre-split, TRANSPOSED bf16 plane maintained next to the weights
+//           (nar_pack_bf16x3): row n holds, per block of 32 k, the 32 hi values followed by the 32 lo values = one
+//           128-byte swizzle row, so ONE K-major TMA box brings both halves and no transpose pass is needed.
+#include "common.cuh"
+#include <cuda_bf16.h>
+#include <stdlib.h>
+#include <string.h>
+
+namespace nar {
+namespace gemm {
+
+constexpr int BM = 128;
+constexpr int BN = 128;
+constexpr int BK = 32;                       // 32 fp32 = 128 B = one 128-byte swizzle span
+constexpr int TILE_BYTES = 128 * BK * 4;     // one 128 x 32 fp32 operand tile (= one 128 x 64 bf16 plane tile)
+constexpr int NUM_THREADS = 256;
+constexpr int EPI_LD = BN + 4;               // floats per staged accumulator row (16-byte aligned rows)
+
+template <int MODE, bool B_MN> struct Cfg {
+  static constexpr bool SPLIT3 = MODE == 1 || MODE == 2;
+  static constexpr bool BLO = MODE == 2;
+  static constexpr bool PREP = B_MN || SPLIT3;                        // B goes through the transpose / split pass
+  static constexpr int STAGE_BYTES = TILE_BYTES * (BLO ? 3 : 2);      // A | B [| B_lo]
+  static constexpr int STAGES = BLO ? 3 : 4;
+  static constexpr int PREP_BYTES = PREP ? TILE_BYTES * (SPLIT3 ? 2 : 1) : 0;   // K-major B_hi [| B_lo]
+  static constexpr int BAR_OFF = STAGES * STAGE_BYTES + PREP_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;              // + barriers + alignment slack
+  static_assert(STAGES * STAGE_BYTES >= BM * EPI_LD * 4, "the epilogue stages the accumulators in the operand ring");
+  static_assert(SMEM_BYTES <= 227 * 1024, "227 KB of shared memory per block");
+};
+
+struct Params {
+  int64_t M, N, K;
+  float* D; int64_t ldd;
+  const float* bias;
+  const float* aux; int64_t ld_aux;
+  int act, dact, accumulate;
+  int k_tiles_per_split;
+  int n_tiles;                 // blockIdx.x = m_blk * n_tiles + n_blk (N fastest: CTAs sharing an A tile run together)
+};
+
+// ---------------------------------------------------------------- PTX wrappers
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  const uint32_t addr = smem_u32(bar);
+  uint32_t ok = 0;
+  // bounded spin: a protocol bug traps (launch error) instead of hanging the GPU
+  for (uint32_t it = 0; it < (1u << 26); ++it) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
+    if (ok) return;
+  }
+  __trap();
+}
+__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+__device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 128] += A[64 x 8] (registers, tf32) * B[128 x 8] (shared memory, K-major)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
+      : "memory");
+}
+// D[64 x 128] += A[64 x 16] (registers, bf16 pairs) * B[128 x 16] (shared memory, K-major)
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
+      : "memory");
+}
+
+// wgmma shared-memory descriptor: [0,14) start>>4, [16,30) LBO>>4 (unused for swizzled K-major), [32,46) SBO>>4,
+// [62,64) layout (1 = 128-byte swizzle).  K-major tile of 128-byte rows, 8-row atoms 1024 B apart; stepping k within
+// the row adds the byte offset to the start address (tiles are 1024-byte aligned, so the swizzle phase is right).
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 62);
+}
+
+__device__ __forceinline__ uint32_t tf32_hi_bits(uint32_t x) { return x & 0xFFFFE000u; }
+
+// x -> (bf16(x), bf16(x - bf16(x))) for two consecutive k values, each pair packed low = even k
+__device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const float2 hf = __bfloat1622float2(h);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(a - hf.x, b - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// Byte offset of element (mn, k) in a 128 x 32 fp32 operand tile as TMA wrote it with the 128-byte swizzle:
+//   K-major:  one box of 128 rows x 128 B, 16-byte chunk c of row r at chunk c ^ (r & 7)
+//   MN-major: four boxes of 32 k-rows x 32 MN (4096 B each), chunk c of k-row k at chunk c ^ (k & 7)
+template <bool MN_MAJOR>
+__device__ __forceinline__ uint32_t tile_off(int mn, int k) {
+  return MN_MAJOR ? (uint32_t)((mn >> 5) * 4096 + k * 128 + ((((mn >> 2) & 7) ^ (k & 7)) << 4) + (mn & 3) * 4)
+                  : (uint32_t)(mn * 128 + (((k >> 2) ^ (mn & 7)) << 4) + (k & 3) * 4);
+}
+
+// B tile of the current stage -> K-major swizzled B_hi [| B_lo] tiles that wgmma reads.
+template <bool B_MN, int MODE>
+__device__ __forceinline__ void prep_b(const uint8_t* b, const uint8_t* blo, uint8_t* hi_out, uint8_t* lo_out, int tid) {
+  constexpr bool SPLIT3 = MODE == 1 || MODE == 2;
+  if (B_MN) {
+    // thread = a block of 4 n x 4 k: four 16-byte reads along n (one per k), four 16-byte writes along k (one per n);
+    // both sides are 8 distinct 16-byte chunks per 8 lanes, i.e. free of bank conflicts
+    const int c = tid & 7, kq = (tid >> 3) & 7, box = tid >> 6;
+    float v[4][4], l[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int k = 4 * kq + i;
+      const uint32_t off = (uint32_t)(box * 4096 + k * 128 + ((c ^ (k & 7)) << 4));
+      const float4 x = *reinterpret_cast<const float4*>(b + off);
+      v[i][0] = x.x; v[i][1] = x.y; v[i][2] = x.z; v[i][3] = x.w;
+      if (MODE == 2) {
+        const float4 y = *reinterpret_cast<const float4*>(blo + off);
+        l[i][0] = y.x; l[i][1] = y.y; l[i][2] = y.z; l[i][3] = y.w;
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int n = box * 32 + 4 * c + q;
+      const uint32_t off = (uint32_t)(n * 128 + ((kq ^ (n & 7)) << 4));
+      float4 h = make_float4(v[0][q], v[1][q], v[2][q], v[3][q]);
+      if (SPLIT3) {
+        const float4 x = h;
+        h.x = __uint_as_float(tf32_hi_bits(__float_as_uint(x.x))); h.y = __uint_as_float(tf32_hi_bits(__float_as_uint(x.y)));
+        h.z = __uint_as_float(tf32_hi_bits(__float_as_uint(x.z))); h.w = __uint_as_float(tf32_hi_bits(__float_as_uint(x.w)));
+        const float4 lo = MODE == 2 ? make_float4(l[0][q], l[1][q], l[2][q], l[3][q])
+                                    : make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+        *reinterpret_cast<float4*>(lo_out + off) = lo;
+      }
+      *reinterpret_cast<float4*>(hi_out + off) = h;
+    }
+  } else {
+    // K-major already: same layout, element-wise split
+#pragma unroll
+    for (int i = 0; i < TILE_BYTES / 16 / NUM_THREADS; ++i) {
+      const uint32_t off = (uint32_t)((tid + i * NUM_THREADS) * 16);
+      const float4 x = *reinterpret_cast<const float4*>(b + off);
+      float4 h;
+      h.x = __uint_as_float(tf32_hi_bits(__float_as_uint(x.x))); h.y = __uint_as_float(tf32_hi_bits(__float_as_uint(x.y)));
+      h.z = __uint_as_float(tf32_hi_bits(__float_as_uint(x.z))); h.w = __uint_as_float(tf32_hi_bits(__float_as_uint(x.w)));
+      const float4 lo = MODE == 2 ? *reinterpret_cast<const float4*>(blo + off)
+                                  : make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+      *reinterpret_cast<float4*>(hi_out + off) = h;
+      *reinterpret_cast<float4*>(lo_out + off) = lo;
+    }
+  }
+}
+
+// Epilogue element work for 4 consecutive columns of one row: bias / activation / activation-derivative / store.
+__device__ __forceinline__ void epilogue_store4(const Params& p, float4 v, int64_t row, int64_t col, const float4& a) {
+  float* d = p.D + row * p.ldd + col;
+  if (col + 4 <= p.N) {
+    if (p.bias) {
+      const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+      v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
+    }
+    if (p.act) { v.x = apply_act(v.x, p.act); v.y = apply_act(v.y, p.act); v.z = apply_act(v.z, p.act); v.w = apply_act(v.w, p.act); }
+    if (p.dact) {        // `a` = aux[row, col..col+3], loaded by the caller
+      v.x *= act_grad_from_output(a.x, p.dact); v.y *= act_grad_from_output(a.y, p.dact);
+      v.z *= act_grad_from_output(a.z, p.dact); v.w *= act_grad_from_output(a.w, p.dact);
+    }
+    if (p.accumulate) atomicAdd(reinterpret_cast<float4*>(d), v);        // red.global.add.v4.f32
+    else *reinterpret_cast<float4*>(d) = v;
+  } else {
+    const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (col + j < p.N) {
+        float x = e[j];
+        if (p.bias) x += p.bias[col + j];
+        x = apply_act(x, p.act);
+        if (p.dact) x *= act_grad_from_output(p.aux[row * p.ld_aux + col + j], p.dact);
+        if (p.accumulate) atomicAdd(d + j, x); else d[j] = x;
+      }
+    }
+  }
+}
+
+// TMA for one 128 x 32 fp32 operand tile at MN coordinate mn0, K element k_elem
+template <bool MN_MAJOR>
+__device__ __forceinline__ void load_operand(uint32_t dst, const CUtensorMap* map, uint64_t* bar, int mn0, int k_elem) {
+  if (!MN_MAJOR) {
+    tma_load_2d(dst, map, bar, k_elem, mn0);                       // one box: 128 rows x 128 B
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) tma_load_2d(dst + i * 4096, map, bar, mn0 + i * 32, k_elem);   // boxes of 32 MN x 32 k
+  }
+}
+
+// ---------------------------------------------------------------- kernel
+template <bool A_MN, bool B_MN, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_blo, const Params p) {
+  using C = Cfg<MODE, B_MN>;
+  constexpr bool BF16 = MODE == 4;
+  static_assert(!BF16 || (!A_MN && !B_MN), "bf16x3: A K-major fp32, B the transposed (K-major) bf16 plane");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* prep = smem + C::STAGES * C::STAGE_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);     // [STAGES] TMA landed
+
+  const int tid = threadIdx.x;
+  const int n_blk = (int)(blockIdx.x % p.n_tiles), m_blk = (int)(blockIdx.x / p.n_tiles);
+  const int k_tiles_total = (int)((p.K + BK - 1) / BK);
+  const int kt0 = blockIdx.y * p.k_tiles_per_split;
+  const int num_kt = min(kt0 + p.k_tiles_per_split, k_tiles_total) - kt0;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    if (C::BLO) tma_prefetch_desc(&tmap_blo);
+    for (int s = 0; s < C::STAGES; ++s) mbar_init(&full[s], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  auto issue = [&](int kt) {          // thread 0: k-tile kt -> stage kt % STAGES
+    const int s = kt % C::STAGES;
+    uint64_t* bar = &full[s];
+    mbar_expect_tx(bar, C::STAGE_BYTES);
+    const uint32_t a_dst = smem_u32(smem + s * C::STAGE_BYTES);
+    const uint32_t b_dst = a_dst + TILE_BYTES;
+    const int k_elem = (kt0 + kt) * BK;
+    load_operand<A_MN>(a_dst, &tmap_a, bar, m_blk * BM, k_elem);
+    if (BF16) {
+      tma_load_2d(b_dst, &tmap_b, bar, (kt0 + kt) * 64, n_blk * BN);    // 128 n-rows x (32 hi | 32 lo) bf16
+    } else {
+      load_operand<B_MN>(b_dst, &tmap_b, bar, n_blk * BN, k_elem);
+      if (C::BLO) load_operand<B_MN>(b_dst + TILE_BYTES, &tmap_blo, bar, n_blk * BN, k_elem);
+    }
+  };
+  if (tid == 0)
+    for (int kt = 0; kt < C::STAGES && kt < num_kt; ++kt) issue(kt);
+
+  // wgmma fragments: warp w (of 8) owns tile rows [16w, 16w + 16); lane = 4 g + t.  A: rows 16w + g (+8), k t (+4)
+  // for tf32, k 2t (+8) for bf16 pairs.  D: rows 16w + g (+8), columns 8j + 2t (+1).
+  const int warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int r0 = warp * 16 + g;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+
+  for (int kt = 0; kt < num_kt; ++kt) {
+    const int s = kt % C::STAGES;
+    mbar_wait(&full[s], (uint32_t)(kt / C::STAGES) & 1u);
+    const uint8_t* sa = smem + s * C::STAGE_BYTES;
+    const uint8_t* sb = sa + TILE_BYTES;
+    if (C::PREP) {
+      prep_b<B_MN, MODE>(sb, sb + TILE_BYTES, prep, prep + TILE_BYTES, tid);
+      fence_proxy_async_smem();       // generic-proxy writes -> wgmma (async proxy) reads
+      __syncthreads();
+    }
+    const uint32_t b_hi = smem_u32(C::PREP ? prep : sb);
+    const uint32_t b_lo = b_hi + TILE_BYTES;        // 3x: the prep B_lo tile
+    if (BF16) {
+      uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int r = r0 + (q & 1) * 8, k = 16 * j + 2 * t + (q >> 1) * 8;
+          const float2 x = *reinterpret_cast<const float2*>(sa + tile_off<false>(r, k));
+          split_bf16x2(x.x, x.y, ahi[j][q], alo[j][q]);
+        }
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {        // two k = 16 steps per 32-k tile: 32 B of the hi half, then of the lo half
+        wgmma_bf16(acc, alo[j], make_desc(b_hi + 32 * j));          // A_lo * B_hi
+        wgmma_bf16(acc, ahi[j], make_desc(b_hi + 64 + 32 * j));     // A_hi * B_lo
+        wgmma_bf16(acc, ahi[j], make_desc(b_hi + 32 * j));          // A_hi * B_hi
+      }
+    } else {
+      uint32_t a[4][4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          a[j][q] = *reinterpret_cast<const uint32_t*>(sa + tile_off<A_MN>(r0 + (q & 1) * 8, 8 * j + t + (q >> 1) * 4));
+      if (C::SPLIT3) {
+        uint32_t alo[4][4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const uint32_t h = tf32_hi_bits(a[j][q]);
+            alo[j][q] = __float_as_uint(__uint_as_float(a[j][q]) - __uint_as_float(h));
+            a[j][q] = h;
+          }
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {      // small terms first
+          wgmma_tf32(acc, alo[j], make_desc(b_hi + 32 * j));
+          wgmma_tf32(acc, a[j], make_desc(b_lo + 32 * j));
+          wgmma_tf32(acc, a[j], make_desc(b_hi + 32 * j));
+        }
+      } else {
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wgmma_tf32(acc, a[j], make_desc(b_hi + 32 * j));
+      }
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_acc(acc);
+    __syncthreads();                  // every thread is done with stage s and the prep tiles
+    if (tid == 0 && kt + C::STAGES < num_kt) issue(kt + C::STAGES);
+  }
+
+  // ===== epilogue: the accumulators go through shared memory (the operand ring is idle now) so that each warp then
+  // handles 128 contiguous bytes of one row of D / aux per instruction
+  float* stage = reinterpret_cast<float*>(smem);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = 8 * j + 2 * t;
+    *reinterpret_cast<float2*>(stage + r0 * EPI_LD + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(stage + (r0 + 8) * EPI_LD + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+  __syncthreads();
+  const int c4 = lane * 4;
+  const int64_t col = (int64_t)n_blk * BN + c4;
+  if (col >= p.N) return;
+  for (int it = 0; it < BM / 8; ++it) {
+    const int rl = it * 8 + warp;
+    const int64_t row = (int64_t)m_blk * BM + rl;
+    if (row >= p.M) break;
+    const float4 v = *reinterpret_cast<const float4*>(stage + rl * EPI_LD + c4);
+    float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (p.dact && col + 4 <= p.N) av = *reinterpret_cast<const float4*>(p.aux + row * p.ld_aux + col);
+    epilogue_store4(p, v, row, col, av);
+  }
+}
+
+// ---------------------------------------------------------------- host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// operand with logical shape [mn, k]; kmajor: ptr[mn*ld + k] else ptr[k*ld + mn].  Out-of-range boxes read zeros.
+static int make_operand_map(const nar_ctx* ctx, CUtensorMap* map, const float* ptr, int64_t mn, int64_t k, int64_t ld, bool kmajor) {
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15u) != 0 || (ld & 3) != 0 || ld <= 0) return NAR_ERR_INVALID;
+  cuuint64_t dims[2]; cuuint64_t strides[1]; cuuint32_t box[2]; cuuint32_t estr[2] = {1, 1};
+  if (kmajor) { dims[0] = (cuuint64_t)k; dims[1] = (cuuint64_t)mn; box[0] = BK; box[1] = 128; }
+  else        { dims[0] = (cuuint64_t)mn; dims[1] = (cuuint64_t)k; box[0] = 32; box[1] = BK; }
+  strides[0] = (cuuint64_t)ld * 4;
+  CUresult r = reinterpret_cast<EncodeTiledFn>(ctx->encode_tiled)(
+      map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
+      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? NAR_OK : NAR_ERR_INVALID;
+}
+
+// the pre-split bf16 weight plane of MODE 4: [n_rows, ld] bf16, K-major, 64 elements (128 B) of it per 32-k tile
+static int make_bf16_plane_map(const nar_ctx* ctx, CUtensorMap* map, const void* ptr, int64_t n_rows, int64_t k_tiles, int64_t ld) {
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15u) != 0 || (ld & 7) != 0 || ld < k_tiles * 64) return NAR_ERR_INVALID;
+  cuuint64_t dims[2] = {(cuuint64_t)(k_tiles * 64), (cuuint64_t)n_rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {64, 128};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = reinterpret_cast<EncodeTiledFn>(ctx->encode_tiled)(
+      map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? NAR_OK : NAR_ERR_INVALID;
+}
+
+// nar_pack_bf16x3: W [K, N] fp32 (row stride ldw) -> plane [N, ld_out] bf16 (see MODE 4).  32 x 32 tiles through shared
+// memory: reads coalesced along n, writes 64 contiguous bytes (32 hi or 32 lo values of one n) per half warp.
+struct PackDesc { const float* W; uint16_t* out; int K, N, ldw, ld_out; };
+constexpr int MAX_PACK = 32;
+constexpr int PACK_MAX_BLOCKS = 2 * 132;     // grid-stride; two blocks per SM of an H100 SXM
+
+__global__ void __launch_bounds__(256)
+pack_bf16x3_kernel(const PackDesc* __restrict__ descs) {
+  __shared__ float tile[32][33];
+  const PackDesc d = descs[blockIdx.y];
+  const int kb_n = (d.K + 31) / 32, nb_n = (d.N + 31) / 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;          // 32 x 8
+  for (int t = blockIdx.x; t < kb_n * nb_n; t += gridDim.x) {
+    const int kb = t / nb_n, nb = t - kb * nb_n;
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8) {
+      const int k = kb * 32 + i, n = nb * 32 + tx;
+      tile[i][tx] = (k < d.K && n < d.N) ? d.W[(int64_t)k * d.ldw + n] : 0.f;
+    }
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8) {                             // i = n within the tile, tx = k within the block
+      const int n = nb * 32 + i;
+      if (n < d.N) {
+        const float x = tile[tx][i];
+        const __nv_bfloat16 h = __float2bfloat16_rn(x);
+        const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
+        uint16_t* o = d.out + (int64_t)n * d.ld_out + kb * 64 + tx;
+        o[0] = *reinterpret_cast<const uint16_t*>(&h);
+        o[32] = *reinterpret_cast<const uint16_t*>(&l);
+      }
+    }
+  }
+}
+
+template <bool A_MN, bool B_MN, int MODE>
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tbl, const Params& p, dim3 grid, cudaStream_t st) {
+  auto kern = gemm_kernel<A_MN, B_MN, MODE>;
+  constexpr int smem = Cfg<MODE, B_MN>::SMEM_BYTES;
+  static bool attr_set = false;     // per instantiation
+  if (!attr_set) {
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set = true;
+  }
+  kern<<<grid, NUM_THREADS, smem, st>>>(ta, tb, tbl, p);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+}  // namespace gemm
+}  // namespace nar
+
+extern "C" int nar_pack_bf16x3(const float* const* W, void* const* out, const int32_t* K, const int32_t* N, const int32_t* ldw,
+                               const int32_t* ld_out, int n, void* descs_dev, void* stream) {
+  using namespace nar::gemm;
+  if (!W || !out || !K || !N || !ldw || !ld_out || !descs_dev || n <= 0 || n > MAX_PACK) return NAR_ERR_INVALID;
+  PackDesc h[MAX_PACK];
+  int max_tiles = 1;
+  for (int i = 0; i < n; ++i) {
+    if (!W[i] || !out[i] || K[i] <= 0 || N[i] <= 0 || ld_out[i] < (K[i] + 31) / 32 * 64) return NAR_ERR_INVALID;
+    h[i].W = W[i]; h[i].out = static_cast<uint16_t*>(out[i]); h[i].K = K[i]; h[i].N = N[i]; h[i].ldw = ldw[i]; h[i].ld_out = ld_out[i];
+    const int t = ((K[i] + 31) / 32) * ((N[i] + 31) / 32);
+    max_tiles = t > max_tiles ? t : max_tiles;
+  }
+  // the descriptor table is written once per distinct set (callers keep it; stream-ordered copy from a pageable buffer
+  // would be a sync, so it goes through a kernel-argument-sized async memcpy only when it changed)
+  static PackDesc last[MAX_PACK]; static int last_n = 0; static void* last_dev = nullptr;
+  if (last_dev != descs_dev || last_n != n || memcmp(last, h, sizeof(PackDesc) * n) != 0) {
+    NAR_CHECK_CUDA(cudaMemcpy(descs_dev, h, sizeof(PackDesc) * n, cudaMemcpyHostToDevice));
+    memcpy(last, h, sizeof(PackDesc) * n); last_n = n; last_dev = descs_dev;
+  }
+  dim3 grid((unsigned)(max_tiles > PACK_MAX_BLOCKS ? PACK_MAX_BLOCKS : max_tiles), (unsigned)n);
+  pack_bf16x3_kernel<<<grid, 256, 0, as_stream(stream)>>>(static_cast<const PackDesc*>(descs_dev));
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda, int a_kmajor,
+                             const float* B, int64_t ldb, int b_kmajor, float* D, int64_t ldd,
+                             const nar_gemm_epilogue* epi, void* stream) {
+  using namespace nar::gemm;
+  if (!ctx || !ctx->encode_tiled) return NAR_ERR_NO_DEVICE;
+  if (!A || !D || !epi || (!B && epi->precision != 4)) return NAR_ERR_INVALID;
+  if (M <= 0 || N <= 0 || K <= 0) return NAR_OK;     // empty problem: nothing to do
+  if ((ldd & 3) != 0 || (reinterpret_cast<uintptr_t>(D) & 15u) != 0) return NAR_ERR_INVALID;
+  if (epi->bias && (reinterpret_cast<uintptr_t>(epi->bias) & 15u) != 0) return NAR_ERR_INVALID;
+  if (epi->dact && (!epi->aux || (epi->ld_aux & 3) != 0 || (reinterpret_cast<uintptr_t>(epi->aux) & 15u) != 0)) return NAR_ERR_INVALID;
+  if (epi->precision != 1 && epi->precision != 3 && epi->precision != 4) return NAR_ERR_INVALID;
+  const bool bf16 = epi->precision == 4;
+  if (bf16 && (!a_kmajor || !epi->b_bf16 || epi->accumulate || epi->split_k > 1)) return NAR_ERR_INVALID;
+  const bool blo = epi->precision == 3 && epi->b_lo != nullptr;
+  const int mode = bf16 ? 4 : (epi->precision == 1 ? 0 : (blo ? 2 : 1));
+  const int64_t n_tiles = (N + BN - 1) / BN, m_tiles = (M + BM - 1) / BM;
+  if (n_tiles * m_tiles > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
+  const int k_tiles = (int)((K + BK - 1) / BK);
+  int split = epi->split_k;
+  if (split <= 0) {          // auto: about two waves of CTAs, at least 8 k-tiles per split
+    split = 1;
+    if (epi->accumulate) {
+      const int64_t want = (2 * (int64_t)ctx->sm_count + n_tiles * m_tiles - 1) / (n_tiles * m_tiles);
+      const int64_t cap = k_tiles / 8 > 1 ? k_tiles / 8 : 1;
+      split = (int)(want < cap ? want : cap);
+      if (split < 1) split = 1;
+    }
+  }
+  if (split > k_tiles) split = k_tiles;
+  if (split > 1 && !epi->accumulate) return NAR_ERR_INVALID;
+  int per = (k_tiles + split - 1) / split;
+  split = (k_tiles + per - 1) / per;          // no empty splits
+  CUtensorMap ta, tb;
+  int rc = make_operand_map(ctx, &ta, A, M, K, lda, a_kmajor != 0);
+  if (rc) return rc;
+  if (bf16) rc = make_bf16_plane_map(ctx, &tb, epi->b_bf16, N, k_tiles, epi->ld_bf16);
+  else rc = make_operand_map(ctx, &tb, B, N, K, ldb, b_kmajor != 0);
+  if (rc) return rc;
+  CUtensorMap tbl = tb;
+  if (blo) {
+    rc = make_operand_map(ctx, &tbl, epi->b_lo, N, K, ldb, b_kmajor != 0);
+    if (rc) return rc;
+  }
+  Params p;
+  p.M = M; p.N = N; p.K = K; p.D = D; p.ldd = ldd; p.bias = epi->bias; p.aux = epi->aux; p.ld_aux = epi->ld_aux;
+  p.act = epi->act; p.dact = epi->dact; p.accumulate = epi->accumulate; p.k_tiles_per_split = per;
+  p.n_tiles = (int)n_tiles;
+  dim3 grid((unsigned)(n_tiles * m_tiles), (unsigned)split, 1);
+  cudaStream_t st = as_stream(stream);
+  if (mode == 4) return launch<false, false, 4>(ta, tb, tbl, p, grid, st);
+  const bool amn = !a_kmajor, bmn = !b_kmajor;
+#define NAR_GEMM_CASE(a, b) \
+  if (amn == a && bmn == b) { \
+    if (mode == 0) return launch<a, b, 0>(ta, tb, tbl, p, grid, st); \
+    if (mode == 1) return launch<a, b, 1>(ta, tb, tbl, p, grid, st); \
+    return launch<a, b, 2>(ta, tb, tbl, p, grid, st); \
+  }
+  NAR_GEMM_CASE(false, false) NAR_GEMM_CASE(false, true) NAR_GEMM_CASE(true, false) NAR_GEMM_CASE(true, true)
+#undef NAR_GEMM_CASE
+  return NAR_ERR_INVALID;
+}

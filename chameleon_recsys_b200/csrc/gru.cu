@@ -5,7 +5,7 @@
 //     [r, u] = sigmoid([x, h] * Wg + bg)          gates/kernel [in+H, 2H], gates/bias (initialised to 1.0)
 //     c      = tanh([x, r*h] * Wc + bc)           candidate/kernel [in+H, H], candidate/bias
 //     h'     = u * h + (1 - u) * c
-// The input projections x*Wg[:in] + bg | x*Wc[:in] + bc of ALL time steps are tcgen05 GEMMs (nar_gemm_tf32) into
+// The input projections x*Wg[:in] + bg | x*Wc[:in] + bc of ALL time steps are wgmma GEMMs (nar_gemm_tf32) into
 // gx [L, 3Hp] = (r | u | c); what is left is the sequential part, independent per session, with TWO dependent
 // matrix-vector products per step (h * Whg, then (r*h) * Whc).  Same work split as csrc/rnn.cu: one CTA owns SB
 // sessions, slots sorted longest first so that finished sessions cost nothing; rows are the valid positions only.

@@ -247,7 +247,7 @@ extern "C" int nar_mul_pred(const float* cand, const float* pred, int64_t n_pos,
   const int64_t rows = n_pos * n_cand;
   if (rows <= 0) return NAR_OK;
   const int64_t total = rows * (C / 4);
-  const unsigned grid = (unsigned)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  const unsigned grid = (unsigned)((total + 255) / 256 > NAR_GRID_SMS * 16 ? NAR_GRID_SMS * 16 : (total + 255) / 256);
   nar::loss::mul_pred_kernel<<<grid, 256, 0, as_stream(stream)>>>(reinterpret_cast<const float4*>(cand), reinterpret_cast<const float4*>(pred),
                                                                    rows, n_cand, (int)(C / 4), reinterpret_cast<float4*>(prod));
   NAR_LAUNCH_CHECK();

@@ -118,7 +118,7 @@ dropout_rows_kernel(const float* __restrict__ src, float* __restrict__ dst, int6
 
 static unsigned grid_for(int64_t n, int per_block) {
   int64_t g = (n + per_block - 1) / per_block;
-  const int64_t cap = 148 * 8;
+  const int64_t cap = NAR_GRID_SMS * 8;
   return (unsigned)(g > cap ? cap : (g < 1 ? 1 : g));
 }
 
@@ -145,7 +145,7 @@ extern "C" const char* nar_status_string(int status) {
     case NAR_OK: return "ok";
     case NAR_ERR_INVALID: return "invalid argument";
     case NAR_ERR_UNSUPPORTED: return "unsupported";
-    case NAR_ERR_NO_DEVICE: return "no sm_100 CUDA device / driver entry point";
+    case NAR_ERR_NO_DEVICE: return "no sm_90 CUDA device / driver entry point";
     case NAR_ERR_WORKSPACE: return "workspace too small";
   }
   if (status > 0) return cudaGetErrorString((cudaError_t)status);
@@ -159,7 +159,7 @@ extern "C" int nar_ctx_create(int device, nar_ctx** out) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0 || device < 0 || device >= n) return NAR_ERR_NO_DEVICE;
   cudaDeviceProp prop;
   NAR_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return NAR_ERR_NO_DEVICE;        // sm_100a code only
+  if (prop.major != 9) return NAR_ERR_NO_DEVICE;         // sm_90a code only
   NAR_CHECK_CUDA(cudaSetDevice(device));
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult q;

@@ -1,5 +1,5 @@
 // UGRNN recurrence of the session RNN (tf.contrib.rnn.UGRNNCell inside dynamic_rnn,
-// nar_model.py:1308-1342).  The input projection x*Wx + b of ALL time steps is one tcgen05 GEMM
+// nar_model.py:1308-1342).  The input projection x*Wx + b of ALL time steps is one wgmma GEMM
 // (nar_gemm_tf32); what is left is the sequential part, independent per session:
 //     act = gx[t] + h * Wh ;  g = sigmoid(act_g + 1) ; c = tanh(act_c) ; h' = g*h + (1-g)*c
 // Rows are the valid positions only (session b owns rows [sess_off[b], sess_off[b+1])), so

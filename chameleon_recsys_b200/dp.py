@@ -1,6 +1,6 @@
 """Data-parallel host logic (numpy only; no CUDA needed, so it is testable with gloo on CPU).
 
-The reference has no distribution at all (README.md:252: single worker on purpose).  The B200 build
+The reference has no distribution at all (README.md:252: single worker on purpose).  The H100 build
 shards the *sessions* of one global batch contiguously across ranks (chronological order per rank is
 kept; boundaries balanced by valid positions, see shard_bounds) and keeps global-batch semantics
 identical to one GPU (SURVEY.md section 8e):

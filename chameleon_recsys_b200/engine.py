@@ -40,7 +40,7 @@ class NarEngine:
                  dedup: Optional[bool] = None, keep_prob: float = 1.0, novelty_reg_factor: float = 0.0,
                  dropout_seed: Optional[int] = None):
         if not torch.cuda.is_available():
-            raise NarError('NarEngine needs a CUDA (sm_100a) device; there is no CPU fallback')
+            raise NarError('NarEngine needs a CUDA (sm_90a) device; there is no CPU fallback')
         if rnn_cell not in ('ugrnn', 'gru'):
             raise ValueError("rnn_cell=%r: 'ugrnn' (the reference's UGRNNCell, nar_model.py:1318) or 'gru' (GRUCell, :1315)" % rnn_cell)
         if rnn_cell != getattr(layout, 'rnn_cell', 'ugrnn'):
@@ -117,8 +117,12 @@ class NarEngine:
         self.ops = ops
         self._ctx = ops.context(self.dev.index)     # fail loudly here if the library / device is unusable
         self._lib = self._ctx.lib
-        # step workspaces: sized for the worst case (every position valid) when that fits the budget, else grown
-        self._ws_budget = int(float(os.environ.get('NAR_WS_BUDGET_GB', '40')) * (1 << 30))
+        # step workspaces: sized for the worst case (every position valid) when that fits the budget, else grown.  Default
+        # budget: a quarter of the device (20 GB on an 80 GB H100), so that a worst-case workspace plus the superseded ones
+        # a regrowth keeps alive leave room for weights, Adam slots and the caching allocator
+        budget = os.environ.get('NAR_WS_BUDGET_GB')
+        self._ws_budget = (int(float(budget) * (1 << 30)) if budget else
+                           torch.cuda.get_device_properties(self.dev).total_memory // 4)
         self._L_cap = 0
         self._ws: Optional[torch.Tensor] = None
         self._prep_ws: Dict[str, torch.Tensor] = {}
@@ -259,7 +263,7 @@ class NarEngine:
 
     def _ensure_capacity(self, Bg: int, B: int, T: int, L: int, slot: str):
         """Workspaces for a step with L valid positions.  Sized once for the worst case (all B*T positions valid) when
-        that fits NAR_WS_BUDGET_GB (the reference configurations at their per-GPU batch: a few GB of the 180 GB); beyond
+        that fits the workspace budget (G1 at its per-GPU batch: 8 GB, within the 20 GB default on an 80 GB H100); beyond
         that (stress shapes) sized for 1.25x the largest L seen - a regrowth keeps the superseded buffers alive until
         the steps that use them are done.  Allocated on the current (main) stream's pool."""
         self._sync_cfg()

@@ -1,6 +1,6 @@
 """``NARModuleModel`` and ``ItemsStateUpdaterHook`` - the reference's model-side API
 (nar_module/nar/nar_model.py:100-129 ctor, :1370-1470 / :1504-1511 / :1635-1650 hook) on top of
-the B200 engine.
+the H100 engine.
 
 TF builds a symbolic graph per ``model_fn`` call and the hook feeds placeholders per step; here
 the object is built once (weights + ACR table resident in HBM) and ``run(features, labels)``

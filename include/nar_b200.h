@@ -1,5 +1,5 @@
 /*
- * nar_b200.h - C ABI of the B200-native NAR (CHAMELEON next-article recommendation)
+ * nar_b200.h - C ABI of the H100-native NAR (CHAMELEON next-article recommendation)
  * training hot path.  libnar_b200.so exports exactly these symbols.
  *
  * The reference (gabrielspmoreira/chameleon_recsys @ 2e50af5) has NO native / FFI layer:
@@ -29,7 +29,7 @@ typedef enum {
   NAR_OK = 0,
   NAR_ERR_INVALID = -1,        /* bad argument (null pointer, misaligned ld, size limit) */
   NAR_ERR_UNSUPPORTED = -2,    /* valid request the library does not implement */
-  NAR_ERR_NO_DEVICE = -3,      /* no sm_100 device / driver entry point missing */
+  NAR_ERR_NO_DEVICE = -3,      /* no sm_90 device / driver entry point missing */
   NAR_ERR_WORKSPACE = -4       /* workspace too small */
 } nar_status;
 
@@ -155,8 +155,8 @@ int nar_scatter_add_rows_f32(float* table, int64_t n_table_rows, int64_t ld, int
 
 /* ---- dense contraction (replaces every tf.layers.Dense nar_model.py:375-473 and the
  *      UGRNN input projection :1317 -> Eigen/MKL or cuBLAS sgemm in the reference).
- *      D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ), TMA-fed tcgen05.mma kind::tf32, fp32
- *      accumulation in TMEM.  a_kmajor: A(m,k) = A[m*lda + k] else A[k*lda + m];
+ *      D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ), TMA-fed wgmma (tf32 or bf16 operands), fp32
+ *      accumulation in registers.  a_kmajor: A(m,k) = A[m*lda + k] else A[k*lda + m];
  *      b_kmajor: B(n,k) = B[n*ldb + k] else B[k*ldb + n].                                  */
 typedef enum { NAR_ACT_NONE = 0, NAR_ACT_LEAKY_RELU = 1, NAR_ACT_TANH = 2 } nar_act;
 
@@ -171,7 +171,7 @@ typedef struct {
   int32_t precision;      /* 1 = TF32, 3 = 3xTF32 (error-compensated, ~fp32 accuracy) */
   const float* b_lo;      /* precision 3 only, optional: x - tf32_trunc(x) of operand B, same shape / ld as B (see
                              nar_tf32_lo; the weights' lo plane is maintained by nar_adam_tf).  NULL: split B in-kernel */
-  const void* b_bf16;     /* precision 4 (bf16x3: bf16 hi + lo pieces on the kind::f16 path, fp32 accumulate; A must be K-major
+  const void* b_bf16;     /* precision 4 (bf16x3: bf16 hi + lo pieces on the bf16 tensor path, fp32 accumulate; A must be K-major
                              fp32): operand B as the pre-split transposed plane written by nar_pack_bf16x3 - [N, ld_bf16]
                              bf16, row n = per block of 32 k the 32 hi values then the 32 lo values; B / ldb are ignored */
   int64_t ld_bf16;        /* elements per row of b_bf16 (>= ceil(K/32)*64, multiple of 8) */

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE - specification of the dropout masks of the B200 NAR path (numpy).
+"""TEST INFRASTRUCTURE - specification of the dropout masks of the H100 NAR path (numpy).
 
 The reference applies tf.layers.dropout to the three feature tensors (nar_model.py:338-340, :351-353, :367-369), to
 the FC1 output (:417-419) and wraps every RNN cell in DropoutWrapper(output_keep_prob) (:1330-1333).  TF's stateful

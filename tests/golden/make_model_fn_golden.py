@@ -39,6 +39,7 @@ ref_state = importlib.import_module('refnar.clicked_items_state')
 
 import torch  # noqa: E402
 from chameleon_recsys_b200.harness import make_problem, warm_state  # noqa: E402
+from oracle.golden_sampling import preset_variables  # noqa: E402
 
 torch.set_num_threads(1)
 golden = np.load(os.path.join(HERE, 'model_golden.npz'))
@@ -62,7 +63,7 @@ for mode, case, skip in (('train', 'train64', 0), ('eval', 'eval64', 1)):
     trainer.clicked_items_state = st
     trainer.FLAGS.disable_eval_benchmarks = True
     trainer.FLAGS.enabled_internal_features = [trainer.ALL_FEATURES]
-    preset = {k[len('train64/var/'):]: golden[k] for k in golden.files if k.startswith('train64/var/')}
+    preset = preset_variables(golden, 'train64')
     shim.configure(float64=True, seed=3, preset=preset, feeds={
         'articles_metadata': [pb.articles_metadata[k] for k in pb.articles_metadata],
         'content_article_embeddings_matrix': pb.content_article_embeddings_matrix,

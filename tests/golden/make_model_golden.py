@@ -4,12 +4,13 @@ stand-in tests/golden/tf1_shim.py (TensorFlow 1.12 itself cannot be installed he
 this pins (the model's wiring - the reference's own code ran) and what it does not (per-op TF kernel semantics, which are
 the shim's restatement of the TF documentation).
 
-Per case the file holds: the batch (features, labels), the state arrays fed to the placeholders, every variable by its
-TF name, the negatives the reference's sampler drew (the oracle takes them as an input: TF's shuffles are not
+Per case the file holds: the batch (features, labels), the state arrays fed to the placeholders, the mean / std of the
+reference's initializer and the shape of every variable (the graph runs with oracle/golden_sampling.preset_variable values), the negatives the reference's sampler drew (the oracle takes them as an input: TF's shuffles are not
 reproducible), the tensors the reference itself sends to tf.summary.histogram (plot_histograms=True), the scaled logits
 (input of the first tf.nn.softmax), total_loss, d(total_loss)/d(variable) for every variable, and the variables after
 the one AdamOptimizer step of the constructor.  EVAL cases hold predicted_item_ids / predicted_item_probs and the batch
-values of the recall@n / MRR@n streaming metrics.
+values of the recall@n / MRR@n streaming metrics.  Gradients, Adam deltas, TRAIN logits and the intermediates (first case
+only) are kept at a fixed seeded sample of their entries / rows (oracle/golden_sampling.sample_index): the file stays < 1 MB.
 
 Run once in the build container (python tests/golden/make_model_golden.py); the .npz is committed."""
 import importlib
@@ -45,6 +46,7 @@ import torch  # noqa: E402
 
 torch.set_num_threads(1)      # float32 scatter-add order (embedding gradients) would otherwise vary run to run at 1e-7
 from chameleon_recsys_b200.harness import make_problem, warm_state  # noqa: E402
+from oracle.golden_sampling import preset_variable, sample_index  # noqa: E402
 
 
 def build(pb, feats, labels, buf, pop, mode, float64, preset, seed, **over):
@@ -77,14 +79,17 @@ def build(pb, feats, labels, buf, pop, mode, float64, preset, seed, **over):
     return model
 
 
-THIN = 8
+GRAD_SAMPLE = 256        # entries kept per gradient / Adam delta
+LOGIT_SAMPLE = 512       # TRAIN logits kept (valid positions)
+HIST_ROWS = 48           # valid positions kept per intermediate
 
 
-def _thin(a, full):
-    return a if (full or a.size <= 20000) else np.ascontiguousarray(a.reshape(-1)[::THIN])
+def _sample(a, k):
+    a = np.asarray(a).reshape(-1)
+    return np.ascontiguousarray(a[sample_index(a.size, k)])
 
 
-def run_case(name, mode='train', float64=True, warm=5, seed=3, hp_over=None, steps_skip=0, keep_adam=False, full_grads=False, keep_hist=False,
+def run_case(name, mode='train', float64=True, warm=5, seed=3, hp_over=None, steps_skip=0, keep_adam=False, keep_hist=False,
              gru=False):
     # gru: the cell nar_model.py:1315 keeps commented out (north_star's "session GRU").  The reference file is not edited:
     # the stand-in hands out its GRUCell when the code asks for tf.contrib.rnn.UGRNNCell - the effect of un-commenting :1315
@@ -100,15 +105,11 @@ def run_case(name, mode='train', float64=True, warm=5, seed=3, hp_over=None, ste
     pop = pb.clicked_items_state.get_articles_recent_pop_norm().astype(np.float32)
     # pass 1: discover the variables (names, shapes, the reference's initializers)
     build(pb, feats, labels, buf, pop, mode, float64, None, seed)
-    rs = np.random.RandomState(11)
-    preset = {}
+    preset, stats = {}, {}
     for n, v in shim.S.vars.items():
         a = v.detach().numpy().astype(np.float64)
-        if n.endswith('bias') or n.endswith('beta_center'):
-            a = a + rs.normal(0, 0.1, a.shape)                # zero-initialised in TF: make them count
-        elif n.endswith('gamma_scale'):
-            a = a + rs.normal(0, 0.1, a.shape)
-        preset[n] = a.astype(np.float32)                      # float32 values, as a TF checkpoint would hold
+        stats[n] = np.array([a.mean(), a.std()])
+        preset[n] = preset_variable(n, a.shape, *stats[n])   # float32 values, as a TF checkpoint would hold
     # pass 2: same sampler seed (-> same negatives), preset variables
     model = build(pb, feats, labels, buf, pop, mode, float64, preset, seed)
     S = shim.S
@@ -120,31 +121,34 @@ def run_case(name, mode='train', float64=True, warm=5, seed=3, hp_over=None, ste
     out['buffer'] = buf
     out['pop_norm'] = pop
     for n, v in S.vars.items():
-        out['var/' + n] = v.detach().numpy().astype(np.float32)          # (float32-valued by construction)
-        assert np.array_equal(out['var/' + n].astype(np.float64), v.detach().numpy().astype(np.float64))
+        assert np.array_equal(preset[n].astype(np.float64), v.detach().numpy().astype(np.float64))
     out['reg_names'] = np.array(sorted(S.regs.keys()))
     out['var_names'] = np.array(list(S.vars.keys()))
+    # row i: variable var_names[i] - initializer mean / std, shape (rank <= 2; -1 pads a rank-1 shape)
+    out['var_stats'] = np.array([stats[n] for n in S.vars])
+    out['var_shapes'] = np.array([list(v.shape) + [-1] * (2 - len(v.shape)) for v in S.vars.values()], dtype=np.int64)
     out['negatives'] = model.batch_negative_items.numpy()
     out['total_loss'] = np.asarray(model.total_loss.detach().numpy())
-    out['logits_scaled'] = S.softmax_inputs[0].numpy()
     mask = (np.arange(feats['item_clicked'].shape[1])[None, :] < (np.asarray(feats['session_size']) - 1)[:, None])
+    if mode == 'train':
+        out['logits_sample'] = _sample(S.softmax_inputs[0].numpy()[mask], LOGIT_SAMPLE)
+    else:
+        out['logits_scaled'] = S.softmax_inputs[0].numpy()
     first = {}
     for hname, t in S.hist:
         first.setdefault(hname, t)
     for hname in (KEEP_HIST if keep_hist else []):            # valid positions only (the rest never reaches the loss)
         if hname in first and first[hname].shape[:2] == mask.shape:
-            out['hist/' + hname] = first[hname].numpy()[mask]
-    for sname, t in S.scalars:
-        out['scalar/' + sname] = np.asarray(t.numpy())
+            h = first[hname].numpy()[mask]
+            out['hist/' + hname] = np.ascontiguousarray(h[sample_index(h.shape[0], HIST_ROWS)])
     if mode == 'train':
         for n, g in S.grads.items():
             g = (g if g is not None else torch.zeros_like(S.vars[n])).detach().numpy()
-            # compared at 1e-6 of the largest gradient: float32 storage suffices.  Only the first case keeps the large
-            # tensors whole; the others keep every 8th element of them (file size)
-            out['grad/' + n] = _thin(g.astype(np.float32), full_grads)
+            # compared at 1e-6 of the largest gradient: float32 storage suffices
+            out['grad/' + n] = _sample(g.astype(np.float32), GRAD_SAMPLE)
         if keep_adam:
             for n, v in S.vars_after.items():
-                out['adam_delta/' + n] = _thin((v.numpy().astype(np.float64) - S.vars[n].detach().numpy().astype(np.float64)).astype(np.float32), False)
+                out['adam_delta/' + n] = _sample((v.numpy().astype(np.float64) - S.vars[n].detach().numpy().astype(np.float64)).astype(np.float32), GRAD_SAMPLE)
     else:
         out['predicted_item_ids'] = model.predicted_item_ids.numpy()
         out['predicted_item_probs'] = model.predicted_item_probs.detach().numpy()
@@ -177,23 +181,16 @@ KEEP_HIST = ['user_context_features', 'input_items_features', 'input_user_items_
 
 def main():
     cases = {}
-    cases.update(run_case('train64', keep_adam=True, full_grads=True, keep_hist=True))
+    cases.update(run_case('train64', keep_adam=True, keep_hist=True))
     cases.update(run_case('train32', float64=False))
-    cases.update(run_case('cold64', warm=0, keep_hist=True))                                   # empty buffer: tf.cond takes the batch statistics
+    cases.update(run_case('cold64', warm=0))                                   # empty buffer: tf.cond takes the batch statistics
     cases.update(run_case('nov64', hp_over=dict(novelty_reg_factor=0.3)))
     cases.update(run_case('layers2_64', hp_over=dict(rnn_num_layers=2)))
     # internal feature switches (nar_trainer_gcom.py:218-230): recency + ACR embeddings only
     cases.update(run_case('featoff64', hp_over=dict(enabled_internal_features=['recency', 'article_content_embeddings'])))
     cases.update(run_case('gru64', hp_over=dict(rnn_num_layers=2), gru=True))
     cases.update(run_case('drop64', hp_over=dict(dropout_keep_prob=0.8, rnn_num_layers=2)))
-    cases.update(run_case('eval64', mode='eval', steps_skip=1, keep_hist=True))
-    # the variables are the same in every single-layer case (same initializer seed): stored once
-    base = {k[len('train64/'):]: v for k, v in cases.items() if k.startswith('train64/var/')}
-    for k in list(cases):
-        c, rest = k.split('/', 1)
-        if c != 'train64' and rest in base and base[rest].shape == cases[k].shape and np.array_equal(base[rest], cases[k]):
-            del cases[k]
-            cases[c + '/same_vars_as'] = np.array('train64')
+    cases.update(run_case('eval64', mode='eval', steps_skip=1))
     path = os.path.join(HERE, 'model_golden.npz')
     np.savez_compressed(path, **cases)
     print('wrote %d arrays, %.1f KB' % (len(cases), os.path.getsize(path) / 1024))

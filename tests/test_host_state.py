@@ -280,13 +280,15 @@ def test_checkpoint_accepts_tf_variable_names(tmp_path):
     the reference model code, tests/golden/model_golden.npz) onto plan.ParamLayout's names."""
     from chameleon_recsys_b200 import checkpoint as ckpt
     d = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'model_golden.npz'))
-    tf_names = [k[len('train64/var/'):] for k in d.files if k.startswith('train64/var/')]
+    from oracle.golden_sampling import preset_variables
+    tf_names = [str(n) for n in d['train64/var_names']]
     pb = make_problem('tiny', profile='B')
     ours = set(pb.layout.init_logical(1).keys())
     assert set(ckpt.layout_name(n + ':0') for n in tf_names) == ours
     assert any(ckpt.layout_name(n) != n for n in tf_names)
     path = str(tmp_path / 'model.ckpt-7.npz')
-    np.savez(path, global_step=np.int64(7), **{'params/' + n: d['train64/var/' + n] for n in tf_names})
+    values = preset_variables(d, 'train64')
+    np.savez(path, global_step=np.int64(7), **{'params/' + n: values[n] for n in tf_names})
     ck = ckpt.load(path)
     assert set(ck['params'].keys()) == ours and ck['global_step'] == 7
 

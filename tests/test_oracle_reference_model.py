@@ -19,10 +19,10 @@ import pytest
 import torch
 
 from chameleon_recsys_b200.harness import make_problem
+from oracle.golden_sampling import preset_variables, sample_index
 from tools.gpu_step_check import make_oracle
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'model_golden.npz')
-THIN = 8            # make_model_golden.py keeps every 8th element of tensors > 20000 elements outside the first case
 
 
 @pytest.fixture(scope='module')
@@ -43,16 +43,18 @@ def _rel(a, b):
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-300))
 
 
+def _sampled(a, ref):
+    """`a` at the entries make_model_golden.py kept of the same tensor (`ref`: the stored sample)."""
+    a = np.asarray(a).reshape(-1)
+    return a[sample_index(a.size, np.asarray(ref).size)]
+
+
 def _load(d, case, hp_over, dtype):
     P = case + '/'
     pb = make_problem('tiny', profile='B', **hp_over)
     orc = make_oracle(pb, dtype)
-    tf_vars = {}
-    if (P + 'same_vars_as') in d.files:          # variables equal to the first case's are stored once (make_model_golden.py)
-        base = str(d[P + 'same_vars_as']) + '/'
-        tf_vars.update({k[len(base) + 4:]: d[k] for k in d.files if k.startswith(base + 'var/')})
-    tf_vars.update({k[len(P) + 4:]: d[k] for k in d.files if k.startswith(P + 'var/')})
-    tf_vars = {str(n): tf_vars[str(n)] for n in d[P + 'var_names']}      # the variables THIS case's graph created
+    # the variables THIS case's graph created, with the values the reference graph ran with
+    tf_vars = preset_variables(d, case)
     orc.set_params({_tf_name_to_layout(n): v for n, v in tf_vars.items()})
     assert set(_tf_name_to_layout(n) for n in tf_vars) == set(pb.layout.init_logical(1).keys())      # same variable set, same shapes
     for n, v in tf_vars.items():
@@ -82,7 +84,7 @@ def test_train_graph_matches_reference_code(golden, case, hp_over, dtype, tol):
     assert mask.sum() > 100
     # loss and (temperature-scaled) logits
     assert abs(float(o['total_loss'].detach()) - float(d[P + 'total_loss'])) / abs(float(d[P + 'total_loss'])) < tol
-    assert _rel(o['logits'].detach().numpy()[mask], d[P + 'logits_scaled'][mask]) < tol
+    assert _rel(_sampled(o['logits'].detach().numpy()[mask], d[P + 'logits_sample']), d[P + 'logits_sample']) < tol
     # which variables the reference regularises: Dense kernels, embeddings, gamma / beta - no bias, no RNN weight
     reg_ref = sorted(_tf_name_to_layout(str(n)) for n in d[P + 'reg_names'])
     assert reg_ref == sorted(n for n in orc.params if not (n.endswith('/bias') or '/RNN/' in n))
@@ -91,26 +93,26 @@ def test_train_graph_matches_reference_code(golden, case, hp_over, dtype, tol):
     # intermediates the reference exposes as histograms (valid positions)
     if (P + 'hist/input_user_items_features') in d.files:
         H = lambda n: d[P + 'hist/' + n]      # noqa: E731
-        assert _rel(o['x_in'].detach().numpy()[mask], H('input_user_items_features')) < tol      # (recency column: f32 division)
+        rows = sample_index(int(mask.sum()), H('input_user_items_features').shape[0])      # the valid positions kept
+        V = lambda t: t.detach().numpy()[mask][rows]      # noqa: E731
+        assert _rel(V(o['x_in']), H('input_user_items_features')) < tol      # (recency column: f32 division)
         n_ctx = H('user_context_features').shape[1]
         # x = concat(user context, item features) * gamma + beta   (nar_model.py:332-333, :997)
         g = tf_vars['main/user_items_contextual_features/input_features_center_scale/gamma_scale'].astype(np.float64)
         b = tf_vars['main/user_items_contextual_features/input_features_center_scale/beta_center'].astype(np.float64)
         cat_pos = np.concatenate([H('user_context_features'), H('positive_items_features')], axis=1)
         assert n_ctx + H('positive_items_features').shape[1] == g.shape[0]
-        assert _rel(o['x_pos'].detach().numpy()[mask], cat_pos * g + b) < tol
-        assert _rel(o['e_in'].detach().numpy()[mask], H('input_contextual_item_embedding')) < tol
-        assert _rel(o['e_pos'].detach().numpy()[mask], H('positive_contextual_item_embedding')) < tol
-        assert _rel(o['rnn_out'].detach().numpy()[mask], H('rnn/outputs')) < tol
-        assert _rel(o['pred'].detach().numpy()[mask], H('predicted_contextual_item_embedding')) < tol
+        assert _rel(V(o['x_pos']), cat_pos * g + b) < tol
+        assert _rel(V(o['e_in']), H('input_contextual_item_embedding')) < tol
+        assert _rel(V(o['e_pos']), H('positive_contextual_item_embedding')) < tol
+        assert _rel(V(o['rnn_out']), H('rnn/outputs')) < tol
+        assert _rel(V(o['pred']), H('predicted_contextual_item_embedding')) < tol
     # gradients of total_loss w.r.t. every variable (the last bias has an analytically zero gradient: absolute scale)
     grads = orc.compute_gradients(o)
     gmax = max(float(np.abs(d[k]).max()) for k in d.files if k.startswith(P + 'grad/'))
     for n_tf in tf_vars:
         g_ref = d[P + 'grad/' + n_tf]
-        g_orc = grads[_tf_name_to_layout(n_tf)].detach().numpy()
-        if g_ref.shape != g_orc.shape:
-            g_orc = g_orc.reshape(-1)[::THIN]
+        g_orc = _sampled(grads[_tf_name_to_layout(n_tf)].detach().numpy(), g_ref)
         assert float(np.abs(g_orc - g_ref).max()) < max(tol, 2e-7) * gmax * 10, n_tf
         if np.abs(g_ref).max() > 1e-6 * gmax:
             assert _rel(g_orc, g_ref) < max(tol * 50, 1e-5), n_tf
@@ -121,11 +123,9 @@ def test_train_graph_matches_reference_code(golden, case, hp_over, dtype, tol):
         after = orc.get_params()
         for n_tf in tf_vars:
             n = _tf_name_to_layout(n_tf)
-            delta = after[n].astype(np.float64) - before[n].astype(np.float64)
             ref = d[P + 'adam_delta/' + n_tf].astype(np.float64)
-            gr = d[P + 'grad/' + n_tf].astype(np.float64)
-            if ref.shape != delta.shape:                      # thinned in the golden file (the gradient of this case is whole)
-                delta, gr = delta.reshape(-1)[::THIN], gr.reshape(-1)[::THIN]
+            delta = _sampled(after[n].astype(np.float64) - before[n].astype(np.float64), ref)
+            gr = d[P + 'grad/' + n_tf].astype(np.float64)          # sampled at the same entries
             sel = np.abs(gr) > 1e-9 * gmax
             if not sel.any():                                 # matching_dense_layer_4/bias: the softmax is shift invariant
                 continue
@@ -206,14 +206,12 @@ def test_dropout_sites_match_reference_code(golden):
     o = orc.forward(f, lab, neg, buf, pop, train_step=1)
     mask = o['mask'].numpy().astype(bool)
     assert abs(float(o['total_loss'].detach()) - float(d[P + 'total_loss'])) / abs(float(d[P + 'total_loss'])) < 1e-7
-    assert _rel(o['logits'].detach().numpy()[mask], d[P + 'logits_scaled'][mask]) < 1e-7
+    assert _rel(_sampled(o['logits'].detach().numpy()[mask], d[P + 'logits_sample']), d[P + 'logits_sample']) < 1e-7
     grads = orc.compute_gradients(o)
     gmax = max(float(np.abs(d[k]).max()) for k in d.files if k.startswith(P + 'grad/'))
     for n_tf in tf_vars:
         g_ref = d[P + 'grad/' + n_tf]
-        g_orc = grads[_tf_name_to_layout(n_tf)].detach().numpy()
-        if g_ref.shape != g_orc.shape:
-            g_orc = g_orc.reshape(-1)[::THIN]
+        g_orc = _sampled(grads[_tf_name_to_layout(n_tf)].detach().numpy(), g_ref)
         assert float(np.abs(g_orc - g_ref).max()) < 2e-6 * gmax, n_tf
     # and without the masks the result differs (the check above is not vacuous)
     orc.mask_override = None

@@ -1,5 +1,5 @@
 """Stand-alone GEMM / gather micro-benchmark (CUDA events, L2 flush between iterations).
-   python tools/gemm_bench.py [quick]      -> prints one JSON line per shape; used under ncu for the captures in profiles/."""
+   python tools/gemm_bench.py [quick]      -> prints one JSON line per shape."""
 import json
 import os
 import sys
@@ -45,9 +45,9 @@ def main():
     Wtlo = torch.empty_like(Wt)
     ops.tf32_lo(Wt, Wt.numel(), Wtlo)
     Wplane = ops.pack_bf16x3(W, K, N)
-    only = os.environ.get('NAR_GEMM_BENCH_ONLY')           # substring filter (used for single-kernel ncu captures)
+    only = os.environ.get('NAR_GEMM_BENCH_ONLY')           # substring filter
     cases = [
-        ('fwd  bf16x3 A:K fp32 -> TMEM, B: packed bf16 plane', lambda: ops.gemm(X, None, Y, M, N, K, a_kmajor=True, b_kmajor=True, ldb=0, bias=bias, act=2, precision=4, b_bf16=Wplane, ld_bf16=Wplane.stride(0)), 2.0 * M * N * K),
+        ('fwd  bf16x3 A:K fp32 split in registers, B: packed bf16 plane', lambda: ops.gemm(X, None, Y, M, N, K, a_kmajor=True, b_kmajor=True, ldb=0, bias=bias, act=2, precision=4, b_bf16=Wplane, ld_bf16=Wplane.stride(0)), 2.0 * M * N * K),
         ('fwd  3x  A:K  B:K(W^T) +B_lo', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=3, b_lo=Wtlo), 2.0 * M * N * K),
         ('fwd  3x  A:K  B:K(W^T) in-kernel split', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=3), 2.0 * M * N * K),
         ('fwd  1x  A:K  B:K(W^T)', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=1), 2.0 * M * N * K),
