@@ -135,6 +135,11 @@ _SIGNATURES = {
     'nar_cosine_softmax_ce': (C.c_int, [vp, vp, i64, i64, i64, f32, f32, vp, vp, vp, vp, C.POINTER(NoveltyReg), vp]),
     'nar_dropout_rows': (C.c_int, [vp, vp, i64, i64, i64, vp, i64, i64, i64, C.c_int, f32, u64, u32, vp]),
     'nar_rank_candidates': (C.c_int, [vp, vp, i64, i64, i32, vp, vp, vp, vp]),
+    'nar_car_combine_grid': (C.c_int, [vp, vp, i64, i64, i64, C.c_int, vp, vp]),
+    'nar_topn_candidates': (C.c_int, [vp, vp, i64, i64, i32, vp, vp, i64, vp, vp, vp, vp]),
+    'nar_engine_recommend_workspace_bytes': (C.c_int, [vp, i64, i64, i64, i32, i64, C.POINTER(i64), C.POINTER(i64),
+                                                       C.POINTER(i64)]),
+    'nar_engine_recommend': (C.c_int, [vp, C.POINTER(StepIO), vp, vp, i64, vp, i64, i32, i32, i64, i64, vp, vp, vp, vp]),
     'nar_host_state_update': (C.c_int, [vp, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, C.c_double]),
     'nar_host_state_update_batch': (C.c_int, [vp, i64, vp, vp, vp, i64, i64, i64, vp, vp, vp, vp, vp, i64, C.c_double]),
     'nar_state_update': (C.c_int, [vp, vp, i64, vp, vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, i64, C.c_double, vp, vp]),

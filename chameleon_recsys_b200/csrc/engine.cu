@@ -23,6 +23,10 @@
 extern "C" int nar_sample_negatives_uidx(nar_ctx*, const int64_t*, int64_t, int64_t, int64_t, int64_t, const int64_t*, int64_t,
                                          int64_t, int64_t, uint64_t, uint32_t, int64_t*, int32_t*, const int64_t**,
                                          const int32_t**, void*, int64_t, void*);
+namespace nar {
+int recommend_rows(const int32_t* pos_idx, int64_t L, const int64_t* item_clicked, const int64_t* cand_ids, int64_t N,
+                   int32_t* row_pos, int64_t* row_item, cudaStream_t st);        // csrc/recommend.cu
+}
 
 namespace {
 
@@ -226,6 +230,40 @@ struct Seq {
   }
 };
 
+// CAR (nar_model.py:374-405) of the L clicked rows sb.X[0:L] on the main stream, then the session branch - RNN (:408,
+// :1308-1342) + FC1 / FC2 (:410-438) -> sb.PR - forked onto the auxiliary stream, so that it runs under whatever the
+// caller queues next on main (the candidate rows); the caller joins before reading sb.PR.  (Moving the two CAR GEMMs
+// into the session branch as well was measured neutral and is not used: DESIGN.md section 6.)
+// dropout(src, dst, rows, cols, row_pos, tensor_id, stream) is only called when `drop` is set.
+template <class Dropout>
+void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop, Dropout&& dropout) {
+  const nar_model_cfg& c = s.c;
+  const nar_step_io* io = s.io;
+  const int64_t B = io->B, C = c.C, Hp = c.Hp, Fp = c.Fp;
+  s.fwd(sb.X, Fp, c.off_W1, C, c.off_b1, sb.H1, C, L, C, Fp, NAR_ACT_LEAKY_RELU, s.main);
+  s.fwd(sb.H1, C, c.off_W2, C, c.off_b2, sb.E, C, L, C, C, NAR_ACT_TANH, s.main);
+  cudaStream_t st = s.fork();
+  const float* rnn_in = sb.E; int64_t n_in = C;
+  for (int i = 0; i < c.layers; ++i) {
+    if (c.rnn_cell == 1) {
+      // GRUCell: gx = (x Wxg + bg | x Wxc + bc), then the recurrence (csrc/gru.cu)
+      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 3 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
+      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wxc[i], Hp, c.off_bc[i], sb.GX[i] + 2 * Hp, 3 * Hp, L, Hp, n_in, NAR_ACT_NONE, st);
+      s.chk(nar_gru_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), s.W(c.off_Whc[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.UO[i],
+                        sb.CD[i], sb.RH[i], st));
+    } else {
+      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 2 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
+      s.chk(nar_ugrnn_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.CD[i], st));
+    }
+    // DropoutWrapper(output_keep_prob) (nar_model.py:1330-1333): the cell's OUTPUT is dropped, its state is not
+    if (drop) dropout(sb.HO[i], sb.HOd[i], L, Hp, io->pos_idx, 8 + i, st);
+    rnn_in = drop ? sb.HOd[i] : sb.HO[i]; n_in = Hp;
+  }
+  s.fwd(rnn_in, Hp, c.off_W3, 512, c.off_b3, sb.F1, 512, L, 512, Hp, NAR_ACT_LEAKY_RELU, st);
+  if (drop) dropout(sb.F1, sb.F1, L, 512, io->pos_idx, 4, st);                                  // nar_model.py:417-419
+  s.fwd(sb.F1, 512, c.off_W4, C, c.off_b4, sb.PR, C, L, C, 512, NAR_ACT_TANH, st);
+}
+
 int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   const nar_model_cfg& c = e->cfg;
   const int64_t B = io->B, T = io->T, L = io->L, K = c.K, n_cand = K + 1, Rc = L * n_cand, R = L + Rc;
@@ -269,35 +307,8 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   s.chk(nar_gather_features(e->ctx, &plan, g_pos, g_item, &rl, io->event_ts, io->max_ts, sb.X, main));
   if (drop) dropout(sb.X, sb.X, R, Fp, pb.row_pos, 0, main);          // nar_model.py:338-340, :351-353, :367-369
 
-  // ---- session branch: RNN (nar_model.py:408, :1308-1342) + FC1 / FC2 (:410-438) on the L clicked rows
-  auto session_branch = [&](cudaStream_t st) {
-    const float* rnn_in = sb.E; int64_t n_in = C;
-    for (int i = 0; i < c.layers; ++i) {
-      if (c.rnn_cell == 1) {
-        // GRUCell: gx = (x Wxg + bg | x Wxc + bc), then the recurrence (csrc/gru.cu)
-        s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 3 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
-        s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wxc[i], Hp, c.off_bc[i], sb.GX[i] + 2 * Hp, 3 * Hp, L, Hp, n_in, NAR_ACT_NONE, st);
-        s.chk(nar_gru_fwd(e->ctx, sb.GX[i], s.W(c.off_Wh[i]), s.W(c.off_Whc[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.UO[i],
-                          sb.CD[i], sb.RH[i], st));
-      } else {
-      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 2 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
-      s.chk(nar_ugrnn_fwd(e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.CD[i], st));
-      }
-      // DropoutWrapper(output_keep_prob) (nar_model.py:1330-1333): the cell's OUTPUT is dropped, its state is not
-      if (drop) dropout(sb.HO[i], sb.HOd[i], L, Hp, io->pos_idx, 8 + i, st);
-      rnn_in = drop ? sb.HOd[i] : sb.HO[i]; n_in = Hp;
-    }
-    s.fwd(rnn_in, Hp, c.off_W3, 512, c.off_b3, sb.F1, 512, L, 512, Hp, NAR_ACT_LEAKY_RELU, st);
-    if (drop) dropout(sb.F1, sb.F1, L, 512, io->pos_idx, 4, st);                                  // nar_model.py:417-419
-    s.fwd(sb.F1, 512, c.off_W4, C, c.off_b4, sb.PR, C, L, C, 512, NAR_ACT_TANH, st);
-  };
-
-  // ---- CAR (nar_model.py:374-405): the clicked rows first, so that the session branch can run under the candidates
-  // (moving these two GEMMs into the session branch as well was measured neutral and is not used: DESIGN.md section 6)
   float* H1c = sb.H1 + L * C; float* Ec = sb.E + L * C;
-  s.fwd(sb.X, Fp, c.off_W1, C, c.off_b1, sb.H1, C, L, C, Fp, NAR_ACT_LEAKY_RELU, main);
-  s.fwd(sb.H1, C, c.off_W2, C, c.off_b2, sb.E, C, L, C, C, NAR_ACT_TANH, main);
-  { cudaStream_t st = s.fork(); session_branch(st); }
+  clicked_rows_forward(s, sb, L, drop, dropout);
   if (c.dedup) {
     s.fwd(sb.X + L * Fp, Fp, c.off_W1, C, c.off_b1, sb.PP, C, L, C, Fp, NAR_ACT_NONE, main);                       // positives: full rows
     s.fwd(sb.X + 2 * L * Fp, Fp, c.off_W1, C, -1, sb.PI, C, U, C, c0, NAR_ACT_NONE, main);                          // item half, once per unique id
@@ -435,6 +446,144 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   s.chk(nar_gather_features_bwd(e->ctx, &plan, g_pos, g_item, &rl, io->event_ts, io->max_ts, sb.dX, s.G(c.off_gamma),
                                 s.G(c.off_beta), main));
   s.join();
+  return s.rc;
+}
+
+// ---------------------------------------------------------------------------------------------- recommend
+// Workspace of one recommend call: L clicked rows, Q queries, N candidates, processed in blocks of qb queries x nb
+// candidates.  The session part reuses the StepBufs fields clicked_rows_forward reads and writes.
+struct RecBufs {
+  StepBufs sb;
+  int32_t* row_pos; int64_t* row_item;
+  float *stats, *PC, *PCq, *PRq, *logits, *lg_chunk, *PI, *H1g, *Eg, *Z1, *Z2, *Z3, *loss;
+};
+
+int64_t rec_carve(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int64_t qb, int64_t nb, int gather_q, void* base,
+                  RecBufs* rb) {
+  const nar_model_cfg& c = e->cfg;
+  const int64_t C = c.C, Hp = c.Hp, Fp = c.Fp, gw = c.rnn_cell == 1 ? 3 : 2, P = qb * nb;
+  memset(rb, 0, sizeof(*rb));
+  StepBufs& sb = rb->sb;
+  Carver cv(base);
+  rb->row_pos = cv.take<int32_t>(L + N);
+  rb->row_item = cv.take<int64_t>(L + N);
+  rb->stats = cv.take<float>(24);
+  rb->loss = cv.take<float>(4);
+  sb.X = cv.take<float>((L + N) * Fp);
+  sb.H1 = cv.take<float>(L * C);
+  sb.E = cv.take<float>(L * C);
+  for (int i = 0; i < c.layers; ++i) {
+    sb.GX[i] = cv.take<float>(L * gw * Hp); sb.HO[i] = cv.take<float>(L * Hp);
+    sb.GT[i] = cv.take<float>(L * Hp); sb.CD[i] = cv.take<float>(L * Hp);
+    if (c.rnn_cell == 1) { sb.UO[i] = cv.take<float>(L * Hp); sb.RH[i] = cv.take<float>(L * Hp); }
+  }
+  sb.F1 = cv.take<float>(L * 512);
+  sb.PR = cv.take<float>(L * C);
+  rb->PC = cv.take<float>(L * C);
+  rb->PCq = gather_q ? cv.take<float>(Q * C) : rb->PC;
+  rb->PRq = gather_q ? cv.take<float>(Q * C) : sb.PR;
+  rb->logits = cv.take<float>(qb * N);
+  rb->lg_chunk = nb < N ? cv.take<float>(P) : rb->logits;
+  rb->PI = cv.take<float>(nb * C);
+  rb->H1g = cv.take<float>(P * C);                 // layer-1 activations, then the product with PR (MLP scorer)
+  rb->Eg = cv.take<float>(P * C);
+  if (c.ranking == 0) { rb->Z1 = cv.take<float>(P * 128); rb->Z2 = cv.take<float>(P * 64); rb->Z3 = cv.take<float>(P * 32); }
+  return cv.off;
+}
+
+// largest candidate chunk the cosine scorer takes (its shared memory holds the prediction row + 3 floats per candidate)
+int64_t cosine_chunk_cap(const nar_model_cfg& c) { return (48 * 1024 / 4 - c.C) / 3; }
+
+// Blocks within `budget` bytes: as many queries as fit with at most half the budget in the [qb, N] logits, then as many
+// candidates per chunk as the rest allows.  Returns the workspace size, or -1 when not even one query x one candidate fits.
+int64_t rec_plan(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int gather_q, int64_t budget, int64_t* qb_out,
+                 int64_t* nb_out) {
+  const nar_model_cfg& c = e->cfg;
+  RecBufs rb;
+  const int64_t fixed = rec_carve(e, L, Q, N, 0, 0, gather_q, nullptr, &rb);
+  if (fixed >= budget) return -1;
+  int64_t qb = (budget - fixed) / 2 / (N * 4);
+  qb = qb > Q ? Q : (qb < 1 ? 1 : qb);
+  const int64_t nb_cap = (c.ranking == 1 && cosine_chunk_cap(c) < N) ? cosine_chunk_cap(c) : N;
+  for (;;) {
+    // bytes per candidate of a chunk: its PI row, qb pairs of activations, qb chunk logits
+    const int64_t per = 4 * (c.C + qb * (2 * c.C + (c.ranking == 0 ? 128 + 64 + 32 : 0) + 1));
+    const int64_t avail = budget - rec_carve(e, L, Q, N, qb, 0, gather_q, nullptr, &rb) - 8 * 256;   // carve alignment
+    int64_t nb = avail > 0 ? avail / per : 0;
+    nb = nb > nb_cap ? nb_cap : nb;
+    while (nb >= 1 && rec_carve(e, L, Q, N, qb, nb, gather_q, nullptr, &rb) > budget) nb -= nb / 64 + 1;
+    if (nb >= 1) { *qb_out = qb; *nb_out = nb; return rec_carve(e, L, Q, N, qb, nb, gather_q, nullptr, &rb); }
+    if (qb == 1) return -1;
+    qb = (qb + 1) / 2;
+  }
+}
+
+int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, const int32_t* q_pos, int64_t Q,
+                  const int64_t* cand_ids, int64_t N, int32_t top_n, int32_t exclude, int64_t qb, int64_t nb, int64_t* out_ids,
+                  float* out_scores, float* out_probs, cudaStream_t main) {
+  const nar_model_cfg& c = e->cfg;
+  const int64_t L = io->L, T = io->T, C = c.C, Fp = c.Fp, c0 = c.ctx_col0;
+  if (L <= 0 || Q <= 0 || Q > L || N <= 0 || qb < 1 || nb < 1 || (c.ranking == 1 && nb > cosine_chunk_cap(c))) return NAR_ERR_INVALID;
+  if (top_n < 1 || top_n > N || top_n > 4096) return NAR_ERR_INVALID;
+  if (qb > Q) qb = Q;
+  if (nb > N) nb = N;
+  const int gather_q = q_rows != nullptr;
+  RecBufs rb;
+  if (rec_carve(e, L, Q, N, qb, nb, gather_q, io->ws, &rb) > io->ws_bytes) return NAR_ERR_WORKSPACE;
+  StepBufs& sb = rb.sb;
+  Seq s(e, io, main);
+
+  // ---- rows, statistics (empty buffer: the candidate rows are group 2, like the negatives), one gather
+  s.chk(nar::recommend_rows(io->pos_idx, L, io->item_clicked, cand_ids, N, rb.row_pos, rb.row_item, main));
+  s.chk(nar_feature_stats(e->ctx, io->buffer, c.buf_len, c.n_norm, c.plan.created_at_ts, io->pop_norm, io->max_ts,
+                          c.plan.log_base_recency, c.plan.log_base_novelty, rb.row_pos, rb.row_item, L + N, L, 0, io->event_ts,
+                          rb.stats, main));
+  nar_feature_plan plan = c.plan;
+  for (int i = 0; i < NAR_MAX_SRC; ++i) { plan.ctx_int[i] = io->ctx_int[i]; plan.ctx_float[i] = io->ctx_float[i]; }
+  plan.pop_norm = io->pop_norm;
+  plan.stats = rb.stats;
+  nar_row_layout rl;
+  rl.n_rows = L + N; rl.n_input = L; rl.n_cand = 0; rl.n_positive = 0; rl.n_full = L; rl.ctx_col0 = c0;
+  s.chk(nar_gather_features(e->ctx, &plan, rb.row_pos, rb.row_item, &rl, io->event_ts, io->max_ts, sb.X, main));
+  if (s.rc) return s.rc;
+
+  // ---- clicked rows + session branch (aux), the context half of layer 1 per position (main)
+  clicked_rows_forward(s, sb, L, false, [](const float*, float*, int64_t, int64_t, const int32_t*, int, cudaStream_t) {});
+  s.fwd(sb.X + c0, Fp, c.off_W1 + c0 * C, C, c.off_b1, rb.PC, C, L, C, Fp - c0, NAR_ACT_NONE, main);
+  s.join();
+  if (gather_q) {
+    s.chk(nar_gather_rows_f32(rb.PC, L, C, (int)C, q_rows, Q, rb.PCq, C, main));
+    s.chk(nar_gather_rows_f32(sb.PR, L, C, (int)C, q_rows, Q, rb.PRq, C, main));
+  }
+
+  // ---- per block of queries: every candidate chunk into logits [qb, N], then the top n of each query
+  for (int64_t q0 = 0; q0 < Q && !s.rc; q0 += qb) {
+    const int64_t Qb = Q - q0 < qb ? Q - q0 : qb;
+    const float* pcq = rb.PCq + q0 * C; const float* prq = rb.PRq + q0 * C;
+    for (int64_t j0 = 0; j0 < N && !s.rc; j0 += nb) {
+      const int64_t Nc = N - j0 < nb ? N - j0 : nb, P = Qb * Nc;
+      s.fwd(sb.X + (L + j0) * Fp, Fp, c.off_W1, C, -1, rb.PI, C, Nc, C, c0, NAR_ACT_NONE, main);     // item half, per candidate
+      s.chk(nar_car_combine_grid(pcq, rb.PI, Qb, Nc, C, NAR_ACT_LEAKY_RELU, rb.H1g, main));
+      s.fwd(rb.H1g, C, c.off_W2, C, c.off_b2, rb.Eg, C, P, C, C, NAR_ACT_TANH, main);
+      float* lg = Nc == N ? rb.logits : rb.lg_chunk;
+      if (c.ranking == 0) {
+        s.chk(nar_mul_pred(rb.Eg, prq, Qb, Nc, C, rb.H1g, main));
+        s.fwd(rb.H1g, C, c.off_M[0], c.ld_M[0], c.off_c[0], rb.Z1, 128, P, 128, C, NAR_ACT_LEAKY_RELU, main);
+        s.fwd(rb.Z1, 128, c.off_M[1], c.ld_M[1], c.off_c[1], rb.Z2, 64, P, 64, 128, NAR_ACT_LEAKY_RELU, main);
+        s.fwd(rb.Z2, 64, c.off_M[2], c.ld_M[2], c.off_c[2], rb.Z3, 32, P, 32, 64, NAR_ACT_LEAKY_RELU, main);
+        s.chk(nar_score_softmax_ce(rb.Z3, 32, 32, s.W(c.off_M[3]), c.ld_M[3], s.W(c.off_c[3]), Qb, Nc, c.inv_temperature, 0.f, lg,
+                                   rb.loss, nullptr, nullptr, nullptr, nullptr, main));
+      } else {
+        s.chk(nar_cosine_softmax_ce(rb.Eg, prq, Qb, Nc, C, c.inv_temperature, 0.f, lg, rb.loss, nullptr, nullptr, nullptr, main));
+      }
+      if (Nc != N)
+        s.chk((int)cudaMemcpy2DAsync(rb.logits + j0, (size_t)N * sizeof(float), lg, (size_t)Nc * sizeof(float),
+                                     (size_t)Nc * sizeof(float), (size_t)Qb, cudaMemcpyDeviceToDevice, main));
+    }
+    s.chk(nar_topn_candidates(rb.logits, cand_ids, Qb, N, top_n, exclude ? io->item_clicked : nullptr, q_pos + q0, T,
+                              out_ids + q0 * top_n, out_scores ? out_scores + q0 * top_n : nullptr,
+                              out_probs ? out_probs + q0 * top_n : nullptr, main));
+  }
   return s.rc;
 }
 
@@ -586,6 +735,25 @@ extern "C" int nar_engine_apply(nar_engine* e, const nar_step_io* io, void* stre
                        io->global_step + 1, c.params_lo, stream);
   if (rc == NAR_OK && c.fwd_precision == 4) rc = planes_refresh(e, as_stream(stream));
   return rc;
+}
+
+extern "C" int nar_engine_recommend_workspace_bytes(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int32_t gather_q,
+                                                    int64_t budget_bytes, int64_t* ws_bytes, int64_t* q_block, int64_t* n_block) {
+  if (!e || !ws_bytes || !q_block || !n_block || L <= 0 || Q <= 0 || Q > L || N <= 0) return NAR_ERR_INVALID;
+  const int64_t b = rec_plan(e, L, Q, N, gather_q != 0, budget_bytes, q_block, n_block);
+  if (b < 0) return NAR_ERR_WORKSPACE;
+  *ws_bytes = b;
+  return NAR_OK;
+}
+
+extern "C" int nar_engine_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, const int32_t* q_pos, int64_t Q,
+                                    const int64_t* cand_ids, int64_t N, int32_t top_n, int32_t exclude_session_clicks,
+                                    int64_t q_block, int64_t n_block, int64_t* out_ids, float* out_scores, float* out_probs,
+                                    void* stream) {
+  if (!e || !io || !io->ws || !q_pos || !cand_ids || !out_ids || !io->buffer || !io->pop_norm || !io->item_clicked) return NAR_ERR_INVALID;
+  if (io->train) return NAR_ERR_INVALID;
+  return run_recommend(e, io, q_rows, q_pos, Q, cand_ids, N, top_n, exclude_session_clicks, q_block, n_block, out_ids, out_scores,
+                       out_probs, as_stream(stream));
 }
 
 extern "C" int64_t nar_engine_launch_count(const nar_engine* e) { return e ? e->launches : 0; }

@@ -679,6 +679,111 @@ class NarEngine:
         out['stage'] = st
         return out
 
+    # ---- recommendation (ModeKeys.PREDICT): score a candidate set for query positions, keep the top n
+    MAX_TOP_N = 4096
+
+    def resolve_candidates(self, candidates, buffer) -> np.ndarray:
+        """``None``: the sorted distinct nonzero ids of the recent-clicks buffer (the pool training negatives come from);
+        ``'catalog'``: every id 1 .. V-1; otherwise an int array of distinct ids in [1, V).  Raises ValueError."""
+        if candidates is None:
+            b = np.asarray(buffer, dtype=np.int64).reshape(-1)
+            return np.unique(b[b != 0])
+        if isinstance(candidates, str):
+            if candidates != 'catalog':
+                raise ValueError("candidates must be None, 'catalog' or an array of article ids, not %r" % candidates)
+            return np.arange(1, self.V, dtype=np.int64)
+        c = np.asarray(candidates)
+        if c.ndim != 1 or c.size == 0 or not np.issubdtype(c.dtype, np.integer):
+            raise ValueError('candidates must be a non-empty 1-D integer array of article ids')
+        c = c.astype(np.int64)
+        if c.min() < 1 or c.max() >= self.V:
+            raise ValueError('candidate ids must be in [1, %d)' % self.V)
+        if np.unique(c).size != c.size:
+            raise ValueError('candidate ids must be distinct')
+        return c
+
+    def recommend(self, features, buffer, pop_norm, top_n: int, candidates=None, positions: str = 'last',
+                  exclude_session_clicks: bool = True, ws_budget: Optional[int] = None) -> dict:
+        """Top-``top_n`` next articles out of ``candidates`` (see resolve_candidates) for the valid positions t <
+        session_size - 1 of the batch ``features`` (``positions='last'``: one query per session at its last valid
+        position; ``'all'``: every valid position, session-major).  A candidate is scored like a sampled negative of the
+        query position (nar_model.py:356-364, :374-405, :444-515); ``exclude_session_clicks`` never returns the query's own
+        clicks item_clicked[b, 0..t].  Reads the weights and the given state only (one C call, csrc/engine.cu).
+        ``ws_budget``: workspace bytes (default: the engine's budget); smaller budgets run more, smaller blocks with
+        bit-identical results.  -> numpy dict: query_session [Q], query_position [Q], predicted_item_ids /
+        predicted_item_scores / predicted_item_probs [Q, top_n], candidates [N]."""
+        if self.world > 1:
+            raise NotImplementedError('recommend runs on one process; data-parallel prediction is not implemented')
+        if positions not in ('last', 'all'):
+            raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
+        if buffer is None or pop_norm is None:
+            raise ValueError('recommend needs the host recent-clicks buffer and popularity')
+        cand = self.resolve_candidates(candidates, buffer)
+        N = int(cand.size)
+        if isinstance(top_n, (bool, np.bool_)) or not isinstance(top_n, (int, np.integer)):
+            raise ValueError('top_n must be an integer')
+        top_n = int(top_n)
+        if not 1 <= top_n <= min(N, self.MAX_TOP_N):
+            raise ValueError('top_n=%d outside [1, min(N=%d, %d)]' % (top_n, N, self.MAX_TOP_N))
+        item_clicked = np.asarray(features['item_clicked'])
+        Bg, T = item_clicked.shape
+        labels = {'label_next_item': np.zeros((Bg, T), dtype=np.int64), 'label_last_item': np.zeros(Bg, dtype=np.int64)}
+        st = self.stage(features, labels, buffer, pop_norm, slot='predict')
+        L, lens = st['L'], st['lens']
+        ends = np.cumsum(lens)
+        if positions == 'last':
+            q_rows = (ends - 1)[lens > 0].astype(np.int64)
+            q_sess = np.flatnonzero(lens > 0).astype(np.int64)
+            q_t = (lens[lens > 0] - 1).astype(np.int64)
+        else:
+            q_rows = np.arange(L, dtype=np.int64)
+            q_sess = np.repeat(np.arange(Bg, dtype=np.int64), lens)
+            q_t = np.arange(L, dtype=np.int64) - np.repeat(ends - lens, lens)
+        Q = int(q_rows.size)
+        out = {'query_session': q_sess, 'query_position': q_t, 'candidates': cand,
+               'predicted_item_ids': np.zeros((Q, top_n), np.int64), 'predicted_item_scores': np.zeros((Q, top_n), np.float32),
+               'predicted_item_probs': np.zeros((Q, top_n), np.float32)}
+        if Q == 0:
+            return out
+        gather_q = positions == 'last'
+        budget = int(self._ws_budget if ws_budget is None else ws_budget)
+        wb, qb, nb = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        check(self._lib.nar_engine_recommend_workspace_bytes(self._handle, L, Q, N, int(gather_q), budget, C.byref(wb),
+                                                             C.byref(qb), C.byref(nb)), 'nar_engine_recommend_workspace_bytes')
+        self._sync_cfg()
+        d = self.dev
+        ws = self._buf('rec_ws', int(wb.value), 1, torch.uint8).view(-1)
+        q_pos = torch.from_numpy(q_sess * T + q_t).to(torch.int32).to(d)
+        q_rows_t = torch.from_numpy(q_rows).to(d) if gather_q else None
+        cand_t = torch.from_numpy(cand).to(d)
+        ids = torch.empty(Q, top_n, dtype=torch.int64, device=d)
+        scores = torch.empty(Q, top_n, dtype=torch.float32, device=d)
+        probs = torch.empty(Q, top_n, dtype=torch.float32, device=d)
+        t = st['t']
+        io = StepIO()
+        io.B, io.Bg, io.T, io.sess0, io.L, io.L_global, io.L_cap = st['B'], Bg, T, st['s0'], L, st['L_global'], L
+        io.global_step, io.train = self.global_step, 0
+        io.all_items, io.event_ts = t['all_items'].data_ptr(), t['event_ts'].data_ptr()
+        io.item_clicked, io.label_next = t['item_clicked'].data_ptr(), t['label_next'].data_ptr()
+        io.buffer, io.max_ts, io.pop_norm = t['buffer'].data_ptr(), t['max_ts'].data_ptr(), t['pop_norm'].data_ptr()
+        for i, n in enumerate(self.plan.ctx_int_names):
+            io.ctx_int[i] = t['ci/' + n].data_ptr()
+        for i, n in enumerate(self.plan.ctx_float_names):
+            io.ctx_float[i] = t['cf/' + n].data_ptr()
+        io.pos_idx, io.sess_off = t['pos_idx'].data_ptr(), t['sess_off'].data_ptr()
+        io.ws, io.ws_bytes = ws.data_ptr(), ws.numel()
+        cur = torch.cuda.current_stream()
+        check(self._lib.nar_engine_recommend(self._handle, C.byref(io), C.c_void_p(0 if q_rows_t is None else q_rows_t.data_ptr()),
+                                             C.c_void_p(q_pos.data_ptr()), Q, C.c_void_p(cand_t.data_ptr()), N, top_n,
+                                             int(bool(exclude_session_clicks)), int(qb.value), int(nb.value),
+                                             C.c_void_p(ids.data_ptr()), C.c_void_p(scores.data_ptr()),
+                                             C.c_void_p(probs.data_ptr()), C.c_void_p(cur.cuda_stream)), 'nar_engine_recommend')
+        out['predicted_item_ids'] = ids.cpu().numpy()
+        out['predicted_item_scores'] = scores.cpu().numpy()
+        out['predicted_item_probs'] = probs.cpu().numpy()
+        out['q_block'], out['n_block'] = int(qb.value), int(nb.value)
+        return out
+
     def train_step(self, features, labels, buffer, pop_norm, keep: bool = False, sync: bool = True) -> dict:
         st = self.stage(features, labels, buffer, pop_norm)
         out = self.step(st, train=True, keep=keep)

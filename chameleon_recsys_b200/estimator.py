@@ -39,13 +39,14 @@ class EstimatorSpec:
     eval_metric_ops: Optional[dict] = None
     evaluation_hooks: List = field(default_factory=list)
     model: Optional[NARModuleModel] = None
+    predictions: Optional[Callable] = None          # PREDICT: predictions(features, feed, top_n, candidates, ...) -> dict
 
 
 def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
     if mode == ModeKeys.TRAIN:
         negative_samples = params['train_total_negative_samples']
         negative_sample_from_buffer = params['train_negative_samples_from_buffer']
-    elif mode == ModeKeys.EVAL:
+    elif mode in (ModeKeys.EVAL, ModeKeys.PREDICT):
         negative_samples = params['eval_total_negative_samples']
         negative_sample_from_buffer = params['eval_negative_samples_from_buffer']
     else:
@@ -96,6 +97,12 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
         def train_op(feats, labs, feed, sync=True):
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
         return EstimatorSpec(mode, loss=None, train_op=train_op, training_chief_hooks=hooks, model=model)
+    if mode == ModeKeys.PREDICT:
+        # one call per batch: the state arrays are read, never updated (no hook runs in PREDICT)
+        def predict(feats, feed, top_n=None, candidates=None, positions='last', exclude_session_clicks=True):
+            return model.recommend(feats, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], top_n=top_n,
+                                   candidates=candidates, positions=positions, exclude_session_clicks=exclude_session_clicks)
+        return EstimatorSpec(mode, loss=None, predictions=predict, model=model)
 
     # ModeKeys.EVAL (nar_trainer_gcom.py:323-332): loss + eval_metric_ops {hitrate_at_n, mrr_at_n}; each "update op" is
     # one call of model.evaluate, the values are read from the device accumulator at the end
@@ -236,6 +243,72 @@ class Estimator:
                 self.save_checkpoint()
         return self
 
+    def _use_trained_weights(self, spec: EstimatorSpec, what: str):
+        """Point the EVAL / PREDICT graph ``spec`` at the trained weights: the training graph's own (shared, no copy) when
+        this Estimator has trained, else the latest checkpoint in model_dir - what tf.estimator.Estimator restores
+        (nar_trainer_gcom.py:523).  Without either it raises: never serve randomly initialised weights."""
+        if self._spec is not None:
+            spec.model.engine.share_params(self._spec.model.engine)        # "restore the latest checkpoint"
+            return
+        latest = ckpt.latest_checkpoint(self.model_dir)
+        if latest is None:
+            raise ValueError('Estimator.%s: no trained model - call train() first or point model_dir at a '
+                             'directory holding a checkpoint (model_dir=%r)' % (what, self.model_dir))
+        restored = getattr(self, '_restored', {})
+        if restored.get(id(spec)) != latest:
+            ckpt.restore(latest, spec.model.engine, None)                   # weights + step; the state is not touched
+            restored[id(spec)] = latest
+            self._restored = restored
+
+    def predict(self, input_fn, steps: Optional[int] = None, top_n: Optional[int] = None, candidates=None,
+                exclude_session_clicks: bool = True, positions: str = 'last'):
+        """tf.estimator.Estimator.predict: a generator over the batches of ``input_fn`` that yields one dict per session -
+        ``session_id``, ``predicted_item_ids`` / ``predicted_item_scores`` / ``predicted_item_probs`` [top_n] (arrays
+        [n_positions, top_n] with ``positions='all'``).  The recommendation is for the article after the session's last
+        valid position (``label_last_item`` on an input_fn batch).  ``top_n`` defaults to eval_metrics_top_n;
+        ``candidates``: None = the distinct ids of the current recent-clicks buffer, 'catalog' = every article, or an array
+        of ids.  Weights as ``evaluate`` gets them; ClickedItemsState, weights, Adam slots and global_step are only read."""
+        import torch
+        if positions not in ('last', 'all'):
+            raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
+        it = input_fn()
+
+        def fetch():
+            try:
+                return it.get_next() if hasattr(it, 'get_next') else next(it)
+            except (OutOfRangeError, StopIteration):
+                return None
+
+        n = 0
+        nxt = fetch() if (steps is None or steps > 0) else None
+        while nxt is not None:
+            features, labels = nxt
+            if getattr(self, '_predict_spec', None) is None:
+                self._predict_spec = self.model_fn(features, labels, ModeKeys.PREDICT, self.params)
+            spec = self._predict_spec
+            if spec.model.engine.world > 1:
+                raise NotImplementedError('Estimator.predict runs on one process; data-parallel prediction is not implemented')
+            if n == 0:
+                self._use_trained_weights(spec, 'predict')
+            state = self._state()
+            feed = {'pop_recent_items_buffer': state.get_recent_clicks_buffer(),
+                    'articles_recent_pop_norm': state.get_articles_recent_pop_norm()}
+            out = spec.predictions(features, feed, top_n=top_n, candidates=candidates, positions=positions,
+                                   exclude_session_clicks=exclude_session_clicks)
+            sids = features.get('session_id')
+            Bg = np.asarray(features['item_clicked']).shape[0]
+            qs = out['query_session']
+            for b in range(Bg):
+                rows = np.flatnonzero(qs == b)
+                sel = rows[0] if (positions == 'last' and rows.size) else rows
+                yield {'session_id': None if sids is None else np.asarray(sids)[b],
+                       'predicted_item_ids': out['predicted_item_ids'][sel],
+                       'predicted_item_scores': out['predicted_item_scores'][sel],
+                       'predicted_item_probs': out['predicted_item_probs'][sel]}
+            n += 1
+            nxt = fetch() if (steps is None or n < steps) else None
+        torch.cuda.synchronize()
+
     def evaluate(self, input_fn, steps: Optional[int] = None, hooks=None, name=None) -> dict:
         """tf.estimator.Estimator.evaluate: runs the EVAL graph over ``input_fn`` with the current weights and returns
         ``{'loss', 'hitrate_at_n', 'mrr_at_n', 'global_step'}`` (streaming means over all valid labels, nar_model.py:
@@ -257,18 +330,7 @@ class Estimator:
         if self._eval_spec is None:
             self._eval_spec = self.model_fn(nxt[0], nxt[1], ModeKeys.EVAL, self.params)
         spec = self._eval_spec
-        if self._spec is not None:
-            spec.model.engine.share_params(self._spec.model.engine)        # "restore the latest checkpoint"
-        else:
-            # fresh Estimator over an existing model_dir: tf.estimator.Estimator.evaluate restores the latest checkpoint
-            # (nar_trainer_gcom.py:523) and fails when there is none - never evaluate randomly initialised weights
-            latest = ckpt.latest_checkpoint(self.model_dir)
-            if latest is None:
-                raise ValueError('Estimator.evaluate: no trained model - call train() first or point model_dir at a '
-                                 'directory holding a checkpoint (model_dir=%r)' % (self.model_dir,))
-            if getattr(self, '_eval_restored', None) != latest:
-                ckpt.restore(latest, spec.model.engine, None)               # weights + step; the hook snapshots the state
-                self._eval_restored = latest
+        self._use_trained_weights(spec, 'evaluate')
         for h in spec.evaluation_hooks:
             h.begin()
         metrics = torch.zeros(3, device=spec.model.engine.dev, dtype=torch.float64)

@@ -119,6 +119,16 @@ class NARModuleModel:
         self.predicted_item_probs = out.get('predicted_item_probs')
         return out
 
+    def recommend(self, features: Dict[str, np.ndarray], pop_recent_items_buffer: np.ndarray,
+                  articles_recent_pop_norm: np.ndarray, top_n: Optional[int] = None, candidates=None, positions: str = 'last',
+                  exclude_session_clicks: bool = True) -> dict:
+        """Top-n next-article recommendations for the batch ``features`` (NarEngine.recommend): ``top_n`` defaults to
+        ``metrics_top_n``; ``candidates`` None = the recent-clicks buffer's distinct ids, 'catalog' = every article, or an
+        array of ids.  Reads the weights and the given state; changes neither."""
+        return self.engine.recommend(features, pop_recent_items_buffer, articles_recent_pop_norm,
+                                     self.metrics_top_n if top_n is None else top_n, candidates=candidates,
+                                     positions=positions, exclude_session_clicks=exclude_session_clicks)
+
     def _publish(self, features, labels, out):
         self.item_clicked = features['item_clicked']
         self.event_timestamp = features['event_timestamp'][..., None]

@@ -228,6 +228,25 @@ def rank_candidates(logits, cand_ids, n_pos, n_cand, top_n, pred_ids, pred_probs
                                           _p(metrics), _stream()), 'nar_rank_candidates')
 
 
+def car_combine_grid(PC, PI, Q, Nc, Cdim, H1, act=ACT_LEAKY):
+    """H1[q*Nc + j] = act(PC[q] + PI[j])  (nar_car_combine_grid)."""
+    global LAUNCHES
+    LAUNCHES += 1
+    _chk_f32(PC, PI, H1)
+    check(_lib.load().nar_car_combine_grid(_p(PC), _p(PI), Q, Nc, Cdim, act, _p(H1), _stream()), 'nar_car_combine_grid')
+
+
+def topn_candidates(logits, cand_ids, Q, N, top_n, out_ids, out_scores=None, out_probs=None, item_clicked=None, q_pos=None, T=0):
+    """Per query row of logits [Q, N]: the top_n candidates (score desc, index asc), their scores and softmax probabilities
+    over the non-excluded candidates; ``item_clicked`` [*, T] + ``q_pos`` [Q] (flat b*T+t) exclude each query's own
+    clicks item_clicked[b, 0..t]  (nar_topn_candidates)."""
+    global LAUNCHES
+    LAUNCHES += 1
+    _chk_f32(logits, out_scores, out_probs)
+    check(_lib.load().nar_topn_candidates(_p(logits), _p(cand_ids), Q, N, int(top_n), _p(item_clicked), _p(q_pos), int(T),
+                                          _p(out_ids), _p(out_scores), _p(out_probs), _stream()), 'nar_topn_candidates')
+
+
 def dropout_rows(src, dst, rows, cols, ld, row_pos, n_input, n_cand, K, tensor_id, keep_prob, seed, step):
     """dst = src * mask / keep_prob with the counter-based masks of oracle/dropout_ref.py (tensor_id 0: feature rows)."""
     global LAUNCHES

@@ -281,6 +281,20 @@ int nar_cosine_softmax_ce(const float* cand, const float* pred, int64_t n_pos, i
 int nar_rank_candidates(const float* logits, const int64_t* cand_ids, int64_t n_pos, int64_t n_cand, int32_t top_n,
                         int64_t* pred_ids, float* pred_probs, double* metrics /*[3] float64*/, void* stream);
 
+/* ---- recommendation (NarEngine.recommend; csrc/recommend.cu).  A candidate is scored for a query position exactly like
+ *      a sampled negative of that position (nar_model.py:356-364, :374-405, :444-515).                               */
+/* CAR layer 1 of a grid of (query, candidate) pairs: H1 [Q*Nc, C], row q*Nc + j = act(PC[q] + PI[j]) (PC [Q,C] context
+ * halves + bias, PI [Nc,C] item halves; all 16-byte aligned).                                                        */
+int nar_car_combine_grid(const float* PC, const float* PI, int64_t Q, int64_t Nc, int64_t C, int act, float* H1, void* stream);
+/* per query row of logits [Q,N] (already / temperature): the top_n (1..min(N, 4096)) largest, by descending score, ties to
+ * the lower candidate index (tf.nn.top_k order).  cand_ids [N] distinct.  item_clicked [*, T] or NULL: when given, query q
+ * at flat position q_pos[q] = b*T+t never returns item_clicked[b*T + 0..t] (T <= 1024).  out_ids / out_scores / out_probs
+ * [Q,top_n] (scores / probs may be NULL); probs = softmax over the non-excluded candidates.  A query with fewer than top_n
+ * non-excluded candidates gets id 0, score -inf, prob 0 in the remaining slots.                                          */
+int nar_topn_candidates(const float* logits, const int64_t* cand_ids, int64_t Q, int64_t N, int32_t top_n,
+                        const int64_t* item_clicked, const int32_t* q_pos, int64_t T, int64_t* out_ids, float* out_scores,
+                        float* out_probs, void* stream);
+
 /* ---- host state (CPU, no CUDA): ClickedItemsState.update_items_state (clicked_items_state.py:187-250) in one pass.
  *      buffer [cap,2] int64 {item, timestamp} newest first, zero padded (in/out); batch_items / batch_ts: the step's
  *      non-padded clicks in batch order (nar_model.py:1635-1646); hours_ms = recent_clicks_buffer_hours * 3.6e6;
@@ -416,6 +430,20 @@ int nar_engine_refresh(nar_engine* eng, void* stream);
  * "PR", "logits", "base_pos", "base_item", ...  Returns NAR_ERR_INVALID for an unknown name.                       */
 int nar_engine_buffer(const nar_engine* eng, const nar_step_io* io /*host*/, const char* name, void** ptr /*host*/,
                       int64_t* rows /*host*/, int64_t* ld /*host*/);
+/* Recommendation (forward only; reads the weights, writes nothing but the workspace and the outputs).  io: a staged batch
+ * as for a step with train = 0 (labels unused), L valid positions, io->ws / ws_bytes = the workspace; prep_ws unused.
+ * Q queries: q_rows [Q] int64 = the local row l (index into pos_idx) of each query, or NULL for every row (Q = L);
+ * q_pos [Q] int32 = its flat position b*T+t.  cand_ids [N] distinct ids in [1, V).  Per query block of q_block queries:
+ * every candidate chunk of n_block candidates through CAR layer 1 (PC + PI, nar_car_combine_grid), layer 2, the scorer
+ * into logits [q_block, N], then nar_topn_candidates (exclusion of the session's own clicks when exclude_session_clicks).
+ * Forward GEMMs follow cfg.fwd_precision without split-K: the outputs do not depend on the block sizes.
+ * nar_engine_recommend_workspace_bytes picks the largest blocks whose workspace fits budget_bytes (gather_q: q_rows != NULL). */
+int nar_engine_recommend_workspace_bytes(const nar_engine* eng, int64_t L, int64_t Q, int64_t N, int32_t gather_q,
+                                         int64_t budget_bytes, int64_t* ws_bytes /*host*/, int64_t* q_block /*host*/,
+                                         int64_t* n_block /*host*/);
+int nar_engine_recommend(nar_engine* eng, const nar_step_io* io /*host*/, const int64_t* q_rows, const int32_t* q_pos, int64_t Q,
+                         const int64_t* cand_ids, int64_t N, int32_t top_n, int32_t exclude_session_clicks, int64_t q_block,
+                         int64_t n_block, int64_t* out_ids, float* out_scores, float* out_probs, void* stream);
 /* kernels launched by this engine so far */
 int64_t nar_engine_launch_count(const nar_engine* eng);
 
