@@ -149,6 +149,13 @@ _SIGNATURES = {
     'nar_transpose_f32': (C.c_int, [vp, i64, i64, i64, vp, i64, vp]),
     'nar_adam_tf': (C.c_int, [vp, vp, vp, vp, i64, i64, f32, f32, f32, f32, f32, i64, vp, vp]),
     'nar_tf32_lo': (C.c_int, [vp, i64, vp, vp]),
+    'nar_baselines_clear': (C.c_int, [vp, vp, vp, vp, i64, vp]),
+    'nar_baselines_rehash': (C.c_int, [vp, vp, vp, vp, i64, vp, vp, vp, vp, i64, vp, vp]),
+    'nar_baselines_update': (C.c_int, [vp, vp, vp, vp, i64, vp, vp, i64, i64, i64, i32, i64, vp, vp]),
+    'nar_baselines_buffer_hist': (C.c_int, [vp, i64, i64, vp, vp, vp, vp]),
+    'nar_baselines_row_norms': (C.c_int, [vp, i64, i64, i64, vp, vp]),
+    'nar_baselines_score': (C.c_int, [vp, vp, vp, vp, i64, vp, vp, vp, i64, i64, i64, vp, vp, vp, vp, i64, i64, vp, i64,
+                                      C.c_double, C.c_double, i32, i32, vp, vp, vp, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = sorted(_SIGNATURES.keys())

@@ -8,7 +8,9 @@ split across ``train`` / ``evaluate`` calls.  TF's bundle format is not reproduc
   layout padding / column permutation), so a checkpoint does not depend on the internal HBM layout,
 * ``global_step``,
 * ``state/*`` - the host-side ``ClickedItemsState`` (recent-clicks buffer, popularity counters) when given; the
-  reference keeps that object alive in the trainer process instead (nar_trainer_gcom.py:486-489).
+  reference keeps that object alive in the trainer process instead (nar_trainer_gcom.py:486-489),
+* ``baselines/*`` - the baseline recommenders' pair table (``baselines.BaselineTables.export``: occupied entries
+  sorted by key, value arrays alongside) when the state holds one.  Checkpoints without it load as before.
 """
 from __future__ import annotations
 
@@ -66,6 +68,10 @@ def save(path: str, engine, clicked_items_state=None) -> str:
         for f in STATE_FIELDS:
             arrays['state/' + f] = np.asarray(getattr(clicked_items_state, f))
         arrays['state/current_step'] = np.asarray(clicked_items_state.current_step, dtype=np.int64)
+        tables = getattr(clicked_items_state, 'baselines', None)
+        if tables is not None:
+            for k, v in tables.state_arrays().items():
+                arrays['baselines/' + k] = v
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     tmp = '%s.tmp%d.npz' % (path, os.getpid())      # unique per process: writers never share a temp file
     np.savez(tmp, **arrays)
@@ -75,7 +81,7 @@ def save(path: str, engine, clicked_items_state=None) -> str:
 
 def load(path: str) -> dict:
     with np.load(path, allow_pickle=False) as z:
-        out = {'params': {}, 'adam_m': {}, 'adam_v': {}, 'state': {}, 'global_step': int(z['global_step'])}
+        out = {'params': {}, 'adam_m': {}, 'adam_v': {}, 'state': {}, 'baselines': {}, 'global_step': int(z['global_step'])}
         for k in z.files:
             if '/' in k:
                 group, name = k.split('/', 1)
@@ -92,4 +98,15 @@ def restore(path: str, engine, clicked_items_state=None) -> int:
         for f in STATE_FIELDS:
             setattr(clicked_items_state, f, np.array(ck['state'][f]))
         clicked_items_state.current_step = int(ck['state']['current_step'])
+    if clicked_items_state is not None and getattr(clicked_items_state, 'baselines', None) is not None and ck['baselines']:
+        clicked_items_state.baselines.load(ck['baselines'])
     return ck['global_step']
+
+
+def restore_baselines(path: str, tables) -> bool:
+    """Load the baseline tables of checkpoint ``path`` into ``tables``; False (tables untouched) when it has none."""
+    ck = load(path)
+    if not ck['baselines']:
+        return False
+    tables.load(ck['baselines'])
+    return True

@@ -6,8 +6,9 @@ hook's batch flattening nar_model.py:1635-1646) is ONE C pass in libnar_b200 (``
 csrc/host_state.cu, host code, ~40 us per G1 step); there is no numpy fallback - without the library every update
 raises.  The numpy specification it is bit-checked against lives with the test infrastructure
 (oracle/clicked_items_state_ref.py, pinned to fixtures produced by the reference class itself).
-Out of scope (SURVEY.md section 8, row a-14): the co-occurrence CSR matrix (:252-255, benchmarks only), cold-start
-bookkeeping (:97-123, :196-203).
+The co-occurrence matrix (:252-255) and the baselines' own state (``benchmarks_states``) are the device pair table of
+``baselines.BaselineTables``, kept in ``self.baselines`` when the hook enables baseline recommenders and snapshot /
+restored with the rest.  Out of scope (SURVEY.md section 8, row a-14): cold-start bookkeeping (:97-123, :196-203).
 """
 from __future__ import annotations
 
@@ -22,9 +23,12 @@ class ClickedItemsState:
         self.recent_clicks_buffer_max_size = recent_clicks_buffer_max_size
         self.recent_clicks_for_normalization = recent_clicks_for_normalization
         self.num_items = num_items
+        self.baselines = None                 # baselines.BaselineTables when baseline recommenders are enabled
         self.reset_state()
 
     def reset_state(self):
+        if self.baselines is not None:
+            self.baselines.clear()
         self.articles_pop = np.zeros(shape=[self.num_items], dtype=np.int64)
         self.articles_recent_pop = np.zeros(shape=[self.num_items], dtype=np.int64)
         # empty buffer: pop / (0 + 1) floored at 1 / recent_clicks_for_normalization (clicked_items_state.py:240-246)
@@ -39,6 +43,8 @@ class ClickedItemsState:
         self.articles_pop_chkp = np.copy(self.articles_pop)
         self.pop_recent_clicks_buffer_chkp = np.copy(self.pop_recent_clicks_buffer)
         self.current_step_chkp = self.current_step
+        if self.baselines is not None:
+            self.baselines.snapshot()
 
     def restore_state_checkpoint(self):
         self.articles_pop = self.articles_pop_chkp
@@ -46,6 +52,8 @@ class ClickedItemsState:
         self.pop_recent_clicks_buffer = self.pop_recent_clicks_buffer_chkp
         del self.pop_recent_clicks_buffer_chkp
         self.current_step = self.current_step_chkp
+        if self.baselines is not None:
+            self.baselines.restore()
         # NB: like the reference, recent_pop / recent_pop_norm are NOT restored here;
         # they are recomputed by the next update_items_state().
 

@@ -92,7 +92,8 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
     hooks = [ItemsStateUpdaterHook(mode, model, eval_metrics_top_n=eval_metrics_top_n, clicked_items_state=state,
                                    eval_sessions_metrics_log=eval_sessions_metrics_log,
                                    content_article_embeddings_matrix=params['content_article_embeddings_matrix'],
-                                   articles_metadata=params['articles_metadata'])]
+                                   articles_metadata=params['articles_metadata'],
+                                   eval_benchmark_classifiers=params.get('eval_benchmarks') or ())]
     if mode == ModeKeys.TRAIN:
         def train_op(feats, labs, feed, sync=True):
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
@@ -191,6 +192,17 @@ class Estimator:
             feed = feed_of(spec)
             st_next = eng.stage_ahead(nxt[0], nxt[1], feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], 'pipe0')
         pending = None                                              # (features, labels, out) of the step whose loss is unread
+        # baseline recommenders (nar_model.py:1641-1646): every batch is folded into their tables on the side stream,
+        # behind the batch's copy; the main stream's work is unchanged
+        tables = getattr(self._state(), 'baselines', None)
+        if tables is not None and not tables.uses_table:
+            tables = None
+
+        def fold(st):
+            if tables is not None and st['has_clicks']:
+                import torch
+                side = eng.side_stream() if eng.use_side_stream else torch.cuda.current_stream()
+                tables.update(st['t']['all_items'], lens=st['fold_lens'], stream=side, after=st.get('copied'))
 
         def finish(p):
             f_, l_, o_ = p
@@ -201,7 +213,11 @@ class Estimator:
 
         while nxt is not None:
             features, labels = nxt
+            if tables is not None:
+                st_next['fold_lens'] = _session_clicks(features, labels)
             out = eng.submit(st_next)                               # step n queued on the main stream
+            if not use_ds:
+                fold(st_next)
             prev_st = st_next
             self.h2d_bytes_per_step = st_next['h2d_bytes']           # bytes of the one pinned H2D copy of this step
             if not use_ds:
@@ -216,12 +232,14 @@ class Estimator:
                 after = pending[2]['done'] if pending is not None else None
                 if use_ds:
                     st_next = eng.stage_ahead_device_state(nxt[0], nxt[1], 'pipe%d' % (n & 1), prev_st, after=after)
+                    fold(prev_st)                                    # after the device state absorbed it
                 else:
                     feed = feed_of(spec)
                     st_next = eng.stage_ahead(nxt[0], nxt[1], feed['pop_recent_items_buffer'],
                                               feed['articles_recent_pop_norm'], 'pipe%d' % (n & 1), after=after)
             elif use_ds:
                 eng.advance_device_state(prev_st)                    # the last batch of this train() call
+                fold(prev_st)
             if pending is not None:
                 finish(pending)                                      # loss of step n-1: the GPU already runs step n
             pending = (features, labels, out)
@@ -257,6 +275,9 @@ class Estimator:
         restored = getattr(self, '_restored', {})
         if restored.get(id(spec)) != latest:
             ckpt.restore(latest, spec.model.engine, None)                   # weights + step; the state is not touched
+            state = self._state()
+            if state is not None and getattr(state, 'baselines', None) is not None:
+                ckpt.restore_baselines(latest, state.baselines)             # what the baselines learnt with those weights
             restored[id(spec)] = latest
             self._restored = restored
 
@@ -343,13 +364,16 @@ class Estimator:
                 feed.update(h.before_run(None))
             out = update(features, labels, feed, metrics, step_id=n + 1)
             run_values = {'clicked_items': features['item_clicked'], 'clicked_timestamps': features['event_timestamp'],
-                          'last_item_label': labels['label_last_item']}
+                          'last_item_label': labels['label_last_item'], 'stage': out['stage'],
+                          'eval_batch_negative_items': out['negatives']}
             for h in spec.evaluation_hooks:
                 h.after_run(None, run_values)
             loss_sum += out['total_loss']
             n += 1
             nxt = fetch() if (steps is None or n < steps) else None
+        bench = {}
         for h in spec.evaluation_hooks:
+            bench.update(h.benchmark_results())
             h.end()
         eng = spec.model.engine
         if eng.world > 1:                                           # data parallel: every rank ranked its own sessions
@@ -357,11 +381,17 @@ class Estimator:
         m = metrics.cpu().numpy()
         cnt = max(float(m[2]), 1.0)
         return {'loss': loss_sum / max(n, 1), 'hitrate_at_n': float(m[0]) / cnt, 'mrr_at_n': float(m[1]) / cnt,
-                'global_step': spec.model.global_step()}
+                'global_step': spec.model.global_step(), **bench}
 
     @property
     def model(self) -> Optional[NARModuleModel]:
         return None if self._spec is None else self._spec.model
+
+
+def _session_clicks(features, labels) -> np.ndarray:
+    """Nonzero clicks of every session of concat(item_clicked, label_last_item) (the baselines' growth bound)."""
+    ic = np.asarray(features['item_clicked'])
+    return np.count_nonzero(ic, axis=1) + (np.asarray(labels['label_last_item']).reshape(-1) != 0)
 
 
 def build_estimator(model_dir, content_article_embeddings_matrix, articles_metadata, articles_features_config,

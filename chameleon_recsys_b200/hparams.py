@@ -141,11 +141,14 @@ class NARHParams:
     ranking: str = 'mlp'             # 'mlp' = reference code (nar_model.py:447-500); 'cosine' = north_star wording
     sampler_seed: int = 42           # RANDOM_SEED, nar_trainer_gcom.py:33
     init_seed: int = 42
+    # baseline recommenders evaluated next to the model (nar_trainer_gcom.py:280-300): suffixes or
+    # {'recommender': <suffix>, 'params': {...}} of 'pop_recent', 'coocurrent', 'item_knn', 'cb', 'sr' (baselines.py)
+    eval_benchmarks: tuple = ()
 
     def to_params(self, session_features_config, articles_features_config, articles_metadata,
                   content_article_embeddings_matrix) -> dict:
         """The ``params`` dict handed to ``nar_module_model_fn`` (nar_trainer_gcom.py:355-384)."""
-        return {
+        params = {
             'batch_size': self.batch_size,
             'lr': self.learning_rate,
             'dropout_keep_prob': self.dropout_keep_prob,
@@ -182,6 +185,9 @@ class NARHParams:
             'rnn_cell': self.rnn_cell,
             'ranking': self.ranking,
         }
+        if self.eval_benchmarks:                 # the key exists only when baselines are requested
+            params['eval_benchmarks'] = list(self.eval_benchmarks)
+        return params
 
     def copy(self, **kw) -> 'NARHParams':
         h = copy.deepcopy(self)

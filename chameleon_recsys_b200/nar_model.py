@@ -159,12 +159,32 @@ class ItemsStateUpdaterHook:
         self.eval_metrics_top_n = eval_metrics_top_n
         self.clicked_items_state = clicked_items_state
         self.eval_sessions_metrics_log = eval_sessions_metrics_log
+        # baseline recommenders (nar_model.py:1399-1407): [{'recommender': <suffix>, 'params': {...}}]; their state is the
+        # BaselineTables object on the ClickedItemsState, shared by the TRAIN and EVAL hooks
+        self.bench_metrics = None
+        self.baselines = None
         if eval_benchmark_classifiers:
-            raise NotImplementedError('benchmark recommenders are out of scope (SURVEY.md section 2, rows 9-11)')
+            from .baselines import BaselineTables, parse_classifiers
+            wanted = parse_classifiers(eval_benchmark_classifiers)
+            eng = model.engine
+            if eng.world > 1:
+                raise NotImplementedError('baseline recommenders run on one process; data-parallel evaluation of the '
+                                          'baselines is not implemented')
+            tables = clicked_items_state.baselines
+            if tables is None:
+                tables = BaselineTables(eval_benchmark_classifiers, clicked_items_state.num_items, acr=eng.acr,
+                                        acr_dim=model.plan.acr_dim, device=eng.dev.index)
+                clicked_items_state.baselines = tables
+            elif tables.params != wanted:
+                raise ValueError('ClickedItemsState already holds baselines %r, not %r' % (tables.params, wanted))
+            self.baselines = tables
 
     def begin(self):
         if self.mode == ModeKeys.EVAL:
             self.clicked_items_state.save_state_checkpoint()        # nar_model.py:1415
+            if self.baselines is not None:
+                import torch
+                self.bench_metrics = torch.zeros(5, 3, dtype=torch.float64, device=self.model.engine.dev)
 
     def before_run(self, run_context=None) -> dict:
         """-> feed dict (nar_model.py:1458-1467)."""
@@ -172,9 +192,25 @@ class ItemsStateUpdaterHook:
                 'pop_recent_items_buffer': self.clicked_items_state.get_recent_clicks_buffer()}
 
     def after_run(self, run_context, run_values: dict):
-        """run_values: {'clicked_items','clicked_timestamps','last_item_label'} (nar_model.py:1505-1508)."""
+        """run_values: {'clicked_items','clicked_timestamps','last_item_label'} (nar_model.py:1505-1508).  In EVAL with
+        baselines enabled also 'stage' (the staged batch of the step) and 'eval_batch_negative_items' ([B,T,K] device):
+        the baselines rank the batch against the state BEFORE it, then learn from it (nar_model.py:1609-1632)."""
+        if self.baselines is not None and self.mode == ModeKeys.EVAL:
+            t = run_values['stage']['t']
+            self.baselines.score(t['item_clicked'], t['label_next'], run_values['eval_batch_negative_items'],
+                                 self.clicked_items_state.get_recent_clicks_buffer(),
+                                 self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n, self.bench_metrics)
+            if run_values['stage']['has_clicks']:
+                self.baselines.update(t['all_items'], lens=np.count_nonzero(np.concatenate(
+                    [run_values['clicked_items'], np.asarray(run_values['last_item_label']).reshape(-1, 1)], axis=1), axis=1))
         self.clicked_items_state.update_from_batch(run_values['clicked_items'], run_values['clicked_timestamps'],
                                                    run_values['last_item_label'])
+
+    def benchmark_results(self) -> dict:
+        """{'hitrate_at_n_<suffix>', 'mrr_at_n_<suffix>'} of this evaluation's baselines ({} without baselines)."""
+        if self.baselines is None or self.bench_metrics is None:
+            return {}
+        return self.baselines.results(self.bench_metrics)
 
     def end(self, session=None):
         if self.mode == ModeKeys.EVAL:

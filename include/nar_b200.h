@@ -447,6 +447,36 @@ int nar_engine_recommend(nar_engine* eng, const nar_step_io* io /*host*/, const 
 /* kernels launched by this engine so far */
 int64_t nar_engine_launch_count(const nar_engine* eng);
 
+/* ---- baseline recommenders of the evaluation hook (csrc/baselines.cu, spec oracle/baselines_ref.py) ----------------
+ * Pair table: cap (a power of two) slots of keys [cap] ((a << 32) | c, -1 empty), cooc [cap] (sessions with a and c at
+ * two different positions), sr_w [cap] (sequential-rules weight in units of 1 / lcm(1..max_clicks_dist)), sr_first [cap]
+ * (min (batch_seq << 32) | ordinal of the rule's occurrences, INT64_MAX when none); count [1] = occupied slots.
+ * nar_baselines_clear empties a table; nar_baselines_rehash clears the new table and moves every entry into it.
+ * nar_baselines_update folds one batch: all_items [Bg, T1] = item_clicked | label_last_item (0 = padding); *err = 1 for
+ * an id outside [0, num_items), 2 when the table is full (the caller sizes it: at most sum len*(len-1) new entries).  */
+int nar_baselines_clear(int64_t* keys, int64_t* cooc, int64_t* sr_w, int64_t* sr_first, int64_t cap, void* stream);
+int nar_baselines_rehash(const int64_t* keys, const int64_t* cooc, const int64_t* sr_w, const int64_t* sr_first, int64_t cap,
+                         int64_t* new_keys, int64_t* new_cooc, int64_t* new_sr_w, int64_t* new_sr_first, int64_t new_cap,
+                         int* err, void* stream);
+int nar_baselines_update(int64_t* keys, int64_t* cooc, int64_t* sr_w, int64_t* sr_first, int64_t cap, int64_t* count,
+                         const int64_t* all_items, int64_t Bg, int64_t T1, int64_t num_items, int32_t max_clicks_dist,
+                         int64_t batch_seq, int* err, void* stream);
+/* count [num_items] / first [num_items] int32: occurrences and first index of every nonzero id of buffer [n] */
+int nar_baselines_buffer_hist(const int64_t* buffer, int64_t n, int64_t num_items, int32_t* count, int32_t* first, int* err,
+                              void* stream);
+/* norms [V] fp64: Euclidean norm of every row of acr [V, ld] (first dim columns) */
+int nar_baselines_row_norms(const float* acr, int64_t V, int64_t dim, int64_t ld, double* norms, void* stream);
+/* Scores, ranks and measures the enabled baselines (bit b of enabled: 0 pop_recent, 1 coocurrent, 2 item_knn, 3 cb, 4 sr)
+ * for every query (b, t) with label_next != 0, over the candidates label + negatives [B, T, K] (first occurrence of an id
+ * only).  metrics [5, 3] fp64 += {hits, sum of reciprocal ranks, queries} per baseline (rank_hist [5, top_n + 1] int64 is
+ * scratch); out_ids [5, B*T, top_n] (optional) = each query's top-n ids, 0-padded.                                    */
+int nar_baselines_score(const int64_t* keys, const int64_t* cooc, const int64_t* sr_w, const int64_t* sr_first, int64_t cap,
+                        const int64_t* item_clicked, const int64_t* label_next, const int64_t* negatives, int64_t B,
+                        int64_t T, int64_t K, const int32_t* buf_count, const int32_t* buf_first,
+                        const int64_t* articles_pop, const float* acr, int64_t acr_dim, int64_t acr_ld,
+                        const double* acr_norm, int64_t num_items, double knn_lambda, double knn_alpha, int32_t enabled,
+                        int32_t top_n, int64_t* rank_hist, double* metrics, int64_t* out_ids, int* err, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
