@@ -9,9 +9,10 @@
 //   dgrad dX = dY * W^T      A = dY (K-major)   B = W   (K-major)
 //   wgrad dW = X^T * dY      A = X  (MN-major)  B = dY  (MN-major), split-K + red.add
 //
-// CTA = 256 threads = two warpgroups, one 128 x 128 output tile, k-tiles of 32 (32 fp32 = one 128-byte swizzle row):
-//   thread 0     keeps STAGES k-tiles of A and B in flight (cp.async.bulk.tensor.2d, 128-byte swizzle, one mbarrier
-//                per stage) and refills a stage as soon as every thread is done with it;
+// CTA = 256 threads = two warpgroups, one 128 x 128 output tile, k-tiles of 32 (32 fp32 = one 128-byte swizzle row);
+// two CTAs per SM when B needs no transpose / split pass (see Cfg), else one:
+//   thread 0     keeps STAGES - 1 k-tiles of A and B ahead of the one being multiplied (cp.async.bulk.tensor.2d,
+//                128-byte swizzle, one mbarrier per stage) and refills a stage as soon as its MMAs are done;
 //   warpgroup w  multiplies rows [64w, 64w + 64) of the tile with wgmma.m64n128: A from registers, B from shared
 //                memory.  A is read from the swizzled TMA tile straight into the register fragment whatever its major,
 //                and that is also where 3xTF32 splits it.  wgmma reads 32-bit B operands only K-major, so a B tile that
@@ -32,6 +33,7 @@
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
+#include <type_traits>
 
 namespace nar {
 namespace gemm {
@@ -48,12 +50,17 @@ template <int MODE, bool B_MN> struct Cfg {
   static constexpr bool BLO = MODE == 2;
   static constexpr bool PREP = B_MN || SPLIT3;                        // B goes through the transpose / split pass
   static constexpr int STAGE_BYTES = TILE_BYTES * (BLO ? 3 : 2);      // A | B [| B_lo]
-  static constexpr int STAGES = BLO ? 3 : 4;
-  static constexpr int PREP_BYTES = PREP ? TILE_BYTES * (SPLIT3 ? 2 : 1) : 0;   // K-major B_hi [| B_lo]
+  // Without a prep pass two CTAs share an SM (3 stages = 96 KB each, <= 128 registers per thread), so that one CTA's
+  // epilogue runs under the other's main loop; with one, the prep tiles leave room for one CTA.
+  static constexpr int CTAS_PER_SM = PREP ? 1 : 2;
+  static constexpr int STAGES = (BLO || !PREP) ? 3 : 4;
+  static constexpr int PREP_TILE_BYTES = PREP ? TILE_BYTES * (SPLIT3 ? 2 : 1) : 0;   // K-major B_hi [| B_lo]
+  static constexpr int PREP_BYTES = 2 * PREP_TILE_BYTES;             // double-buffered: k-tile kt uses buffer kt & 1
   static constexpr int BAR_OFF = STAGES * STAGE_BYTES + PREP_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;              // + barriers + alignment slack
   static_assert(STAGES * STAGE_BYTES >= BM * EPI_LD * 4, "the epilogue stages the accumulators in the operand ring");
   static_assert(SMEM_BYTES <= 227 * 1024, "227 KB of shared memory per block");
+  static_assert(CTAS_PER_SM * (SMEM_BYTES + 1024) <= 228 * 1024, "228 KB of shared memory per SM (1 KB reserved per block)");
 };
 
 struct Params {
@@ -104,7 +111,9 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// waits until at most N committed groups of this warpgroup's MMAs are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
 __device__ __forceinline__ void fence_acc(float (&d)[64]) {
 #pragma unroll
@@ -276,7 +285,7 @@ __device__ __forceinline__ void load_operand(uint32_t dst, const CUtensorMap* ma
 
 // ---------------------------------------------------------------- kernel
 template <bool A_MN, bool B_MN, int MODE>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(NUM_THREADS, (Cfg<MODE, B_MN>::CTAS_PER_SM))
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_blo, const Params p) {
   using C = Cfg<MODE, B_MN>;
@@ -317,8 +326,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       if (C::BLO) load_operand<B_MN>(b_dst + TILE_BYTES, &tmap_blo, bar, n_blk * BN, k_elem);
     }
   };
+  // k-tile kt goes to stage kt % STAGES; the stage of kt - 1 is refilled (with kt - 1 + STAGES) during k-tile kt, once
+  // the MMAs of kt - 1 are done, so STAGES - 1 k-tiles are ahead of the one being multiplied
   if (tid == 0)
-    for (int kt = 0; kt < C::STAGES && kt < num_kt; ++kt) issue(kt);
+    for (int kt = 0; kt < C::STAGES - 1 && kt < num_kt; ++kt) issue(kt);
 
   // wgmma fragments: warp w (of 8) owns tile rows [16w, 16w + 16); lane = 4 g + t.  A: rows 16w + g (+8), k t (+4)
   // for tf32, k 2t (+8) for bf16 pairs.  D: rows 16w + g (+8), columns 8j + 2t (+1).
@@ -327,72 +338,89 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  // A fragments, double-buffered: the MMAs of a k-tile read theirs asynchronously, so k-tile kt writes buffer kt & 1,
+  // whose last readers (the MMAs of kt - 2) are complete after the wait_group 1 of kt - 1
+  uint32_t a[2][4][4], alo[2][4][4];      // tf32: hi (or the single-pass value) | lo (3xTF32)
+  uint32_t ahi16[2][2][4], alo16[2][2][4];  // bf16x3: A_hi | A_lo pairs
 
-  for (int kt = 0; kt < num_kt; ++kt) {
+  // One k-tile; BUF = kt & 1 is a compile-time constant (the loop below is unrolled by two) so that the fragments stay
+  // in registers.  The MMAs of kt are left in flight while the next k-tile waits for its TMA and stages its operands.
+  auto k_tile = [&](const int kt, auto buf_tag) {
+    constexpr int BUF = decltype(buf_tag)::value;
     const int s = kt % C::STAGES;
     mbar_wait(&full[s], (uint32_t)(kt / C::STAGES) & 1u);
     const uint8_t* sa = smem + s * C::STAGE_BYTES;
     const uint8_t* sb = sa + TILE_BYTES;
+    uint8_t* pb = prep + BUF * C::PREP_TILE_BYTES;
     if (C::PREP) {
-      prep_b<B_MN, MODE>(sb, sb + TILE_BYTES, prep, prep + TILE_BYTES, tid);
+      prep_b<B_MN, MODE>(sb, sb + TILE_BYTES, pb, pb + TILE_BYTES, tid);
       fence_proxy_async_smem();       // generic-proxy writes -> wgmma (async proxy) reads
-      __syncthreads();
+      __syncthreads();                // both warpgroups read the whole prep tile
     }
-    const uint32_t b_hi = smem_u32(C::PREP ? prep : sb);
+    const uint32_t b_hi = smem_u32(C::PREP ? pb : sb);
     const uint32_t b_lo = b_hi + TILE_BYTES;        // 3x: the prep B_lo tile
     if (BF16) {
-      uint32_t ahi[2][4], alo[2][4];
+      uint32_t (&ahi)[2][4] = ahi16[BUF];
+      uint32_t (&al)[2][4] = alo16[BUF];
 #pragma unroll
       for (int j = 0; j < 2; ++j)
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const int r = r0 + (q & 1) * 8, k = 16 * j + 2 * t + (q >> 1) * 8;
           const float2 x = *reinterpret_cast<const float2*>(sa + tile_off<false>(r, k));
-          split_bf16x2(x.x, x.y, ahi[j][q], alo[j][q]);
+          split_bf16x2(x.x, x.y, ahi[j][q], al[j][q]);
         }
       wgmma_fence();
 #pragma unroll
       for (int j = 0; j < 2; ++j) {        // two k = 16 steps per 32-k tile: 32 B of the hi half, then of the lo half
-        wgmma_bf16(acc, alo[j], make_desc(b_hi + 32 * j));          // A_lo * B_hi
+        wgmma_bf16(acc, al[j], make_desc(b_hi + 32 * j));           // A_lo * B_hi
         wgmma_bf16(acc, ahi[j], make_desc(b_hi + 64 + 32 * j));     // A_hi * B_lo
         wgmma_bf16(acc, ahi[j], make_desc(b_hi + 32 * j));          // A_hi * B_hi
       }
     } else {
-      uint32_t a[4][4];
+      uint32_t (&ah)[4][4] = a[BUF];
+      uint32_t (&al)[4][4] = alo[BUF];
 #pragma unroll
       for (int j = 0; j < 4; ++j)
 #pragma unroll
         for (int q = 0; q < 4; ++q)
-          a[j][q] = *reinterpret_cast<const uint32_t*>(sa + tile_off<A_MN>(r0 + (q & 1) * 8, 8 * j + t + (q >> 1) * 4));
+          ah[j][q] = *reinterpret_cast<const uint32_t*>(sa + tile_off<A_MN>(r0 + (q & 1) * 8, 8 * j + t + (q >> 1) * 4));
       if (C::SPLIT3) {
-        uint32_t alo[4][4];
 #pragma unroll
         for (int j = 0; j < 4; ++j)
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            const uint32_t h = tf32_hi_bits(a[j][q]);
-            alo[j][q] = __float_as_uint(__uint_as_float(a[j][q]) - __uint_as_float(h));
-            a[j][q] = h;
+            const uint32_t h = tf32_hi_bits(ah[j][q]);
+            al[j][q] = __float_as_uint(__uint_as_float(ah[j][q]) - __uint_as_float(h));
+            ah[j][q] = h;
           }
         wgmma_fence();
 #pragma unroll
         for (int j = 0; j < 4; ++j) {      // small terms first
-          wgmma_tf32(acc, alo[j], make_desc(b_hi + 32 * j));
-          wgmma_tf32(acc, a[j], make_desc(b_lo + 32 * j));
-          wgmma_tf32(acc, a[j], make_desc(b_hi + 32 * j));
+          wgmma_tf32(acc, al[j], make_desc(b_hi + 32 * j));
+          wgmma_tf32(acc, ah[j], make_desc(b_lo + 32 * j));
+          wgmma_tf32(acc, ah[j], make_desc(b_hi + 32 * j));
         }
       } else {
         wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 4; ++j) wgmma_tf32(acc, a[j], make_desc(b_hi + 32 * j));
+        for (int j = 0; j < 4; ++j) wgmma_tf32(acc, ah[j], make_desc(b_hi + 32 * j));
       }
     }
     wgmma_commit();
-    wgmma_wait_all();
-    fence_acc(acc);
-    __syncthreads();                  // every thread is done with stage s and the prep tiles
-    if (tid == 0 && kt + C::STAGES < num_kt) issue(kt + C::STAGES);
+    wgmma_wait<1>();                  // this warpgroup's MMAs of kt - 1 are done
+    __syncthreads();                  // ... and the other's: stage (kt - 1) % STAGES and prep buffer (kt - 1) & 1 are free
+    if (tid == 0 && kt + C::STAGES - 1 < num_kt) issue(kt + C::STAGES - 1);
+  };
+  int kt = 0;
+  for (; kt + 1 < num_kt; kt += 2) {
+    k_tile(kt, std::integral_constant<int, 0>());
+    k_tile(kt + 1, std::integral_constant<int, 1>());
   }
+  if (kt < num_kt) k_tile(kt, std::integral_constant<int, 0>());
+  wgmma_wait<0>();
+  fence_acc(acc);
+  __syncthreads();                    // the other warpgroup's last MMAs may still read B from the operand ring
 
   // ===== epilogue: the accumulators go through shared memory (the operand ring is idle now) so that each warp then
   // handles 128 contiguous bytes of one row of D / aux per instruction
@@ -491,6 +519,8 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
   static bool attr_set = false;     // per instantiation
   if (!attr_set) {
     NAR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    // all of the SM's unified L1 / shared memory as shared memory, so that CTAS_PER_SM blocks fit side by side
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     attr_set = true;
   }
   kern<<<grid, NUM_THREADS, smem, st>>>(ta, tb, tbl, p);

@@ -1,5 +1,12 @@
-"""Stand-alone GEMM / gather micro-benchmark (CUDA events, L2 flush between iterations).
-   python tools/gemm_bench.py [quick]      -> prints one JSON line per shape."""
+"""Stand-alone GEMM micro-benchmark (CUDA events, L2 flush between iterations).
+   python tools/gemm_bench.py [quick]      -> prints one JSON line per shape.
+
+Two groups of cases: operand-major / precision variants at 24000 x 1024 x 1024, and the training step's own GEMMs at
+the shapes bench.py's roofline times (R = 23 600 candidate rows, C = 1024): CAR layer 2 forward (bf16x3, bias + tanh),
+dgrad (single-pass TF32, leaky derivative from a separate aux) and split-K wgrad, and the scorer's first layer
+(C -> 128) forward / dgrad / wgrad.  Each step case also reports the share of the data-sheet peak of the tensor path it
+issues on (bf16 for bf16x3, counting its 3 MMAs per product; TF32 otherwise) and the rate at which TMA fills shared
+memory with operand tiles."""
 import json
 import os
 import sys
@@ -10,6 +17,9 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from chameleon_recsys_b200 import ops  # noqa: E402
+
+BF16_PEAK, TF32_PEAK = 989.0, 495.0      # dense TFLOP/s, H100 SXM data sheet (700 W)
+STEP_R, C = 23600, 1024
 
 
 def bench(fn, iters=10, flush=None):
@@ -26,11 +36,8 @@ def bench(fn, iters=10, flush=None):
     return float(np.median(ts))
 
 
-def main():
-    quick = len(sys.argv) > 1 and sys.argv[1] == 'quick'
-    iters = 2 if quick else 10
-    dev = 'cuda'
-    flush = None if quick else torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+def variant_cases(dev):
+    """(name, fn, flops, output) at 24000 x 1024 x 1024: every operand major and precision the kernel has."""
     M, N, K = 24000, 1024, 1024
     X = torch.randn(M, K, device=dev)
     W = torch.randn(K, N, device=dev) / 32
@@ -45,25 +52,83 @@ def main():
     Wtlo = torch.empty_like(Wt)
     ops.tf32_lo(Wt, Wt.numel(), Wtlo)
     Wplane = ops.pack_bf16x3(W, K, N)
-    only = os.environ.get('NAR_GEMM_BENCH_ONLY')           # substring filter
-    cases = [
-        ('fwd  bf16x3 A:K fp32 split in registers, B: packed bf16 plane', lambda: ops.gemm(X, None, Y, M, N, K, a_kmajor=True, b_kmajor=True, ldb=0, bias=bias, act=2, precision=4, b_bf16=Wplane, ld_bf16=Wplane.stride(0)), 2.0 * M * N * K),
-        ('fwd  3x  A:K  B:K(W^T) +B_lo', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=3, b_lo=Wtlo), 2.0 * M * N * K),
-        ('fwd  3x  A:K  B:K(W^T) in-kernel split', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=3), 2.0 * M * N * K),
-        ('fwd  1x  A:K  B:K(W^T)', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=1), 2.0 * M * N * K),
-        ('fwd  3x  A:K  B:MN +B_lo', lambda: ops.gemm(X, W, Y, M, N, K, a_kmajor=True, b_kmajor=False, bias=bias, act=2, precision=3, b_lo=Wlo), 2.0 * M * N * K),
-        ('fwd  3x  A:K  B:MN', lambda: ops.gemm(X, W, Y, M, N, K, a_kmajor=True, b_kmajor=False, bias=bias, act=2, precision=3), 2.0 * M * N * K),
-        ('fwd  1x  A:K  B:MN', lambda: ops.gemm(X, W, Y, M, N, K, a_kmajor=True, b_kmajor=False, bias=bias, act=2, precision=1), 2.0 * M * N * K),
-        ('dgrad 1x A:K  B:K ', lambda: ops.gemm(dY, W, Y, M, K, N, a_kmajor=True, b_kmajor=True, precision=1), 2.0 * M * N * K),
-        ('dgrad 1x +dact aux sep', lambda: ops.gemm(dY, W, Y, M, K, N, a_kmajor=True, b_kmajor=True, precision=1, dact=1, aux=X), 2.0 * M * N * K),
-        ('dgrad 1x +dact in place', lambda: ops.gemm(dY, W, X2, M, K, N, a_kmajor=True, b_kmajor=True, precision=1, dact=1, aux=X2), 2.0 * M * N * K),
-        ('wgrad 1x A:MN B:MN', lambda: ops.gemm(X, dY, dW, K, N, M, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), 2.0 * M * N * K),
+    f = 2.0 * M * N * K
+    return [
+        ('fwd  bf16x3 A:K fp32 split in registers, B: packed bf16 plane', lambda: ops.gemm(X, None, Y, M, N, K, a_kmajor=True, b_kmajor=True, ldb=0, bias=bias, act=2, precision=4, b_bf16=Wplane, ld_bf16=Wplane.stride(0)), f, Y),
+        ('fwd  3x  A:K  B:K(W^T) +B_lo', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=3, b_lo=Wtlo), f, Y),
+        ('fwd  3x  A:K  B:K(W^T) in-kernel split', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=3), f, Y),
+        ('fwd  1x  A:K  B:K(W^T)', lambda: ops.gemm(X, Wt, Y, M, N, K, a_kmajor=True, b_kmajor=True, bias=bias, act=2, precision=1), f, Y),
+        ('fwd  3x  A:K  B:MN +B_lo', lambda: ops.gemm(X, W, Y, M, N, K, a_kmajor=True, b_kmajor=False, bias=bias, act=2, precision=3, b_lo=Wlo), f, Y),
+        ('fwd  3x  A:K  B:MN', lambda: ops.gemm(X, W, Y, M, N, K, a_kmajor=True, b_kmajor=False, bias=bias, act=2, precision=3), f, Y),
+        ('fwd  1x  A:K  B:MN', lambda: ops.gemm(X, W, Y, M, N, K, a_kmajor=True, b_kmajor=False, bias=bias, act=2, precision=1), f, Y),
+        ('dgrad 1x A:K  B:K ', lambda: ops.gemm(dY, W, Y, M, K, N, a_kmajor=True, b_kmajor=True, precision=1), f, Y),
+        ('dgrad 1x +dact aux sep', lambda: ops.gemm(dY, W, Y, M, K, N, a_kmajor=True, b_kmajor=True, precision=1, dact=1, aux=X), f, Y),
+        ('dgrad 1x +dact in place', lambda: ops.gemm(dY, W, X2, M, K, N, a_kmajor=True, b_kmajor=True, precision=1, dact=1, aux=X2), f, X2),
+        ('wgrad 1x A:MN B:MN', lambda: ops.gemm(X, dY, dW, K, N, M, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), f, dW),
     ]
-    for name, fn, flops in cases:
+
+
+def step_cases(dev):
+    """(name, fn, [M, N, K], output, precision) of the training step's CAR layer-2 and scorer layer-1 GEMMs, operands as
+    engine.cu passes them: forward A = activations (K-major) with the bf16x3 plane of W [in, out]; dgrad A = dY, B = W
+    read K-major; wgrad A = X and B = dY both MN-major, split-K chosen by the library, red.add into dW."""
+    R = STEP_R
+    H1 = torch.randn(R, C, device=dev)
+    E = torch.empty(R, C, device=dev)
+    dE = torch.randn(R, C, device=dev)
+    dH1 = torch.empty(R, C, device=dev)
+    W2 = torch.randn(C, C, device=dev) / 32
+    b2 = torch.randn(C, device=dev) * 0.1
+    dW2 = torch.zeros(C, C, device=dev)
+    W2plane = ops.pack_bf16x3(W2, C, C)
+    PD = torch.randn(R, C, device=dev)
+    Z1 = torch.empty(R, 128, device=dev)
+    dZ1 = torch.randn(R, 128, device=dev)
+    dPD = torch.empty(R, C, device=dev)
+    M0 = torch.randn(C, 128, device=dev) / 32
+    c0 = torch.randn(128, device=dev) * 0.1
+    dM0 = torch.zeros(C, 128, device=dev)
+    M0plane = ops.pack_bf16x3(M0, C, 128)
+    return [
+        ('step L2 fwd   bf16x3 +bias tanh', lambda: ops.gemm(H1, None, E, R, C, C, ldb=0, bias=b2, act=ops.ACT_TANH, precision=4, b_bf16=W2plane, ld_bf16=W2plane.stride(0)), [R, C, C], E, 4),
+        ('step L2 dgrad 1x +dact leaky aux sep', lambda: ops.gemm(dE, W2, dH1, R, C, C, precision=1, dact=ops.ACT_LEAKY, aux=H1), [R, C, C], dH1, 1),
+        ('step L2 wgrad 1x split-K', lambda: ops.gemm(H1, dE, dW2, C, C, R, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), [C, C, R], dW2, 1),
+        ('step M1 fwd   bf16x3 +bias leaky', lambda: ops.gemm(PD, None, Z1, R, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0)), [R, 128, C], Z1, 4),
+        ('step M1 dgrad 1x', lambda: ops.gemm(dZ1, M0, dPD, R, C, 128, precision=1), [R, C, 128], dPD, 1),
+        ('step M1 wgrad 1x split-K', lambda: ops.gemm(PD, dZ1, dM0, C, 128, R, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), [C, 128, R], dM0, 1),
+    ]
+
+
+def step_rates(shape, precision, us):
+    """algorithmic TFLOP/s, share of the issuing tensor path's peak, and the shared-memory fill rate: TMA brings one
+    32 KB pair of operand tiles (A 128 x 32 fp32 + B 128 x 32 fp32, or B's 128 x 64 bf16 plane tile) per 128 x 128
+    output tile and 32-wide k-tile"""
+    M, N, K = shape
+    flops = 2.0 * M * N * K
+    tflops = flops / (us * 1e-6) / 1e12
+    share = 3 * tflops / BF16_PEAK if precision == 4 else tflops / TF32_PEAK
+    tiles = -(-M // 128) * -(-N // 128) * -(-K // 32)
+    return {'tflops': tflops, 'share_of_peak': share, 'peak': 'bf16 %.0f (3 MMAs per product)' % BF16_PEAK if precision == 4
+            else 'tf32 %.0f' % TF32_PEAK, 'smem_ingest_GBps': tiles * 32768 / (us * 1e-6) / 1e9}
+
+
+def main():
+    quick = len(sys.argv) > 1 and sys.argv[1] == 'quick'
+    iters = 2 if quick else 10
+    dev = 'cuda'
+    torch.manual_seed(0)
+    flush = None if quick else torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    only = os.environ.get('NAR_GEMM_BENCH_ONLY')           # substring filter
+    for name, fn, flops, _ in variant_cases(dev):
         if only and only not in name:
             continue
         ms = bench(fn, iters, flush)
-        print(json.dumps({'case': name, 'shape': [M, N, K], 'us': ms * 1e3, 'tflops': flops / (ms * 1e-3) / 1e12}), flush=True)
+        print(json.dumps({'case': name, 'shape': [24000, 1024, 1024], 'us': ms * 1e3, 'tflops': flops / (ms * 1e-3) / 1e12}), flush=True)
+    for name, fn, shape, _, prec in step_cases(dev):
+        if only and only not in name:
+            continue
+        ms = bench(fn, iters, flush)
+        print(json.dumps({'case': name, 'shape': shape, 'us': ms * 1e3, **step_rates(shape, prec, ms * 1e3)}), flush=True)
 
 
 if __name__ == '__main__':
