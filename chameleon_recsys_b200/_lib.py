@@ -156,6 +156,9 @@ _SIGNATURES = {
     'nar_baselines_row_norms': (C.c_int, [vp, i64, i64, i64, vp, vp]),
     'nar_baselines_score': (C.c_int, [vp, vp, vp, vp, i64, vp, vp, vp, i64, i64, i64, vp, vp, vp, vp, i64, i64, vp, i64,
                                       C.c_double, C.c_double, i32, i32, vp, vp, vp, vp, vp]),
+    'nar_sknn_update': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, i64, i64, i64, vp, vp]),
+    'nar_sknn_score': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, i64, i64, i64, i64, i64, i64, i32, i32, i32,
+                                 vp, vp, vp, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = sorted(_SIGNATURES.keys())

@@ -8,8 +8,12 @@ enabled baselines in one launch.  It hangs off the ``ClickedItemsState`` (``stat
 restore it around an evaluation.
 
 Baselines, by the reference's suffixes: ``pop_recent``, ``coocurrent``, ``item_knn`` (``reg_lambda``, ``alpha``), ``cb``
-(content-based cosine of the ACR rows) and ``sr`` (``max_clicks_dist`` <= 20, ``dist_between_clicks_decay='div'``).
-V-SkNN (``vsknn``) is not implemented.  Ties, scores and timing: DESIGN.md section 9.
+(content-based cosine of the ACR rows), ``sr`` (``max_clicks_dist`` <= 20, ``dist_between_clicks_decay='div'``), and the
+session-based kNN baselines ``v-sknn`` (``first_session_clicks_decay='div'``) and ``sknn`` (``'same'``) with the
+reference's ``sessions_buffer_size`` (<= 4096), ``candidate_sessions_sample_size``, ``sampling_strategy='recent'``,
+``nearest_neighbor_session_for_scoring`` and ``similarity`` ('cosine' / 'jaccard'); each kNN suffix keeps its own ring of
+recent sessions (sknn.py, csrc/sknn.cu) and needs the batches' session ids.  Ties, scores and timing: DESIGN.md
+section 9.
 """
 from __future__ import annotations
 
@@ -21,6 +25,7 @@ import torch
 
 from . import _lib
 from ._lib import check
+from .sknn import KNN_SUFFIXES, SessionKNN, parse_params as _knn_params
 
 SUFFIXES = ('pop_recent', 'coocurrent', 'item_knn', 'cb', 'sr')
 DEFAULT_PARAMS = {'pop_recent': {}, 'coocurrent': {}, 'item_knn': {'reg_lambda': 20, 'alpha': 0.75}, 'cb': {},
@@ -31,14 +36,19 @@ _EMPTY = -1
 
 def parse_classifiers(classifiers) -> Dict[str, dict]:
     """The hook's ``eval_benchmark_classifiers`` list ``[{'recommender': <suffix>, 'params': {...}}]`` (or bare suffixes)
-    -> {suffix: params} in request order.  Raises for V-SkNN, unknown names and unsupported parameters."""
+    -> {suffix: params} in request order.  Raises for unknown names and unsupported parameters."""
     out: Dict[str, dict] = {}
     for clf in classifiers:
         name, params = (clf, {}) if isinstance(clf, str) else (clf['recommender'], dict(clf.get('params') or {}))
         if name == 'vsknn':
-            raise NotImplementedError('the V-SkNN baseline (session_knn.py) is not implemented')
+            raise NotImplementedError("there is no 'vsknn' baseline: the session-based kNN baselines are named by the "
+                                      "reference's suffixes, 'v-sknn' (decay 'div') and 'sknn' (decay 'same')")
+        if name in KNN_SUFFIXES:
+            out[name] = _knn_params(name, params)
+            continue
         if name not in SUFFIXES:
-            raise ValueError('unknown baseline recommender %r (expected one of %s)' % (name, ', '.join(SUFFIXES)))
+            raise ValueError('unknown baseline recommender %r (expected one of %s)'
+                             % (name, ', '.join(SUFFIXES + KNN_SUFFIXES)))
         p = dict(DEFAULT_PARAMS[name])
         p.update({k: v for k, v in params.items() if k in p})
         if name == 'sr':
@@ -66,14 +76,19 @@ class BaselineTables:
         self.num_items = int(num_items)
         self.dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
         self.lib = _lib.load()
-        self.mask = sum(1 << SUFFIXES.index(s) for s in self.enabled)
+        self.mask = sum(1 << SUFFIXES.index(s) for s in self.enabled if s in SUFFIXES)
         self.uses_table = any(s in _TABLE_USERS for s in self.enabled)
+        # rows of the metrics accumulator: SUFFIXES, then KNN_SUFFIXES when a kNN baseline is enabled
+        self.n_rows = len(SUFFIXES) + (len(KNN_SUFFIXES) if any(s in KNN_SUFFIXES for s in self.enabled) else 0)
         sr = self.params.get('sr', DEFAULT_PARAMS['sr'])
         self.max_clicks_dist = int(sr['max_clicks_dist'])
         knn = self.params.get('item_knn', DEFAULT_PARAMS['item_knn'])
         self.reg_lambda, self.alpha = float(knn['reg_lambda']), float(knn['alpha'])
         d = self.dev
         self.err = torch.zeros(1, dtype=torch.int32, device=d)
+        self.knn = {s: SessionKNN(s, self.params[s], self.num_items, self.lib, d, self.err)
+                    for s in self.enabled if s in KNN_SUFFIXES}
+        self.trains = self.uses_table or bool(self.knn)           # some baseline learns from the training batches
         self.acr, self.acr_dim, self.acr_norm = None, int(acr_dim), None
         if 'cb' in self.enabled:
             if acr is None:
@@ -141,12 +156,16 @@ class BaselineTables:
 
     # ---- training: fold one batch
     def update(self, all_items: torch.Tensor, lens: Optional[Sequence[int]] = None, stream=None,
-               after: Optional[torch.cuda.Event] = None):
-        """Fold one batch (``all_items`` [Bg, T+1] int64 device = item_clicked | label_last_item) into the pair table on
-        ``stream`` (default: the current stream), after ``after``.  ``lens`` = the sessions' click counts (for the
-        growth bound; default T+1 each).  Queues work only: no host synchronisation."""
+               after: Optional[torch.cuda.Event] = None, session_ids=None):
+        """Fold one batch (``all_items`` [Bg, T+1] int64 device = item_clicked | label_last_item) into the pair table and
+        the kNN rings on ``stream`` (default: the current stream), after ``after``.  ``lens`` = the sessions' click counts
+        (for the growth bound; default T+1 each).  ``session_ids`` [Bg] (host array or tensor) is required when a kNN
+        baseline is enabled; host ids go up through a pinned copy on ``stream``.  Queues work only: no host
+        synchronisation."""
+        if self.knn and session_ids is None:
+            raise ValueError('the session kNN baselines (%s) need the batch\'s session ids' % ', '.join(self.knn))
         self.batch_seq += 1
-        if not self.uses_table:
+        if not self.trains:
             return
         s = torch.cuda.current_stream(self.dev) if stream is None else stream
         Bg, T1 = all_items.shape
@@ -154,6 +173,20 @@ class BaselineTables:
         if after is not None:
             s.wait_event(after)
         self._wait(s)
+        if self.knn:
+            if torch.is_tensor(session_ids) and session_ids.is_cuda:
+                sids = session_ids.to(self.dev, torch.int64).contiguous().view(-1)
+            else:
+                host = torch.as_tensor(np.ascontiguousarray(np.asarray(session_ids, dtype=np.int64).reshape(-1)))
+                with torch.cuda.stream(s):
+                    sids = host.pin_memory().to(self.dev, non_blocking=True)
+            sids.record_stream(s)
+            all_items.record_stream(s)
+            for ring in self.knn.values():
+                ring.update(all_items, sids, s)
+        if not self.uses_table:
+            self._mark(s)
+            return
         lens = np.full(Bg, T1, dtype=np.int64) if lens is None else np.asarray(lens, dtype=np.int64)
         pairs = int(np.sum(lens * (lens - 1)))
         bound = self._occupancy_bound() + pairs
@@ -182,15 +215,16 @@ class BaselineTables:
     def score(self, item_clicked: torch.Tensor, label_next: torch.Tensor, negatives: torch.Tensor, buffer_ids,
               articles_pop, top_n: int, metrics: torch.Tensor, out_ids: Optional[torch.Tensor] = None):
         """Rank label + negatives [B, T, K] of every query (label != 0) for every enabled baseline against the current
-        tables, ``buffer_ids`` (recent-clicks buffer) and ``articles_pop``; ``metrics`` [5, 3] fp64 device accumulator
-        (rows in SUFFIXES order) += {hits, sum of reciprocal ranks, queries}.  ``out_ids`` [5, B*T, top_n] int64: the
-        top-n ids per query (0-padded).  Runs on the current stream."""
+        tables, ``buffer_ids`` (recent-clicks buffer) and ``articles_pop``; ``metrics`` [n_rows, 3] fp64 device
+        accumulator (rows in SUFFIXES order, then KNN_SUFFIXES when a kNN baseline is enabled) += {hits, sum of
+        reciprocal ranks, queries}.  ``out_ids`` [n_rows, B*T, top_n] int64: the top-n ids per query (0-padded).  Runs on
+        the current stream."""
         s = torch.cuda.current_stream(self.dev)
         self._wait(s)
         d = self.dev
         B, T = item_clicked.shape
         K = negatives.shape[2] if negatives.dim() == 3 else 0
-        assert metrics.dtype == torch.float64 and metrics.numel() >= 15
+        assert metrics.dtype == torch.float64 and metrics.numel() >= 3 * self.n_rows
         ic = item_clicked.to(d, torch.int64).contiguous()
         ln = label_next.to(d, torch.int64).contiguous()
         ng = negatives.to(d, torch.int64).contiguous()
@@ -204,9 +238,15 @@ class BaselineTables:
         if 'item_knn' in self.enabled:
             pop = torch.as_tensor(np.asarray(articles_pop, dtype=np.int64) if not torch.is_tensor(articles_pop) else articles_pop)
             pop = pop.to(d, torch.int64).contiguous()
-        hist = torch.empty(5 * (top_n + 1), dtype=torch.int64, device=d)
         if out_ids is not None:
-            assert out_ids.dtype == torch.int64 and out_ids.shape == (5, B * T, top_n) and out_ids.is_contiguous()
+            assert out_ids.dtype == torch.int64 and out_ids.shape == (self.n_rows, B * T, top_n) and out_ids.is_contiguous()
+        for sfx, ring in self.knn.items():
+            row = len(SUFFIXES) + KNN_SUFFIXES.index(sfx)
+            ring.score(ic, ln, ng, B, T, K, top_n, metrics.view(-1)[3 * row:3 * row + 3],
+                       None if out_ids is None else out_ids[row], s)
+        if not self.mask:
+            return
+        hist = torch.empty(5 * (top_n + 1), dtype=torch.int64, device=d)
         check(self.lib.nar_baselines_score(
             *[_p(x) for x in self._tables()], self.cap, _p(ic), _p(ln), _p(ng), B, T, K,
             _p(getattr(self, 'hist_count', None)), _p(getattr(self, 'hist_first', None)), _p(pop), _p(self.acr),
@@ -215,11 +255,11 @@ class BaselineTables:
             'nar_baselines_score')
 
     def results(self, metrics: torch.Tensor) -> Dict[str, float]:
-        """{'hitrate_at_n_<suffix>', 'mrr_at_n_<suffix>'} of the enabled baselines from a [5, 3] accumulator."""
-        m = metrics.view(5, 3).cpu().numpy()
+        """{'hitrate_at_n_<suffix>', 'mrr_at_n_<suffix>'} of the enabled baselines from an [n_rows, 3] accumulator."""
+        m = metrics.view(-1, 3).cpu().numpy()
         out = {}
         for sfx in self.enabled:
-            h, rr, cnt = m[SUFFIXES.index(sfx)]
+            h, rr, cnt = m[SUFFIXES.index(sfx) if sfx in SUFFIXES else len(SUFFIXES) + KNN_SUFFIXES.index(sfx)]
             cnt = max(float(cnt), 1.0)
             out['hitrate_at_n_%s' % sfx] = float(h) / cnt
             out['mrr_at_n_%s' % sfx] = float(rr) / cnt
@@ -231,6 +271,8 @@ class BaselineTables:
         self._wait(s)
         self._chk = ([x.clone() for x in self._tables()], self.count.clone(), self.cap, self.batch_seq, self._occ,
                      self._pairs_since, list(self._pending))
+        for ring in self.knn.values():
+            ring.snapshot()
 
     def restore(self):
         s = torch.cuda.current_stream(self.dev)
@@ -239,10 +281,14 @@ class BaselineTables:
         del self._chk
         self.keys, self.cooc, self.sr_w, self.sr_first = tabs
         self.count = cnt
+        for ring in self.knn.values():
+            ring.restore()
         self._ready = None
 
     def clear(self):
         self.batch_seq = 0
+        for ring in self.knn.values():
+            ring.clear()
         self._alloc(self.cap, torch.cuda.current_stream(self.dev))
 
     # ---- export / load (checkpoints, tests): occupied entries sorted by key
@@ -263,8 +309,23 @@ class BaselineTables:
         vals = {n: t[occ][order].cpu().numpy() for n, t in (('cooc', self.cooc), ('sr_w', self.sr_w), ('sr_first', self.sr_first))}
         return {'keys': keys.cpu().numpy(), **vals, 'batch_seq': np.asarray(self.batch_seq, dtype=np.int64)}
 
+    def export_knn(self, suffix: str) -> Dict[str, np.ndarray]:
+        """The ring of kNN ``suffix`` in insertion order: ids [n], lens [n], items [n, W] (sorted sets, 0-padded), live
+        [n, W] (the pair (item, session id) is in the reference's item -> sessions map)."""
+        s = torch.cuda.current_stream(self.dev)
+        self._wait(s)
+        self.check_errors()
+        return self.knn[suffix].export()
+
     def load(self, arrays: Dict[str, np.ndarray]):
-        """Replace the tables by exported ones."""
+        """Replace the tables by exported ones (a kNN ring without saved arrays starts empty)."""
+        if self.knn:
+            s = torch.cuda.current_stream(self.dev)
+            self._wait(s)
+            for sfx, ring in self.knn.items():
+                pre = 'sknn_%s_' % sfx
+                ring.load({k[len(pre):]: v for k, v in arrays.items() if k.startswith(pre)})
+            self._mark(s)
         if 'keys' not in arrays:
             self.batch_seq = int(arrays.get('batch_seq', 0))
             return
@@ -288,4 +349,7 @@ class BaselineTables:
         self._mark(s)
 
     def state_arrays(self) -> Dict[str, np.ndarray]:
-        return self.export() if self.uses_table else {'batch_seq': np.asarray(self.batch_seq, dtype=np.int64)}
+        out = self.export() if self.uses_table else {'batch_seq': np.asarray(self.batch_seq, dtype=np.int64)}
+        for sfx in self.knn:
+            out.update({'sknn_%s_%s' % (sfx, k): v for k, v in self.export_knn(sfx).items()})
+        return out

@@ -10,7 +10,9 @@ split across ``train`` / ``evaluate`` calls.  TF's bundle format is not reproduc
 * ``state/*`` - the host-side ``ClickedItemsState`` (recent-clicks buffer, popularity counters) when given; the
   reference keeps that object alive in the trainer process instead (nar_trainer_gcom.py:486-489),
 * ``baselines/*`` - the baseline recommenders' pair table (``baselines.BaselineTables.export``: occupied entries
-  sorted by key, value arrays alongside) when the state holds one.  Checkpoints without it load as before.
+  sorted by key, value arrays alongside) when the state holds one, and the session kNN rings under
+  ``baselines/sknn_<suffix>_*`` (ids, lens, items, live in insertion order).  Checkpoints without them load as before
+  (a kNN ring without saved arrays starts empty).
 """
 from __future__ import annotations
 

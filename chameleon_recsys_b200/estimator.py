@@ -192,17 +192,19 @@ class Estimator:
             feed = feed_of(spec)
             st_next = eng.stage_ahead(nxt[0], nxt[1], feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], 'pipe0')
         pending = None                                              # (features, labels, out) of the step whose loss is unread
-        # baseline recommenders (nar_model.py:1641-1646): every batch is folded into their tables on the side stream,
-        # behind the batch's copy; the main stream's work is unchanged
+        # baseline recommenders (nar_model.py:1641-1646): every batch is folded into their tables (and the session kNN
+        # rings, with the batch's session ids) on the side stream, behind the batch's copy; the main stream's work is
+        # unchanged
         tables = getattr(self._state(), 'baselines', None)
-        if tables is not None and not tables.uses_table:
+        if tables is not None and not tables.trains:
             tables = None
 
         def fold(st):
             if tables is not None and st['has_clicks']:
                 import torch
                 side = eng.side_stream() if eng.use_side_stream else torch.cuda.current_stream()
-                tables.update(st['t']['all_items'], lens=st['fold_lens'], stream=side, after=st.get('copied'))
+                tables.update(st['t']['all_items'], lens=st['fold_lens'], stream=side, after=st.get('copied'),
+                              session_ids=st['fold_sids'])
 
         def finish(p):
             f_, l_, o_ = p
@@ -215,6 +217,7 @@ class Estimator:
             features, labels = nxt
             if tables is not None:
                 st_next['fold_lens'] = _session_clicks(features, labels)
+                st_next['fold_sids'] = features.get('session_id')
             out = eng.submit(st_next)                               # step n queued on the main stream
             if not use_ds:
                 fold(st_next)
@@ -365,7 +368,7 @@ class Estimator:
             out = update(features, labels, feed, metrics, step_id=n + 1)
             run_values = {'clicked_items': features['item_clicked'], 'clicked_timestamps': features['event_timestamp'],
                           'last_item_label': labels['label_last_item'], 'stage': out['stage'],
-                          'eval_batch_negative_items': out['negatives']}
+                          'eval_batch_negative_items': out['negatives'], 'session_ids': features.get('session_id')}
             for h in spec.evaluation_hooks:
                 h.after_run(None, run_values)
             loss_sum += out['total_loss']

@@ -142,7 +142,8 @@ class NARHParams:
     sampler_seed: int = 42           # RANDOM_SEED, nar_trainer_gcom.py:33
     init_seed: int = 42
     # baseline recommenders evaluated next to the model (nar_trainer_gcom.py:280-300): suffixes or
-    # {'recommender': <suffix>, 'params': {...}} of 'pop_recent', 'coocurrent', 'item_knn', 'cb', 'sr' (baselines.py)
+    # {'recommender': <suffix>, 'params': {...}} of 'pop_recent', 'coocurrent', 'item_knn', 'cb', 'sr', and the session
+    # kNN baselines 'v-sknn' / 'sknn' (baselines.py, sknn.py; they need the batches' 'session_id' feature)
     eval_benchmarks: tuple = ()
 
     def to_params(self, session_features_config, articles_features_config, articles_metadata,

@@ -184,7 +184,7 @@ class ItemsStateUpdaterHook:
             self.clicked_items_state.save_state_checkpoint()        # nar_model.py:1415
             if self.baselines is not None:
                 import torch
-                self.bench_metrics = torch.zeros(5, 3, dtype=torch.float64, device=self.model.engine.dev)
+                self.bench_metrics = torch.zeros(self.baselines.n_rows, 3, dtype=torch.float64, device=self.model.engine.dev)
 
     def before_run(self, run_context=None) -> dict:
         """-> feed dict (nar_model.py:1458-1467)."""
@@ -193,8 +193,9 @@ class ItemsStateUpdaterHook:
 
     def after_run(self, run_context, run_values: dict):
         """run_values: {'clicked_items','clicked_timestamps','last_item_label'} (nar_model.py:1505-1508).  In EVAL with
-        baselines enabled also 'stage' (the staged batch of the step) and 'eval_batch_negative_items' ([B,T,K] device):
-        the baselines rank the batch against the state BEFORE it, then learn from it (nar_model.py:1609-1632)."""
+        baselines enabled also 'stage' (the staged batch of the step), 'eval_batch_negative_items' ([B,T,K] device) and
+        'session_ids' ([B], needed by the session kNN baselines): the baselines rank the batch against the state BEFORE
+        it, then learn from it (nar_model.py:1609-1632)."""
         if self.baselines is not None and self.mode == ModeKeys.EVAL:
             t = run_values['stage']['t']
             self.baselines.score(t['item_clicked'], t['label_next'], run_values['eval_batch_negative_items'],
@@ -202,7 +203,8 @@ class ItemsStateUpdaterHook:
                                  self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n, self.bench_metrics)
             if run_values['stage']['has_clicks']:
                 self.baselines.update(t['all_items'], lens=np.count_nonzero(np.concatenate(
-                    [run_values['clicked_items'], np.asarray(run_values['last_item_label']).reshape(-1, 1)], axis=1), axis=1))
+                    [run_values['clicked_items'], np.asarray(run_values['last_item_label']).reshape(-1, 1)], axis=1), axis=1),
+                    session_ids=run_values.get('session_ids'))
         self.clicked_items_state.update_from_batch(run_values['clicked_items'], run_values['clicked_timestamps'],
                                                    run_values['last_item_label'])
 

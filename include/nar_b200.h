@@ -477,6 +477,26 @@ int nar_baselines_score(const int64_t* keys, const int64_t* cooc, const int64_t*
                         const double* acr_norm, int64_t num_items, double knn_lambda, double knn_alpha, int32_t enabled,
                         int32_t top_n, int64_t* rank_hist, double* metrics, int64_t* out_ids, int* err, void* stream);
 
+/* ---- session-based kNN baseline, V-SkNN / SkNN (csrc/sknn.cu, spec oracle/sknn_ref.py) -------------------------------
+ * Ring of S slots (logical index i at slot (head + i) % S, count entries, oldest first; head and count are the caller's):
+ * ids [S] session id, lens [S], items [S, W] int32 sorted item set, +x while (x, id) is in the item -> sessions map and
+ * -x once an eviction discarded it.  nar_sknn_update appends one batch (all_items [B, T1], 0 = padding; session_ids [B]),
+ * then evicts the max(0, count + B - S) oldest entries; st_* [S] / [S, W] are staging scratch.  Requires B <= S,
+ * T1 <= W <= 128.  Afterwards head += evicted (mod S), count += B - evicted.  *err = 1 for an id outside [0, num_items). */
+int nar_sknn_update(int64_t* ids, int32_t* lens, int32_t* items, int64_t S, int64_t W, int64_t head, int64_t count,
+                    int64_t* st_ids, int32_t* st_lens, int32_t* st_items, const int64_t* all_items,
+                    const int64_t* session_ids, int64_t B, int64_t T1, int64_t num_items, int* err, void* stream);
+/* Ranks label + negatives [B, T, K] of every query (b, t) with label_next != 0 by the kNN item scores of the active
+ * session item_clicked[b, :t+1] (sample_size 0 = no 'recent' cut; decay_div 1 = 'div', 0 = 'same'; jaccard 1 = jaccard,
+ * 0 = cosine).  metrics [3] fp64 += {hits, sum of reciprocal ranks, queries} (rank_hist [top_n + 1] int64 is scratch);
+ * out_ids [B*T, top_n] (optional) = the top-n ids of each query, 0-padded.  NAR_ERR_UNSUPPORTED for S > 4096, T > 64
+ * or K + 1 > 1024.                                                                                                     */
+int nar_sknn_score(const int64_t* ids, const int32_t* lens, const int32_t* items, int64_t S, int64_t W, int64_t head,
+                   int64_t count, const int64_t* item_clicked, const int64_t* label_next, const int64_t* negatives,
+                   int64_t B, int64_t T, int64_t K, int64_t num_items, int64_t sample_size, int64_t nn, int32_t decay_div,
+                   int32_t jaccard, int32_t top_n, int64_t* rank_hist, double* metrics, int64_t* out_ids, int* err,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif
