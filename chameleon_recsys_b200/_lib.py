@@ -159,6 +159,11 @@ _SIGNATURES = {
     'nar_sknn_update': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, i64, i64, i64, vp, vp]),
     'nar_sknn_score': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, i64, i64, i64, i64, i64, i64, i32, i32, i32,
                                  vp, vp, vp, vp, vp]),
+    'nar_eval_metrics_mark': (C.c_int, [vp, i64, i64, i32, vp, vp, vp]),
+    'nar_eval_metrics_lists': (C.c_int, [vp, i64, i64, i64, i64, i64, i64, i32, vp, i64, vp, vp, i64, i64, vp, i64,
+                                         C.c_double, vp, vp, vp, vp]),
+    'nar_eval_metrics_reduce': (C.c_int, [vp, i64, i64, i64, vp, vp]),
+    'nar_eval_metrics_popcount': (C.c_int, [vp, i64, i64, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = sorted(_SIGNATURES.keys())

@@ -254,12 +254,17 @@ class BaselineTables:
             self.alpha, self.mask, int(top_n), _p(hist), _p(metrics), _p(out_ids), _p(self.err), stream),
             'nar_baselines_score')
 
+    @staticmethod
+    def row(sfx: str) -> int:
+        """Row of baseline ``sfx`` in the metrics accumulator and in ``out_ids``."""
+        return SUFFIXES.index(sfx) if sfx in SUFFIXES else len(SUFFIXES) + KNN_SUFFIXES.index(sfx)
+
     def results(self, metrics: torch.Tensor) -> Dict[str, float]:
         """{'hitrate_at_n_<suffix>', 'mrr_at_n_<suffix>'} of the enabled baselines from an [n_rows, 3] accumulator."""
         m = metrics.view(-1, 3).cpu().numpy()
         out = {}
         for sfx in self.enabled:
-            h, rr, cnt = m[SUFFIXES.index(sfx) if sfx in SUFFIXES else len(SUFFIXES) + KNN_SUFFIXES.index(sfx)]
+            h, rr, cnt = m[self.row(sfx)]
             cnt = max(float(cnt), 1.0)
             out['hitrate_at_n_%s' % sfx] = float(h) / cnt
             out['mrr_at_n_%s' % sfx] = float(rr) / cnt

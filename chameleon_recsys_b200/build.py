@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnar_b200.so')
 SOURCES = ['gemm_wgmma.cu', 'features.cu', 'sampler.cu', 'rnn.cu', 'loss.cu', 'misc.cu', 'host_state.cu', 'state.cu', 'car.cu',
-           'gru.cu', 'recommend.cu', 'engine.cu', 'baselines.cu', 'sknn.cu']
+           'gru.cu', 'recommend.cu', 'engine.cu', 'baselines.cu', 'sknn.cu',
+           'eval_metrics.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-diag-suppress', '128',
               '-Xcompiler', '-fPIC']
 

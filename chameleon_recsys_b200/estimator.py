@@ -93,7 +93,9 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
                                    eval_sessions_metrics_log=eval_sessions_metrics_log,
                                    content_article_embeddings_matrix=params['content_article_embeddings_matrix'],
                                    articles_metadata=params['articles_metadata'],
-                                   eval_benchmark_classifiers=params.get('eval_benchmarks') or ())]
+                                   eval_negative_sample_relevance=params.get('eval_negative_sample_relevance'),
+                                   eval_benchmark_classifiers=params.get('eval_benchmarks') or (),
+                                   eval_extended_metrics=bool(params.get('eval_extended_metrics', False)))]
     if mode == ModeKeys.TRAIN:
         def train_op(feats, labs, feed, sync=True):
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
@@ -337,7 +339,9 @@ class Estimator:
         """tf.estimator.Estimator.evaluate: runs the EVAL graph over ``input_fn`` with the current weights and returns
         ``{'loss', 'hitrate_at_n', 'mrr_at_n', 'global_step'}`` (streaming means over all valid labels, nar_model.py:
         835-885; ``loss`` = mean of the per-batch total_loss like Estimator does).  The hook snapshots ClickedItemsState at
-        ``begin`` and restores it at ``end`` (nar_model.py:1415, :1693), and keeps updating it batch by batch in between."""
+        ``begin`` and restores it at ``end`` (nar_model.py:1415, :1693), and keeps updating it batch by batch in between.
+        With ``eval_extended_metrics`` also ``ndcg_at_n``, ``item_coverage_at_n``, ``esi-r_at_n``, ``esi-rr_at_n``,
+        ``content_eild-r_at_n`` and ``content_eild-rr_at_n``, and each as ``<key>_<suffix>`` for every baseline."""
         import torch
         it = input_fn()
 
@@ -349,8 +353,14 @@ class Estimator:
 
         nxt = fetch() if (steps is None or steps > 0) else None
         if nxt is None:
-            return {'loss': float('nan'), 'hitrate_at_n': float('nan'), 'mrr_at_n': float('nan'),
-                    'global_step': 0 if self._spec is None else self._spec.model.global_step()}
+            empty = {'loss': float('nan'), 'hitrate_at_n': float('nan'), 'mrr_at_n': float('nan'),
+                     'global_step': 0 if self._spec is None else self._spec.model.global_step()}
+            if self.params.get('eval_extended_metrics'):
+                from .baselines import parse_classifiers
+                from .eval_metrics import metric_names
+                for s in [''] + list(parse_classifiers(self.params.get('eval_benchmarks') or ())):
+                    empty.update({k: float('nan') for k in metric_names(s)})
+            return empty
         if self._eval_spec is None:
             self._eval_spec = self.model_fn(nxt[0], nxt[1], ModeKeys.EVAL, self.params)
         spec = self._eval_spec
@@ -368,7 +378,8 @@ class Estimator:
             out = update(features, labels, feed, metrics, step_id=n + 1)
             run_values = {'clicked_items': features['item_clicked'], 'clicked_timestamps': features['event_timestamp'],
                           'last_item_label': labels['label_last_item'], 'stage': out['stage'],
-                          'eval_batch_negative_items': out['negatives'], 'session_ids': features.get('session_id')}
+                          'eval_batch_negative_items': out['negatives'], 'session_ids': features.get('session_id'),
+                          'predicted_item_ids': out.get('predicted_item_ids')}
             for h in spec.evaluation_hooks:
                 h.after_run(None, run_values)
             loss_sum += out['total_loss']
@@ -377,6 +388,7 @@ class Estimator:
         bench = {}
         for h in spec.evaluation_hooks:
             bench.update(h.benchmark_results())
+            bench.update(h.extended_results())
             h.end()
         eng = spec.model.engine
         if eng.world > 1:                                           # data parallel: every rank ranked its own sessions

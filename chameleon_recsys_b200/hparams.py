@@ -145,6 +145,9 @@ class NARHParams:
     # {'recommender': <suffix>, 'params': {...}} of 'pop_recent', 'coocurrent', 'item_knn', 'cb', 'sr', and the session
     # kNN baselines 'v-sknn' / 'sknn' (baselines.py, sknn.py; they need the batches' 'session_id' feature)
     eval_benchmarks: tuple = ()
+    # NDCG, item coverage, ESI-R / ESI-RR and EILD-R / EILD-RR of the model and every baseline in Estimator.evaluate
+    # (the reference hook's create_eval_metrics; eval_metrics.py)
+    eval_extended_metrics: bool = False
 
     def to_params(self, session_features_config, articles_features_config, articles_metadata,
                   content_article_embeddings_matrix) -> dict:
@@ -188,6 +191,8 @@ class NARHParams:
         }
         if self.eval_benchmarks:                 # the key exists only when baselines are requested
             params['eval_benchmarks'] = list(self.eval_benchmarks)
+        if self.eval_extended_metrics:           # likewise only when requested
+            params['eval_extended_metrics'] = True
         return params
 
     def copy(self, **kw) -> 'NARHParams':

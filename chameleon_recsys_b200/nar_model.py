@@ -153,12 +153,23 @@ class ItemsStateUpdaterHook:
                  eval_sessions_metrics_log=None, sessions_negative_items_log=None,
                  sessions_chameleon_recommendations_log=None, content_article_embeddings_matrix=None,
                  articles_metadata=None, eval_negative_sample_relevance=None, eval_benchmark_classifiers=(),
-                 eval_metrics_by_session_position=False, eval_cold_start=False):
+                 eval_metrics_by_session_position=False, eval_cold_start=False, eval_extended_metrics=False):
         self.mode = mode
         self.model = model
         self.eval_metrics_top_n = eval_metrics_top_n
         self.clicked_items_state = clicked_items_state
         self.eval_sessions_metrics_log = eval_sessions_metrics_log
+        # NDCG, coverage, novelty and diversity of the model and every baseline (create_eval_metrics, nar_model.py:
+        # 1696-1721): an eval_metrics.EvalMetrics accumulator, row 0 the model, rows 1.. the baselines' rows
+        self.eval_negative_sample_relevance = eval_negative_sample_relevance
+        self.extended_metrics = eval_extended_metrics and mode == ModeKeys.EVAL
+        self.extended = None
+        if self.extended_metrics:
+            from .eval_metrics import check_params
+            if model.engine.world > 1:
+                raise NotImplementedError('the extended evaluation metrics run on one process; data-parallel evaluation '
+                                          'of them is not implemented')
+            check_params(eval_metrics_top_n, eval_negative_sample_relevance)
         # baseline recommenders (nar_model.py:1399-1407): [{'recommender': <suffix>, 'params': {...}}]; their state is the
         # BaselineTables object on the ClickedItemsState, shared by the TRAIN and EVAL hooks
         self.bench_metrics = None
@@ -185,6 +196,15 @@ class ItemsStateUpdaterHook:
             if self.baselines is not None:
                 import torch
                 self.bench_metrics = torch.zeros(self.baselines.n_rows, 3, dtype=torch.float64, device=self.model.engine.dev)
+            if self.extended_metrics:
+                if self.extended is None:
+                    from .eval_metrics import EvalMetrics
+                    eng, tables = self.model.engine, self.baselines
+                    self.extended = EvalMetrics(1 + (tables.n_rows if tables is not None else 0),
+                                                self.clicked_items_state.num_items, eng.acr, self.model.plan.acr_dim,
+                                                self.eval_metrics_top_n, self.eval_negative_sample_relevance,
+                                                acr_norm=None if tables is None else tables.acr_norm)
+                self.extended.begin(self.clicked_items_state.get_recent_clicks_buffer())
 
     def before_run(self, run_context=None) -> dict:
         """-> feed dict (nar_model.py:1458-1467)."""
@@ -195,16 +215,39 @@ class ItemsStateUpdaterHook:
         """run_values: {'clicked_items','clicked_timestamps','last_item_label'} (nar_model.py:1505-1508).  In EVAL with
         baselines enabled also 'stage' (the staged batch of the step), 'eval_batch_negative_items' ([B,T,K] device) and
         'session_ids' ([B], needed by the session kNN baselines): the baselines rank the batch against the state BEFORE
-        it, then learn from it (nar_model.py:1609-1632)."""
+        it, then learn from it (nar_model.py:1609-1632).  With the extended metrics on also 'predicted_item_ids' (the
+        model's ranked candidates [L, 1+K] on the device, None without queries): the model's and the baselines' top-n
+        lists are measured with the popularity the batch was fed with, before the state learns from the batch
+        (:1591-1603)."""
+        ext = self.extended                                 # set in EVAL only
+        if ext is not None:
+            st = run_values['stage']
+            pred = run_values.get('predicted_item_ids')
+            if pred is not None:
+                # each query's label is column 0 of the candidate ids the ranking read
+                cand = self.model.engine.buffer(st, 'row_item').view(-1)[st['L']:]
+                ext.add_lists(pred, cand, st['t']['pop_norm'], label_stride=pred.shape[1])
         if self.baselines is not None and self.mode == ModeKeys.EVAL:
             t = run_values['stage']['t']
+            out_ids = None
+            if ext is not None:
+                import torch
+                out_ids = torch.empty(self.baselines.n_rows, t['label_next'].numel(), self.eval_metrics_top_n,
+                                      dtype=torch.int64, device=self.model.engine.dev)
             self.baselines.score(t['item_clicked'], t['label_next'], run_values['eval_batch_negative_items'],
                                  self.clicked_items_state.get_recent_clicks_buffer(),
-                                 self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n, self.bench_metrics)
+                                 self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n, self.bench_metrics,
+                                 out_ids=out_ids)
+            if ext is not None:
+                ext.add_lists(out_ids, t['label_next'].view(-1), t['pop_norm'], row0=1,
+                              row_mask=sum(1 << self.baselines.row(s) for s in self.baselines.enabled))
             if run_values['stage']['has_clicks']:
                 self.baselines.update(t['all_items'], lens=np.count_nonzero(np.concatenate(
                     [run_values['clicked_items'], np.asarray(run_values['last_item_label']).reshape(-1, 1)], axis=1), axis=1),
                     session_ids=run_values.get('session_ids'))
+        if ext is not None:
+            t = run_values['stage']['t']
+            ext.add_clicks(t['item_clicked'], t['label_next'])
         self.clicked_items_state.update_from_batch(run_values['clicked_items'], run_values['clicked_timestamps'],
                                                    run_values['last_item_label'])
 
@@ -213,6 +256,17 @@ class ItemsStateUpdaterHook:
         if self.baselines is None or self.bench_metrics is None:
             return {}
         return self.baselines.results(self.bench_metrics)
+
+    def extended_results(self) -> dict:
+        """The extended metrics of this evaluation ({} with them off): the model's keys without a suffix, each baseline's
+        as ``<key>_<suffix>``."""
+        if self.extended is None:
+            return {}
+        from .eval_metrics import KEYS, COVERAGE_KEY
+        rows = self.extended.results()
+        named = [('', rows[0])] + ([(s, rows[1 + self.baselines.row(s)]) for s in self.baselines.enabled]
+                                   if self.baselines is not None else [])
+        return {k + ('_' + s if s else ''): r[k] for s, r in named for k in KEYS + (COVERAGE_KEY,)}
 
     def end(self, session=None):
         if self.mode == ModeKeys.EVAL:

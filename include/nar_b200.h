@@ -497,6 +497,28 @@ int nar_sknn_score(const int64_t* ids, const int32_t* lens, const int32_t* items
                    int32_t jaccard, int32_t top_n, int64_t* rank_hist, double* metrics, int64_t* out_ids, int* err,
                    void* stream);
 
+/* ---- NDCG, item coverage, ESI-R / ESI-RR and EILD-R / EILD-RR of top-n lists (csrc/eval_metrics.cu, spec
+ *      oracle/eval_metrics_ref.py; the reference's metrics.py).  Coverage sets are bitmaps of (num_items + 31) / 32
+ *      uint32 words.  *err = 1 for an id outside [0, num_items).                                                     */
+/* sets the bit of every id of ids [n] (zeros skipped when skip_zero) */
+int nar_eval_metrics_mark(const int64_t* ids, int64_t n, int64_t num_items, int32_t skip_zero, uint32_t* bitmap, int* err,
+                          void* stream);
+/* For every recommender row r < rows with bit r of row_mask set and every query q < nq whose label
+ * labels[q * label_stride] is nonzero: the list ids[r * row_stride + q * q_stride + j], j < len, scored over its first
+ * m = min(top_n, len) ids (2 <= m <= 64); NDCG counts the label's occurrences over all len.  pop [num_items] float32
+ * normalised recent popularity; acr [num_items, acr_ld] float32 (first acr_dim columns) with fp64 row norms acr_norm.
+ * per_query [rows, nq, 6] fp64 = {ndcg, esi-r, esi-rr, eild-r, eild-rr, 1} (zeros for label 0); the ids go into the
+ * row's bitmap rec_bitmaps[r].                                                                                        */
+int nar_eval_metrics_lists(const int64_t* ids, int64_t row_stride, int64_t q_stride, int64_t rows, int64_t row_mask,
+                           int64_t nq, int64_t len, int32_t top_n, const int64_t* labels, int64_t label_stride,
+                           const float* pop, const float* acr, int64_t acr_dim, int64_t acr_ld, const double* acr_norm,
+                           int64_t num_items, double neg_relevance, double* per_query, uint32_t* rec_bitmaps, int* err,
+                           void* stream);
+/* acc [rows, 6] fp64 += the sum over q of per_query [rows, nq, 6], for the rows of row_mask, in a fixed order */
+int nar_eval_metrics_reduce(const double* per_query, int64_t rows, int64_t row_mask, int64_t nq, double* acc, void* stream);
+/* counts [n_maps] int64 = set bits of each of the bitmaps [n_maps, words] */
+int nar_eval_metrics_popcount(const uint32_t* bitmaps, int64_t n_maps, int64_t words, int64_t* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
