@@ -10,14 +10,15 @@
 //   wgrad dW = X^T * dY      A = X  (MN-major)  B = dY  (MN-major), split-K + red.add
 //
 // CTA = 256 threads = two warpgroups, one 128 x 128 output tile, k-tiles of 32 (32 fp32 = one 128-byte swizzle row);
-// two CTAs per SM when B needs no transpose / split pass (see Cfg), else one:
+// two CTAs per SM unless B needs separate 3xTF32 split tiles (see Cfg), else one:
 //   thread 0     keeps STAGES - 1 k-tiles of A and B ahead of the one being multiplied (cp.async.bulk.tensor.2d,
 //                128-byte swizzle, one mbarrier per stage) and refills a stage as soon as its MMAs are done;
 //   warpgroup w  multiplies rows [64w, 64w + 64) of the tile with wgmma.m64n128: A from registers, B from shared
 //                memory.  A is read from the swizzled TMA tile straight into the register fragment whatever its major,
 //                and that is also where 3xTF32 splits it.  wgmma reads 32-bit B operands only K-major, so a B tile that
 //                arrives MN-major (the forward weights W [in,out], the wgrad dY) is first transposed in shared memory
-//                by all 256 threads; the same pass writes B's lo part for 3xTF32.
+//                by all 256 threads: in place for single-pass TF32, into separate tiles for 3xTF32, where the same
+//                pass writes B's lo part.
 //   epilogue     accumulators -> shared memory -> row-contiguous bias / activation / activation-derivative and
 //                st.global.v4, or red.global.add.v4 for split-K.
 //
@@ -49,12 +50,14 @@ template <int MODE, bool B_MN> struct Cfg {
   static constexpr bool SPLIT3 = MODE == 1 || MODE == 2;
   static constexpr bool BLO = MODE == 2;
   static constexpr bool PREP = B_MN || SPLIT3;                        // B goes through the transpose / split pass
+  // MODE 0 transposes an MN-major B within its own stage (prep_b); only the 3xTF32 split writes separate prep tiles
+  static constexpr bool PREP_TILES = SPLIT3;
   static constexpr int STAGE_BYTES = TILE_BYTES * (BLO ? 3 : 2);      // A | B [| B_lo]
-  // Without a prep pass two CTAs share an SM (3 stages = 96 KB each, <= 128 registers per thread), so that one CTA's
-  // epilogue runs under the other's main loop; with one, the prep tiles leave room for one CTA.
-  static constexpr int CTAS_PER_SM = PREP ? 1 : 2;
-  static constexpr int STAGES = (BLO || !PREP) ? 3 : 4;
-  static constexpr int PREP_TILE_BYTES = PREP ? TILE_BYTES * (SPLIT3 ? 2 : 1) : 0;   // K-major B_hi [| B_lo]
+  // Without prep tiles two CTAs share an SM (3 stages = 96 KB each, <= 128 registers per thread), so that one CTA's
+  // epilogue runs under the other's main loop; with them, there is room for one CTA.
+  static constexpr int CTAS_PER_SM = PREP_TILES ? 1 : 2;
+  static constexpr int STAGES = (BLO || !PREP_TILES) ? 3 : 4;
+  static constexpr int PREP_TILE_BYTES = PREP_TILES ? TILE_BYTES * 2 : 0;   // K-major B_hi | B_lo
   static constexpr int PREP_BYTES = 2 * PREP_TILE_BYTES;             // double-buffered: k-tile kt uses buffer kt & 1
   static constexpr int BAR_OFF = STAGES * STAGE_BYTES + PREP_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;              // + barriers + alignment slack
@@ -190,19 +193,24 @@ __device__ __forceinline__ uint32_t tile_off(int mn, int k) {
                   : (uint32_t)(mn * 128 + (((k >> 2) ^ (mn & 7)) << 4) + (k & 3) * 4);
 }
 
-// B tile of the current stage -> K-major swizzled B_hi [| B_lo] tiles that wgmma reads.
+// B tile of the current stage -> K-major swizzled B_hi [| B_lo] tiles that wgmma reads.  MODE 0 passes hi_out == b and
+// transposes in place.
 template <bool B_MN, int MODE>
 __device__ __forceinline__ void prep_b(const uint8_t* b, const uint8_t* blo, uint8_t* hi_out, uint8_t* lo_out, int tid) {
   constexpr bool SPLIT3 = MODE == 1 || MODE == 2;
   if (B_MN) {
     // thread = a block of 4 n x 4 k: four 16-byte reads along n (one per k), four 16-byte writes along k (one per n);
-    // both sides are 8 distinct 16-byte chunks per 8 lanes, i.e. free of bank conflicts
+    // both sides are 8 distinct 16-byte chunks per 8 lanes, i.e. free of bank conflicts.  Box `box` (n in
+    // [32 box, 32 box + 32)) is the same 4096 bytes in both layouts and only warps 2 box and 2 box + 1 touch it.
     const int c = tid & 7, kq = (tid >> 3) & 7, box = tid >> 6;
+    // k = 4 kq + i and n = 32 box + 4 c + q have (k & 7) = 4 (kq & 1) ^ i and (n & 7) = 4 (c & 1) ^ q, so each side is
+    // one base offset with i (q) XORed into the chunk and added to the row: two live registers instead of eight
+    const uint32_t rd = (uint32_t)(box * 4096 + kq * 512 + ((c ^ ((kq & 1) << 2)) << 4));
+    const uint32_t wr = (uint32_t)(box * 4096 + c * 512 + ((kq ^ ((c & 1) << 2)) << 4));
     float v[4][4], l[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int k = 4 * kq + i;
-      const uint32_t off = (uint32_t)(box * 4096 + k * 128 + ((c ^ (k & 7)) << 4));
+      const uint32_t off = (rd ^ (i << 4)) + i * 128;
       const float4 x = *reinterpret_cast<const float4*>(b + off);
       v[i][0] = x.x; v[i][1] = x.y; v[i][2] = x.z; v[i][3] = x.w;
       if (MODE == 2) {
@@ -210,10 +218,16 @@ __device__ __forceinline__ void prep_b(const uint8_t* b, const uint8_t* blo, uin
         l[i][0] = y.x; l[i][1] = y.y; l[i][2] = y.z; l[i][3] = y.w;
       }
     }
+    // in place: the box's two warps have read all of it before either overwrites it.  Warpgroup w (boxes 2w, 2w + 1)
+    // meets at named barrier 1 + w; immediate ids, so that ptxas reserves 3 barriers rather than all 16, and a per-box
+    // barrier (a 4-way branch) costs spills at 128 registers.
+    if (!SPLIT3) {
+      if (tid < 128) asm volatile("bar.sync 1, 128;" ::: "memory");
+      else asm volatile("bar.sync 2, 128;" ::: "memory");
+    }
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const int n = box * 32 + 4 * c + q;
-      const uint32_t off = (uint32_t)(n * 128 + ((kq ^ (n & 7)) << 4));
+      const uint32_t off = (wr ^ (q << 4)) + q * 128;
       float4 h = make_float4(v[0][q], v[1][q], v[2][q], v[3][q]);
       if (SPLIT3) {
         const float4 x = h;
@@ -342,6 +356,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   // whose last readers (the MMAs of kt - 2) are complete after the wait_group 1 of kt - 1
   uint32_t a[2][4][4], alo[2][4][4];      // tf32: hi (or the single-pass value) | lo (3xTF32)
   uint32_t ahi16[2][2][4], alo16[2][2][4];  // bf16x3: A_hi | A_lo pairs
+  // tf32 A fragment q of k-step j is at a_off[q] + 1024 j (MN-major: 8 k-rows on) or a_off[q] ^ 32 j (K-major: the
+  // 16-byte chunk index (2 j + q / 2) ^ (row & 7) is chunk (q / 2) ^ (row & 7) with 2 j XORed in)
+  uint32_t a_off[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) a_off[q] = tile_off<A_MN>(r0 + (q & 1) * 8, t + (q >> 1) * 4);
 
   // One k-tile; BUF = kt & 1 is a compile-time constant (the loop below is unrolled by two) so that the fragments stay
   // in registers.  The MMAs of kt are left in flight while the next k-tile waits for its TMA and stages its operands.
@@ -350,14 +369,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const int s = kt % C::STAGES;
     mbar_wait(&full[s], (uint32_t)(kt / C::STAGES) & 1u);
     const uint8_t* sa = smem + s * C::STAGE_BYTES;
-    const uint8_t* sb = sa + TILE_BYTES;
-    uint8_t* pb = prep + BUF * C::PREP_TILE_BYTES;
+    uint8_t* sb = smem + s * C::STAGE_BYTES + TILE_BYTES;
+    // the prep tiles, or (MODE 0) B's own stage: the MMAs of kt - 1, still in flight, read another stage
+    uint8_t* pb = C::PREP_TILES ? prep + BUF * C::PREP_TILE_BYTES : sb;
     if (C::PREP) {
       prep_b<B_MN, MODE>(sb, sb + TILE_BYTES, pb, pb + TILE_BYTES, tid);
       fence_proxy_async_smem();       // generic-proxy writes -> wgmma (async proxy) reads
       __syncthreads();                // both warpgroups read the whole prep tile
     }
-    const uint32_t b_hi = smem_u32(C::PREP ? pb : sb);
+    const uint32_t b_hi = smem_u32(pb);
     const uint32_t b_lo = b_hi + TILE_BYTES;        // 3x: the prep B_lo tile
     if (BF16) {
       uint32_t (&ahi)[2][4] = ahi16[BUF];
@@ -384,7 +404,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       for (int j = 0; j < 4; ++j)
 #pragma unroll
         for (int q = 0; q < 4; ++q)
-          ah[j][q] = *reinterpret_cast<const uint32_t*>(sa + tile_off<A_MN>(r0 + (q & 1) * 8, 8 * j + t + (q >> 1) * 4));
+          ah[j][q] = *reinterpret_cast<const uint32_t*>(sa + (A_MN ? a_off[q] + 1024 * j : a_off[q] ^ (32 * j)));
       if (C::SPLIT3) {
 #pragma unroll
         for (int j = 0; j < 4; ++j)
@@ -528,6 +548,9 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
   return NAR_OK;
 }
 
+template <int MODE>
+static int ctas_per_sm(bool b_mn) { return b_mn ? Cfg<MODE, true>::CTAS_PER_SM : Cfg<MODE, false>::CTAS_PER_SM; }
+
 }  // namespace gemm
 }  // namespace nar
 
@@ -574,13 +597,15 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   const int64_t n_tiles = (N + BN - 1) / BN, m_tiles = (M + BM - 1) / BM;
   if (n_tiles * m_tiles > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
   const int k_tiles = (int)((K + BK - 1) / BK);
+  const bool amn = !a_kmajor, bmn = !b_kmajor;
   int split = epi->split_k;
-  if (split <= 0) {          // auto: about two waves of CTAs, at least 8 k-tiles per split
-    split = 1;
+  if (split <= 0) {          // auto, for accumulate: as many CTAs as fit in one wave of the SMs' resident slots
+    split = 1;               // (a CTA past a whole wave would run alone in a second one), at least 8 k-tiles per split
     if (epi->accumulate) {
-      const int64_t want = (2 * (int64_t)ctx->sm_count + n_tiles * m_tiles - 1) / (n_tiles * m_tiles);
+      const int per_sm = mode == 0 ? ctas_per_sm<0>(bmn) : (mode == 1 ? ctas_per_sm<1>(bmn) : ctas_per_sm<2>(bmn));
+      const int64_t fit = (int64_t)per_sm * ctx->sm_count / (n_tiles * m_tiles);
       const int64_t cap = k_tiles / 8 > 1 ? k_tiles / 8 : 1;
-      split = (int)(want < cap ? want : cap);
+      split = (int)(fit < cap ? fit : cap);
       if (split < 1) split = 1;
     }
   }
@@ -606,7 +631,6 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   dim3 grid((unsigned)(n_tiles * m_tiles), (unsigned)split, 1);
   cudaStream_t st = as_stream(stream);
   if (mode == 4) return launch<false, false, 4>(ta, tb, tbl, p, grid, st);
-  const bool amn = !a_kmajor, bmn = !b_kmajor;
 #define NAR_GEMM_CASE(a, b) \
   if (amn == a && bmn == b) { \
     if (mode == 0) return launch<a, b, 0>(ta, tb, tbl, p, grid, st); \

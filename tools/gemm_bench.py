@@ -3,7 +3,8 @@
 
 Two groups of cases: operand-major / precision variants at 24000 x 1024 x 1024, and the training step's own GEMMs at
 the shapes bench.py's roofline times (R = 23 600 candidate rows, C = 1024): CAR layer 2 forward (bf16x3, bias + tanh),
-dgrad (single-pass TF32, leaky derivative from a separate aux) and split-K wgrad, and the scorer's first layer
+dgrad (single-pass TF32, leaky derivative from a separate aux) and split-K wgrad (single-pass TF32, both operands
+MN-major, split chosen by the library), and the scorer's first layer
 (C -> 128) forward / dgrad / wgrad.  Each step case also reports the share of the data-sheet peak of the tensor path it
 issues on (bf16 for bf16x3, counting its 3 MMAs per product; TF32 otherwise) and the rate at which TMA fills shared
 memory with operand tiles."""
@@ -71,7 +72,9 @@ def variant_cases(dev):
 def step_cases(dev):
     """(name, fn, [M, N, K], output, precision) of the training step's CAR layer-2 and scorer layer-1 GEMMs, operands as
     engine.cu passes them: forward A = activations (K-major) with the bf16x3 plane of W [in, out]; dgrad A = dY, B = W
-    read K-major; wgrad A = X and B = dY both MN-major, split-K chosen by the library, red.add into dW."""
+    read K-major; wgrad A = X and B = dY both MN-major (dY transposed in place in shared memory, two CTAs per SM),
+    split-K chosen by the library to fill one wave of the SMs' CTA slots (64 x 4 CTAs for layer 2, 8 x 33 for the
+    scorer on 132 SMs), red.add into dW."""
     R = STEP_R
     H1 = torch.randn(R, C, device=dev)
     E = torch.empty(R, C, device=dev)
