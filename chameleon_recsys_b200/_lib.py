@@ -164,6 +164,8 @@ _SIGNATURES = {
                                          C.c_double, vp, vp, vp, vp]),
     'nar_eval_metrics_reduce': (C.c_int, [vp, i64, i64, i64, vp, vp]),
     'nar_eval_metrics_popcount': (C.c_int, [vp, i64, i64, vp, vp]),
+    'nar_eval_by_position': (C.c_int, [vp, i64, i64, i64, i64, i64, i64, i32, vp, i64, vp, i64, vp, i64, vp, i64, vp, vp,
+                                       i64, vp, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = sorted(_SIGNATURES.keys())

@@ -180,6 +180,116 @@ __global__ void popcount_kernel(const unsigned* bitmaps, int64_t words, unsigned
   if (threadIdx.x == 0) counts[blockIdx.x] = s_n;
 }
 
+// ---- hit rate by session position (the reference's HitRateBySessionPosition, metrics.py:136-168; spec
+// oracle/by_position_ref.py).  Rows y < rows: a grid-stride loop over the queries of recommender row y builds per-CTA
+// position histograms in shared memory and adds them to hits / total with integer atomics (exact in any order).  Row
+// y == rows (only when pop is given, one CTA): chunk by chunk of sessions, the CTA gathers pop[label] of every (session,
+// position) cell into shared memory in parallel, then one thread per position t adds the chunk's values for b in order
+// - a sequential float32 sum with no FMA, carried in norm_pop from batch to batch: the reference's own order.
+constexpr int POS_THREADS = 256;
+constexpr int MAX_POS = 1024;              // positions T per batch (shared-memory histograms)
+constexpr int POP_CHUNK = 4096;            // (session, position) cells gathered per round
+constexpr int GATHER_UNROLL = 8;           // cells whose loads one thread has in flight at once
+
+struct PosArgs {
+  const int64_t* ids; int64_t row_stride, q_stride, nq; int m; long long row_mask; int rows;
+  const int64_t* labels; int64_t label_stride;
+  const int32_t* pos_idx; int T;           // pos_idx null: query q sits at position q % T
+  const int32_t* sess_off; int64_t n_sess; const float* pop;
+  int64_t num_items;
+  unsigned long long* hits; unsigned long long* total; int64_t ld;   // [rows, ld]
+  float* norm_pop;                         // [T]
+  int* err;
+};
+
+__device__ void norm_pop_pass(const PosArgs& a) {
+  __shared__ float s_v[POP_CHUNK];
+  constexpr int PER = MAX_POS / POS_THREADS;
+  const int T = a.T, per_chunk = POP_CHUNK / T;
+  float sum[PER];
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    const int t = threadIdx.x + k * POS_THREADS;
+    sum[k] = t < T ? a.norm_pop[t] : 0.f;
+  }
+  bool bad = false;
+  for (int64_t b0 = 0; b0 < a.n_sess; b0 += per_chunk) {
+    const int nb = (int)(a.n_sess - b0 < per_chunk ? a.n_sess - b0 : per_chunk), n = nb * T;
+    // three rounds of independent loads (offsets, labels, pop) over GATHER_UNROLL cells per thread
+    for (int i0 = threadIdx.x; i0 < n; i0 += POS_THREADS * GATHER_UNROLL) {
+      int32_t off[GATHER_UNROLL], end[GATHER_UNROLL];
+      int tt[GATHER_UNROLL];
+#pragma unroll
+      for (int u = 0; u < GATHER_UNROLL; ++u) {
+        const int i = i0 + u * POS_THREADS;
+        const int64_t b = i < n ? b0 + i / T : a.n_sess;     // past the chunk: an empty session
+        tt[u] = i % T;
+        off[u] = a.sess_off[b];
+        end[u] = a.sess_off[b < a.n_sess ? b + 1 : b];
+      }
+      int64_t label[GATHER_UNROLL];
+#pragma unroll
+      for (int u = 0; u < GATHER_UNROLL; ++u)
+        label[u] = tt[u] < end[u] - off[u] ? a.labels[(int64_t)(off[u] + tt[u]) * a.label_stride] : 0;
+#pragma unroll
+      for (int u = 0; u < GATHER_UNROLL; ++u) {
+        const bool ok = label[u] > 0 && label[u] < a.num_items;
+        bad |= label[u] != 0 && !ok;
+        const int i = i0 + u * POS_THREADS;
+        const float v = ok ? a.pop[label[u]] : 0.f;
+        if (i < n) s_v[i] = v;
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < PER; ++k) {
+      const int t = threadIdx.x + k * POS_THREADS;
+      if (t < T)
+        for (int b = 0; b < nb; ++b) sum[k] = __fadd_rn(sum[k], s_v[b * T + t]);   // s + 0 == s (s is never -0)
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    const int t = threadIdx.x + k * POS_THREADS;
+    if (t < T) a.norm_pop[t] = sum[k];
+  }
+  if (bad) atomicExch(a.err, 1);
+}
+
+__global__ void __launch_bounds__(POS_THREADS) by_position_kernel(PosArgs a) {
+  const int row = blockIdx.y;
+  if (row == a.rows) {                     // the model's label popularity per position
+    if (blockIdx.x == 0) norm_pop_pass(a);
+    return;
+  }
+  if (!((a.row_mask >> row) & 1)) return;
+  __shared__ unsigned s_hit[MAX_POS], s_tot[MAX_POS];
+  for (int t = threadIdx.x; t < a.T; t += POS_THREADS) { s_hit[t] = 0; s_tot[t] = 0; }
+  __syncthreads();
+  const int64_t* lists = a.ids + row * a.row_stride;
+  for (int64_t q = blockIdx.x * (int64_t)POS_THREADS + threadIdx.x; q < a.nq; q += (int64_t)gridDim.x * POS_THREADS) {
+    const int64_t label = a.labels[q * a.label_stride];
+    if (label == 0) continue;
+    bool bad = label < 0 || label >= a.num_items, hit = false;
+    const int64_t* list = lists + q * a.q_stride;
+    for (int j = 0; j < a.m; ++j) {
+      const int64_t id = list[j];
+      hit |= id == label;
+      bad |= id < 0 || id >= a.num_items;
+    }
+    if (bad) { atomicExch(a.err, 1); continue; }
+    const int t = (int)((a.pos_idx ? (int64_t)a.pos_idx[q] : q) % a.T);
+    atomicAdd(&s_tot[t], 1u);
+    if (hit) atomicAdd(&s_hit[t], 1u);
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < a.T; t += POS_THREADS) {
+    if (s_tot[t]) atomicAdd(a.total + row * a.ld + t, (unsigned long long)s_tot[t]);
+    if (s_hit[t]) atomicAdd(a.hits + row * a.ld + t, (unsigned long long)s_hit[t]);
+  }
+}
+
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
   return (int)(g < 1 ? 1 : (g > 8 * NAR_GRID_SMS ? 8 * NAR_GRID_SMS : g));
@@ -232,6 +342,31 @@ extern "C" int nar_eval_metrics_reduce(const double* per_query, int64_t rows, in
   if (!per_query || !acc || rows < 1 || rows > 63 || nq < 0) return NAR_ERR_INVALID;
   if (nq == 0) return NAR_OK;
   reduce_kernel<<<(unsigned)rows, REDUCE_THREADS, 0, as_stream(stream)>>>(per_query, nq, row_mask, acc);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_eval_by_position(const int64_t* ids, int64_t row_stride, int64_t q_stride, int64_t rows, int64_t row_mask,
+                                    int64_t nq, int64_t len, int32_t top_n, const int64_t* labels, int64_t label_stride,
+                                    const int32_t* pos_idx, int64_t T, const int32_t* sess_off, int64_t n_sess,
+                                    const float* pop, int64_t num_items, int64_t* hits, int64_t* total, int64_t ld,
+                                    float* norm_pop, int* err, void* stream) {
+  if (!ids || !labels || !hits || !total || !err || rows < 1 || rows > 63 || nq < 0 || len < 1 || q_stride < len ||
+      label_stride < 1 || top_n < 1 || T < 1 || ld < T || num_items <= 0 || (nq > 0 && !pos_idx && nq % T) ||
+      (pop && (!pos_idx || !sess_off || !norm_pop || n_sess < 0)))
+    return NAR_ERR_INVALID;
+  if (T > MAX_POS || nq > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
+  const long long mask = row_mask & ((1LL << rows) - 1);
+  if (nq == 0 || (mask == 0 && !pop)) return NAR_OK;
+  PosArgs a;
+  a.ids = ids; a.row_stride = row_stride; a.q_stride = q_stride; a.nq = nq; a.m = (int)(top_n < len ? top_n : len);
+  a.row_mask = mask; a.rows = (int)rows;
+  a.labels = labels; a.label_stride = label_stride; a.pos_idx = pos_idx; a.T = (int)T;
+  a.sess_off = sess_off; a.n_sess = n_sess; a.pop = pop; a.num_items = num_items;
+  a.hits = reinterpret_cast<unsigned long long*>(hits); a.total = reinterpret_cast<unsigned long long*>(total); a.ld = ld;
+  a.norm_pop = norm_pop; a.err = err;
+  const dim3 grid((unsigned)grid_for(nq, POS_THREADS), (unsigned)(rows + (pop ? 1 : 0)));
+  by_position_kernel<<<grid, POS_THREADS, 0, as_stream(stream)>>>(a);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

@@ -95,7 +95,9 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
                                    articles_metadata=params['articles_metadata'],
                                    eval_negative_sample_relevance=params.get('eval_negative_sample_relevance'),
                                    eval_benchmark_classifiers=params.get('eval_benchmarks') or (),
-                                   eval_extended_metrics=bool(params.get('eval_extended_metrics', False)))]
+                                   eval_extended_metrics=bool(params.get('eval_extended_metrics', False)),
+                                   eval_metrics_by_session_position=bool(
+                                       params.get('eval_metrics_by_session_position', False)))]
     if mode == ModeKeys.TRAIN:
         def train_op(feats, labs, feed, sync=True):
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
@@ -341,7 +343,10 @@ class Estimator:
         835-885; ``loss`` = mean of the per-batch total_loss like Estimator does).  The hook snapshots ClickedItemsState at
         ``begin`` and restores it at ``end`` (nar_model.py:1415, :1693), and keeps updating it batch by batch in between.
         With ``eval_extended_metrics`` also ``ndcg_at_n``, ``item_coverage_at_n``, ``esi-r_at_n``, ``esi-rr_at_n``,
-        ``content_eild-r_at_n`` and ``content_eild-rr_at_n``, and each as ``<key>_<suffix>`` for every baseline."""
+        ``content_eild-r_at_n`` and ``content_eild-rr_at_n``, and each as ``<key>_<suffix>`` for every baseline.  With
+        ``eval_metrics_by_session_position`` also ``hitrate_at_n_by_pos_PP``, ``clicks_at_pos_PP`` and
+        ``avg_norm_pop_by_pos_PP`` of the model and ``hitrate_at_n_by_pos_<suffix>_PP`` of every baseline, for each
+        session position PP ('%02d', from 01) that had a query (none without input)."""
         import torch
         it = input_fn()
 
@@ -389,6 +394,7 @@ class Estimator:
         for h in spec.evaluation_hooks:
             bench.update(h.benchmark_results())
             bench.update(h.extended_results())
+            bench.update(h.by_position_results())
             h.end()
         eng = spec.model.engine
         if eng.world > 1:                                           # data parallel: every rank ranked its own sessions

@@ -5,12 +5,16 @@ metrics.py).  Definitions and the reference's quirks: DESIGN.md section 10; spec
 ``EvalMetrics`` accumulates them for several recommenders (rows) over one evaluation: each batch's top-n id lists go in
 with ``add_lists`` straight from the device buffers that hold them (the model's ranked candidates, the baselines'
 ``out_ids``), the batch's clicks with ``add_clicks``, and ``results`` reads the accumulator once at the end.
+
+``ByPosition`` does the same for the hit rate by session position (the reference's ``HitRateBySessionPosition``, switch
+``eval_metrics_by_session_position``; DESIGN.md section 11, spec oracle/by_position_ref.py).
 """
 from __future__ import annotations
 
 import ctypes as C
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -127,4 +131,78 @@ class EvalMetrics:
             res[COVERAGE_KEY] = int(counts[r]) / clicked if clicked else float('nan')
             res.update(queries=int(q), recommended=int(counts[r]), clicked=clicked)
             out.append(res)
+        return out
+
+
+MAX_POSITIONS = 1024       # session positions (T) the by-position kernel counts per batch
+BY_POSITION_KEY = 'hitrate_at_n_by_pos'
+
+
+def check_by_position_params(top_n):
+    if not 1 <= int(top_n) <= MAX_TOP_N:
+        raise ValueError('eval_metrics_by_session_position needs 1 <= eval_metrics_top_n <= %d, not %r'
+                         % (MAX_TOP_N, top_n))
+
+
+class ByPosition:
+    """Hit rate at n by session position of ``rows`` recommenders over one evaluation.  Position p = t + 1 of a query
+    (b, t) with a nonzero label; per row and position the query count and the hits (label among the first n ids of the
+    list), and for the lists added with ``pop`` (the model's) the float32 sum of the labels' normalised popularity."""
+
+    def __init__(self, rows: int, num_items: int, top_n: int, device, err: Optional[torch.Tensor] = None):
+        check_by_position_params(top_n)
+        self.rows, self.num_items, self.top_n = int(rows), int(num_items), int(top_n)
+        self.dev = torch.device(device)
+        self.lib = _lib.load()
+        self.err = torch.zeros(1, dtype=torch.int32, device=self.dev) if err is None else err
+        self.counts = torch.zeros(2, self.rows, MAX_POSITIONS, dtype=torch.int64, device=self.dev)   # hits, queries
+        self.norm_pop = torch.zeros(MAX_POSITIONS, dtype=torch.float32, device=self.dev)
+
+    def begin(self):
+        self.counts.zero_()
+        self.norm_pop.zero_()
+
+    def add(self, ids: torch.Tensor, labels: torch.Tensor, T: int, pos_idx: Optional[torch.Tensor] = None,
+            sess_off: Optional[torch.Tensor] = None, pop: Optional[torch.Tensor] = None, row0: int = 0,
+            row_mask: Optional[int] = None, label_stride: int = 1):
+        """Count one batch's lists of the rows ``row0 ..``: ``ids`` [rows, Q, len] or [Q, len] int64 device, ``labels``
+        [Q * label_stride] int64 device (0 = no query).  Query q sits at position ``pos_idx[q] % T`` (int32 flat b*T + t,
+        the model's compacted rows), or at ``q % T`` without ``pos_idx`` (a [B*T] grid).  ``pop`` [V] float32 device with
+        ``sess_off`` [B + 1] int32 (session b's rows start at sess_off[b]): the labels' popularity joins the position
+        sums, session by session in order.  ``row_mask`` (bit r: row row0 + r) defaults to all."""
+        ids3 = ids if ids.dim() == 3 else ids.unsqueeze(0)
+        rows, nq, length = ids3.shape
+        assert ids3.dtype == torch.int64 and ids3.stride(2) == 1 and 0 <= row0 and row0 + rows <= self.rows
+        assert labels.dtype == torch.int64 and labels.is_contiguous()
+        assert pos_idx is None or (pos_idx.dtype == torch.int32 and pos_idx.is_contiguous() and pos_idx.numel() >= nq)
+        assert pop is None or (pop.dtype == torch.float32 and sess_off is not None and sess_off.dtype == torch.int32)
+        if int(T) > MAX_POSITIONS:
+            raise ValueError('eval_metrics_by_session_position counts at most %d session positions, not %d'
+                             % (MAX_POSITIONS, T))
+        if nq == 0:
+            return
+        mask = (1 << rows) - 1 if row_mask is None else int(row_mask)
+        check(self.lib.nar_eval_by_position(
+            _p(ids3), ids3.stride(0), ids3.stride(1), rows, mask, nq, length, self.top_n, _p(labels), label_stride,
+            _p(pos_idx), int(T), _p(sess_off), 0 if sess_off is None else sess_off.numel() - 1, _p(pop), self.num_items,
+            _p(self.counts[0, row0]), _p(self.counts[1, row0]), MAX_POSITIONS, _p(self.norm_pop), _p(self.err),
+            C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)), 'nar_eval_by_position')
+
+    def results(self, names) -> Dict[str, float]:
+        """``names`` [(row, suffix)]: ``hitrate_at_n_by_pos[_<suffix>]_PP`` = hits / queries for every position p with a
+        query (PP = '%02d' % p); for the empty suffix (the model) also ``clicks_at_pos_PP`` = queries and
+        ``avg_norm_pop_by_pos_PP`` = the float32 popularity sum / queries, divided in float32.  Raises ValueError when an
+        id was outside [0, num_items)."""
+        counts, norm_pop, err = self.counts.cpu().numpy(), self.norm_pop.cpu().numpy(), int(self.err.item())
+        if err == 1:
+            raise ValueError('evaluation metrics: an article id lies outside [0, num_items)')
+        out: Dict[str, float] = {}
+        for row, s in names:
+            hits, total = counts[0, row], counts[1, row]
+            for t in np.flatnonzero(total):
+                p, q = int(t) + 1, int(total[t])
+                out['%s%s_%02d' % (BY_POSITION_KEY, '_' + s if s else '', p)] = int(hits[t]) / float(q)
+                if not s:
+                    out['clicks_at_pos_%02d' % p] = q
+                    out['avg_norm_pop_by_pos_%02d' % p] = float(np.float32(norm_pop[t]) / np.float32(q))
         return out

@@ -148,6 +148,10 @@ class NARHParams:
     # NDCG, item coverage, ESI-R / ESI-RR and EILD-R / EILD-RR of the model and every baseline in Estimator.evaluate
     # (the reference hook's create_eval_metrics; eval_metrics.py)
     eval_extended_metrics: bool = False
+    # the hit rate at the 1st, 2nd, ... click of a session for the model and every baseline, and the model's query count
+    # and mean label popularity per position, in Estimator.evaluate (the reference trainer's flag of the same name,
+    # nar_trainer_gcom.py:56; eval_metrics.ByPosition)
+    eval_metrics_by_session_position: bool = False
 
     def to_params(self, session_features_config, articles_features_config, articles_metadata,
                   content_article_embeddings_matrix) -> dict:
@@ -170,7 +174,7 @@ class NARHParams:
             'eval_negative_samples_from_buffer': self.eval_negative_samples_from_buffer,
             'softmax_temperature': self.softmax_temperature,
             'save_histograms': False,
-            'eval_metrics_by_session_position': False,
+            'eval_metrics_by_session_position': self.eval_metrics_by_session_position,
             'novelty_reg_factor': self.novelty_reg_factor,
             'diversity_reg_factor': self.diversity_reg_factor,
             'eval_negative_sample_relevance': 0.1,

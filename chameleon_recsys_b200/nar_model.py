@@ -170,6 +170,16 @@ class ItemsStateUpdaterHook:
                 raise NotImplementedError('the extended evaluation metrics run on one process; data-parallel evaluation '
                                           'of them is not implemented')
             check_params(eval_metrics_top_n, eval_negative_sample_relevance)
+        # hit rate by session position of the model and every baseline (nar_model.py:1718-1719): an
+        # eval_metrics.ByPosition accumulator with the same rows
+        self.by_position_on = eval_metrics_by_session_position and mode == ModeKeys.EVAL
+        self.by_position = None
+        if self.by_position_on:
+            from .eval_metrics import check_by_position_params
+            if model.engine.world > 1:
+                raise NotImplementedError('the hit rate by session position runs on one process; data-parallel '
+                                          'evaluation of it is not implemented')
+            check_by_position_params(eval_metrics_top_n)
         # baseline recommenders (nar_model.py:1399-1407): [{'recommender': <suffix>, 'params': {...}}]; their state is the
         # BaselineTables object on the ClickedItemsState, shared by the TRAIN and EVAL hooks
         self.bench_metrics = None
@@ -205,6 +215,13 @@ class ItemsStateUpdaterHook:
                                                 self.eval_metrics_top_n, self.eval_negative_sample_relevance,
                                                 acr_norm=None if tables is None else tables.acr_norm)
                 self.extended.begin(self.clicked_items_state.get_recent_clicks_buffer())
+            if self.by_position_on:
+                if self.by_position is None:
+                    from .eval_metrics import ByPosition
+                    self.by_position = ByPosition(1 + (self.baselines.n_rows if self.baselines is not None else 0),
+                                                  self.clicked_items_state.num_items, self.eval_metrics_top_n,
+                                                  self.model.engine.dev)
+                self.by_position.begin()
 
     def before_run(self, run_context=None) -> dict:
         """-> feed dict (nar_model.py:1458-1467)."""
@@ -218,19 +235,23 @@ class ItemsStateUpdaterHook:
         it, then learn from it (nar_model.py:1609-1632).  With the extended metrics on also 'predicted_item_ids' (the
         model's ranked candidates [L, 1+K] on the device, None without queries): the model's and the baselines' top-n
         lists are measured with the popularity the batch was fed with, before the state learns from the batch
-        (:1591-1603)."""
-        ext = self.extended                                 # set in EVAL only
-        if ext is not None:
+        (:1591-1603).  The hit rate by session position takes the same lists."""
+        ext, bp = self.extended, self.by_position           # set in EVAL only
+        if ext is not None or bp is not None:
             st = run_values['stage']
             pred = run_values.get('predicted_item_ids')
             if pred is not None:
                 # each query's label is column 0 of the candidate ids the ranking read
                 cand = self.model.engine.buffer(st, 'row_item').view(-1)[st['L']:]
-                ext.add_lists(pred, cand, st['t']['pop_norm'], label_stride=pred.shape[1])
+                if ext is not None:
+                    ext.add_lists(pred, cand, st['t']['pop_norm'], label_stride=pred.shape[1])
+                if bp is not None:
+                    bp.add(pred, cand, st['T'], pos_idx=st['t']['pos_idx'], sess_off=st['t']['sess_off'],
+                           pop=st['t']['pop_norm'], label_stride=pred.shape[1])
         if self.baselines is not None and self.mode == ModeKeys.EVAL:
             t = run_values['stage']['t']
             out_ids = None
-            if ext is not None:
+            if ext is not None or bp is not None:
                 import torch
                 out_ids = torch.empty(self.baselines.n_rows, t['label_next'].numel(), self.eval_metrics_top_n,
                                       dtype=torch.int64, device=self.model.engine.dev)
@@ -238,9 +259,12 @@ class ItemsStateUpdaterHook:
                                  self.clicked_items_state.get_recent_clicks_buffer(),
                                  self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n, self.bench_metrics,
                                  out_ids=out_ids)
-            if ext is not None:
-                ext.add_lists(out_ids, t['label_next'].view(-1), t['pop_norm'], row0=1,
-                              row_mask=sum(1 << self.baselines.row(s) for s in self.baselines.enabled))
+            if out_ids is not None:
+                mask = sum(1 << self.baselines.row(s) for s in self.baselines.enabled)
+                if ext is not None:
+                    ext.add_lists(out_ids, t['label_next'].view(-1), t['pop_norm'], row0=1, row_mask=mask)
+                if bp is not None:
+                    bp.add(out_ids, t['label_next'].view(-1), run_values['stage']['T'], row0=1, row_mask=mask)
             if run_values['stage']['has_clicks']:
                 self.baselines.update(t['all_items'], lens=np.count_nonzero(np.concatenate(
                     [run_values['clicked_items'], np.asarray(run_values['last_item_label']).reshape(-1, 1)], axis=1), axis=1),
@@ -267,6 +291,15 @@ class ItemsStateUpdaterHook:
         named = [('', rows[0])] + ([(s, rows[1 + self.baselines.row(s)]) for s in self.baselines.enabled]
                                    if self.baselines is not None else [])
         return {k + ('_' + s if s else ''): r[k] for s, r in named for k in KEYS + (COVERAGE_KEY,)}
+
+    def by_position_results(self) -> dict:
+        """The hit rate by session position of this evaluation ({} with it off): the model's keys without a suffix, each
+        baseline's with its suffix (eval_metrics.ByPosition.results)."""
+        if self.by_position is None:
+            return {}
+        names = [(0, '')] + ([(1 + self.baselines.row(s), s) for s in self.baselines.enabled]
+                             if self.baselines is not None else [])
+        return self.by_position.results(names)
 
     def end(self, session=None):
         if self.mode == ModeKeys.EVAL:

@@ -518,6 +518,20 @@ int nar_eval_metrics_lists(const int64_t* ids, int64_t row_stride, int64_t q_str
 int nar_eval_metrics_reduce(const double* per_query, int64_t rows, int64_t row_mask, int64_t nq, double* acc, void* stream);
 /* counts [n_maps] int64 = set bits of each of the bitmaps [n_maps, words] */
 int nar_eval_metrics_popcount(const uint32_t* bitmaps, int64_t n_maps, int64_t words, int64_t* counts, void* stream);
+/* Hit rate by session position: replaces the reference hook's HitRateBySessionPosition.add (metrics.py:136-168, fed by
+ * evaluation.py update_metrics from nar_model.py:1595-1603 and benchmarks.py:35-55; spec oracle/by_position_ref.py).
+ * For every recommender row r < rows with bit r of row_mask set and every query q < nq whose label
+ * labels[q * label_stride] is nonzero, at position t = pos_idx[q] % T (pos_idx null: q % T, nq a multiple of T):
+ * total[r * ld + t] += 1, and hits[r * ld + t] += 1 when the label is among the first min(top_n, len) ids of
+ * ids[r * row_stride + q * q_stride + j].  hits / total int64 [rows, ld], ld >= T, T <= 1024.  With pop (float32 [V],
+ * needs pos_idx and sess_off [n_sess + 1]: query rows of session b are sess_off[b] + t, t < sess_off[b+1] - sess_off[b]):
+ * norm_pop[t] (float32 [T]) += pop[label] of each such row with a nonzero label, sessions b in order, one float32
+ * round per add.  *err = 1 for an id outside [0, num_items) (the query is not counted).                             */
+int nar_eval_by_position(const int64_t* ids, int64_t row_stride, int64_t q_stride, int64_t rows, int64_t row_mask,
+                         int64_t nq, int64_t len, int32_t top_n, const int64_t* labels, int64_t label_stride,
+                         const int32_t* pos_idx, int64_t T, const int32_t* sess_off, int64_t n_sess, const float* pop,
+                         int64_t num_items, int64_t* hits, int64_t* total, int64_t ld, float* norm_pop, int* err,
+                         void* stream);
 
 #ifdef __cplusplus
 }
