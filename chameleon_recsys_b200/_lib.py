@@ -86,7 +86,9 @@ class NoveltyReg(C.Structure):
 class GemmEpilogue(C.Structure):
     _fields_ = [('bias', C.c_void_p), ('act', C.c_int32), ('dact', C.c_int32), ('aux', C.c_void_p),
                 ('ld_aux', C.c_int64), ('accumulate', C.c_int32), ('split_k', C.c_int32),
-                ('precision', C.c_int32), ('b_lo', C.c_void_p), ('b_bf16', C.c_void_p), ('ld_bf16', C.c_int64)]
+                ('precision', C.c_int32), ('b_lo', C.c_void_p), ('b_bf16', C.c_void_p), ('ld_bf16', C.c_int64),
+                ('a_scale', C.c_void_p), ('ld_a_scale', C.c_int64), ('a_scale_group', C.c_int64),
+                ('pred', C.c_void_p), ('d_pred', C.c_void_p), ('ld_pred', C.c_int64), ('pred_group', C.c_int64)]
 
 
 _lib: Optional[C.CDLL] = None

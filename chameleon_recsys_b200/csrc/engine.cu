@@ -81,9 +81,20 @@ struct nar_engine {
   float* WhT[NAR_MAX_LAYERS];
   float* WhcT[NAR_MAX_LAYERS];     // GRU: transposed candidate recurrent block
   int64_t launches;
+  int fused_product;               // NAR_FUSED_SCORER_PRODUCT (default 1), read when the engine is created
 };
 
 namespace {
+
+// The MLP scorer's product PD = Ec * PR[position] (nar_model.py:478, :493) folded into its first Dense layer's GEMMs: the
+// forward and the weight gradient scale Ec by PR as they load it (nar_gemm_epilogue.a_scale, the same rounded product), the
+// dgrad's epilogue forms dEc and dPR from whole positions (nar_gemm_epilogue.pred).  PD and dPD are never stored.  Needs
+// the bf16x3 forward and single-pass TF32 backward, and positions that fit an M tile (1 + K <= 128); otherwise, or with
+// NAR_FUSED_SCORER_PRODUCT=0, nar_mul_pred / nar_mul_pred_bwd run around the plain GEMMs.
+bool fused_product(const nar_engine* e) {
+  const nar_model_cfg& c = e->cfg;
+  return e->fused_product && c.ranking == 0 && c.K + 1 <= 128 && c.fwd_precision == 4 && c.bwd_precision == 1;
+}
 
 int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_t L_cap, void* base, PrepBufs* pb) {
   const nar_model_cfg& c = e->cfg;
@@ -126,8 +137,10 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
   sb->PR = cv.take<float>(L_cap * C);
   sb->logits = cv.take<float>(L_cap * n_cand);
   if (c.dedup) { sb->PP = cv.take<float>(L_cap * C); sb->PI = cv.take<float>(U * C); sb->PC = cv.take<float>(L_cap * C); }
+  const bool fused = fused_product(e);
   if (c.ranking == 0) {
-    sb->PD = cv.take<float>(Rc * C); sb->Z1 = cv.take<float>(Rc * 128); sb->Z2 = cv.take<float>(Rc * 64); sb->Z3 = cv.take<float>(Rc * 32);
+    if (!fused) sb->PD = cv.take<float>(Rc * C);
+    sb->Z1 = cv.take<float>(Rc * 128); sb->Z2 = cv.take<float>(Rc * 64); sb->Z3 = cv.take<float>(Rc * 32);
   }
   if (train) {
     sb->dE = cv.take<float>(R * C);
@@ -136,7 +149,8 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
       sb->dGX[i] = cv.take<float>(L_cap * gw * Hp); sb->HPV[i] = cv.take<float>(L_cap * Hp); sb->dHOb[i] = cv.take<float>(L_cap * Hp);
     }
     if (c.ranking == 0) {
-      sb->dZ3 = cv.take<float>(Rc * 32); sb->dZ2 = cv.take<float>(Rc * 64); sb->dZ1 = cv.take<float>(Rc * 128); sb->dPD = cv.take<float>(Rc * C);
+      sb->dZ3 = cv.take<float>(Rc * 32); sb->dZ2 = cv.take<float>(Rc * 64); sb->dZ1 = cv.take<float>(Rc * 128);
+      if (!fused) sb->dPD = cv.take<float>(Rc * C);
     }
     if (c.keep_prob < 1.f)
       for (int i = 0; i < c.layers; ++i) sb->HOd[i] = cv.take<float>(L_cap * Hp);
@@ -196,9 +210,11 @@ struct Seq {
   float* G(int64_t off) const { return c.grads + off; }
 
   // Y[M,N] = act(X[M,Kd] * W[Kd,N] + b)      (W stored [in,out]: MN-major B operand, or its bf16x3 plane)
+  // (a_scale: X's row i scaled by a_scale[i / group] as it is loaded, see fused_product)
   void fwd(const float* X, int64_t ldx, int64_t off_W, int64_t ldw, int64_t off_b, float* Y, int64_t ldy, int64_t M, int64_t N,
-           int64_t Kd, int act, cudaStream_t st) {
+           int64_t Kd, int act, cudaStream_t st, const float* a_scale = nullptr, int64_t ld_scale = 0, int64_t group = 0) {
     nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
+    ep.a_scale = a_scale; ep.ld_a_scale = ld_scale; ep.a_scale_group = group;
     ep.bias = off_b >= 0 ? W(off_b) : nullptr; ep.act = act; ep.split_k = 1; ep.precision = c.fwd_precision;
     ep.b_lo = c.fwd_precision == 3 ? c.params_lo + off_W : nullptr;
     if (c.fwd_precision == 4) {
@@ -219,11 +235,22 @@ struct Seq {
     chk(nar_gemm_tf32(e->ctx, M, n_in, n_out, dY, lddy, 1, W(off_W), ldw, 1, dX, lddx, &ep, st));
   }
   // dW[n_in,n_out] += X[rows,n_in]^T * dY[rows,n_out]   (split-K, red.add into the gradient buffer)
+  // (a_scale: as in fwd)
   void wgrad(const float* X, int64_t ldx, const float* dY, int64_t lddy, int64_t off_W, int64_t ldw, int64_t n_in, int64_t n_out,
-             int64_t rows, cudaStream_t st) {
+             int64_t rows, cudaStream_t st, const float* a_scale = nullptr, int64_t ld_scale = 0, int64_t group = 0) {
     nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
+    ep.a_scale = a_scale; ep.ld_a_scale = ld_scale; ep.a_scale_group = group;
     ep.accumulate = 1; ep.split_k = 0; ep.precision = c.bwd_precision;
     chk(nar_gemm_tf32(e->ctx, n_in, n_out, rows, X, ldx, 0, dY, lddy, 0, G(off_W), ldw, &ep, st));
+  }
+  // through the scorer product and the CAR tanh: v = dY W^T; dX[r] = v[r] * pred[r / group] * tanh'(cand[r]) and
+  // dpred[l] = sum over position l's rows of v * cand (nar_mul_pred_bwd's arithmetic)
+  void dgrad_prod(const float* dY, int64_t lddy, int64_t off_W, int64_t ldw, const float* cand, const float* pred, int64_t group,
+                  float* dX, float* dpred, int64_t M, int64_t n_in, int64_t n_out, cudaStream_t st) {
+    nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
+    ep.dact = NAR_ACT_TANH; ep.aux = cand; ep.ld_aux = n_in; ep.split_k = 1; ep.precision = c.bwd_precision;
+    ep.pred = pred; ep.d_pred = dpred; ep.ld_pred = n_in; ep.pred_group = group;
+    chk(nar_gemm_tf32(e->ctx, M, n_in, n_out, dY, lddy, 1, W(off_W), ldw, 1, dX, n_in, &ep, st));
   }
   void bgrad(const float* dY, int64_t ld, int64_t rows, int64_t cols, int64_t off_b, cudaStream_t st) {
     chk(nar_colsum_add(dY, rows, cols, ld, G(off_b), st));
@@ -325,9 +352,14 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   nov.factor = c.novelty_reg_factor; nov.log_base = c.plan.log_base_novelty; nov.pop_norm = io->pop_norm;
   nov.cand_ids = pb.row_item + L; nov.loss_nov = io->loss + 2;
   const nar_novelty_reg* novp = c.novelty_reg_factor > 0.f ? &nov : nullptr;
+  const bool fused = fused_product(e);
   if (c.ranking == 0) {
-    s.chk(nar_mul_pred(Ec, sb.PR, L, n_cand, C, sb.PD, main));
-    s.fwd(sb.PD, C, c.off_M[0], c.ld_M[0], c.off_c[0], sb.Z1, 128, Rc, 128, C, NAR_ACT_LEAKY_RELU, main);
+    if (fused) {
+      s.fwd(Ec, C, c.off_M[0], c.ld_M[0], c.off_c[0], sb.Z1, 128, Rc, 128, C, NAR_ACT_LEAKY_RELU, main, sb.PR, C, n_cand);
+    } else {
+      s.chk(nar_mul_pred(Ec, sb.PR, L, n_cand, C, sb.PD, main));
+      s.fwd(sb.PD, C, c.off_M[0], c.ld_M[0], c.off_c[0], sb.Z1, 128, Rc, 128, C, NAR_ACT_LEAKY_RELU, main);
+    }
     s.fwd(sb.Z1, 128, c.off_M[1], c.ld_M[1], c.off_c[1], sb.Z2, 64, Rc, 64, 128, NAR_ACT_LEAKY_RELU, main);
     s.fwd(sb.Z2, 64, c.off_M[2], c.ld_M[2], c.off_c[2], sb.Z3, 32, Rc, 32, 64, NAR_ACT_LEAKY_RELU, main);
     s.chk(nar_score_softmax_ce(sb.Z3, 32, 32, s.W(c.off_M[3]), c.ld_M[3], s.W(c.off_c[3]), L, n_cand, c.inv_temperature, inv_count,
@@ -349,10 +381,19 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
     s.dgrad(sb.dZ3, 32, c.off_M[2], c.ld_M[2], sb.dZ2, 64, Rc, 64, 32, NAR_ACT_LEAKY_RELU, sb.Z2, 64, 0, main);
     { cudaStream_t st = s.fork(); s.wgrad(sb.Z1, 128, sb.dZ2, 64, c.off_M[1], c.ld_M[1], 128, 64, Rc, st); s.bgrad(sb.dZ2, 64, Rc, 64, c.off_c[1], st); }
     s.dgrad(sb.dZ2, 64, c.off_M[1], c.ld_M[1], sb.dZ1, 128, Rc, 128, 64, NAR_ACT_LEAKY_RELU, sb.Z1, 128, 0, main);
-    { cudaStream_t st = s.fork(); s.wgrad(sb.PD, C, sb.dZ1, 128, c.off_M[0], c.ld_M[0], C, 128, Rc, st); s.bgrad(sb.dZ1, 128, Rc, 128, c.off_c[0], st); }
-    s.dgrad(sb.dZ1, 128, c.off_M[0], c.ld_M[0], sb.dPD, C, Rc, C, 128, NAR_ACT_NONE, nullptr, 0, 0, main);
+    {
+      cudaStream_t st = s.fork();
+      if (fused) s.wgrad(Ec, C, sb.dZ1, 128, c.off_M[0], c.ld_M[0], C, 128, Rc, st, sb.PR, C, n_cand);
+      else s.wgrad(sb.PD, C, sb.dZ1, 128, c.off_M[0], c.ld_M[0], C, 128, Rc, st);
+      s.bgrad(sb.dZ1, 128, Rc, 128, c.off_c[0], st);
+    }
     // candidate rows: through the product and the CAR tanh in one pass; d(pred) reduced over the candidates
-    s.chk(nar_mul_pred_bwd(sb.dPD, Ec, sb.PR, L, n_cand, C, NAR_ACT_TANH, dEc, sb.dPR, main));
+    if (fused) {
+      s.dgrad_prod(sb.dZ1, 128, c.off_M[0], c.ld_M[0], Ec, sb.PR, n_cand, dEc, sb.dPR, Rc, C, 128, main);
+    } else {
+      s.dgrad(sb.dZ1, 128, c.off_M[0], c.ld_M[0], sb.dPD, C, Rc, C, 128, NAR_ACT_NONE, nullptr, 0, 0, main);
+      s.chk(nar_mul_pred_bwd(sb.dPD, Ec, sb.PR, L, n_cand, C, NAR_ACT_TANH, dEc, sb.dPR, main));
+    }
   } else {
     s.chk(nar_act_bwd(dEc, Ec, Rc * C, NAR_ACT_TANH, dEc, main));
   }
@@ -567,8 +608,12 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
       s.fwd(rb.H1g, C, c.off_W2, C, c.off_b2, rb.Eg, C, P, C, C, NAR_ACT_TANH, main);
       float* lg = Nc == N ? rb.logits : rb.lg_chunk;
       if (c.ranking == 0) {
-        s.chk(nar_mul_pred(rb.Eg, prq, Qb, Nc, C, rb.H1g, main));
-        s.fwd(rb.H1g, C, c.off_M[0], c.ld_M[0], c.off_c[0], rb.Z1, 128, P, 128, C, NAR_ACT_LEAKY_RELU, main);
+        if (e->fused_product && c.fwd_precision == 4) {     // the product folded into the GEMM as in run_step (any Nc)
+          s.fwd(rb.Eg, C, c.off_M[0], c.ld_M[0], c.off_c[0], rb.Z1, 128, P, 128, C, NAR_ACT_LEAKY_RELU, main, prq, C, Nc);
+        } else {
+          s.chk(nar_mul_pred(rb.Eg, prq, Qb, Nc, C, rb.H1g, main));
+          s.fwd(rb.H1g, C, c.off_M[0], c.ld_M[0], c.off_c[0], rb.Z1, 128, P, 128, C, NAR_ACT_LEAKY_RELU, main);
+        }
         s.fwd(rb.Z1, 128, c.off_M[1], c.ld_M[1], c.off_c[1], rb.Z2, 64, P, 64, 128, NAR_ACT_LEAKY_RELU, main);
         s.fwd(rb.Z2, 64, c.off_M[2], c.ld_M[2], c.off_c[2], rb.Z3, 32, P, 32, 64, NAR_ACT_LEAKY_RELU, main);
         s.chk(nar_score_softmax_ce(rb.Z3, 32, 32, s.W(c.off_M[3]), c.ld_M[3], s.W(c.off_c[3]), Qb, Nc, c.inv_temperature, 0.f, lg,
@@ -638,6 +683,7 @@ extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_eng
   nar_engine* e = new nar_engine();
   memset(e, 0, sizeof(*e));
   e->ctx = ctx; e->cfg = *cfg;
+  { const char* v = getenv("NAR_FUSED_SCORER_PRODUCT"); e->fused_product = !(v && atoi(v) == 0); }
   NAR_CHECK_CUDA(cudaSetDevice(ctx->device));
   if (cudaStreamCreateWithFlags(&e->aux, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&e->aux2, cudaStreamNonBlocking) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }

@@ -30,6 +30,9 @@
 //           TMA, split in registers.  B: a pre-split, TRANSPOSED bf16 plane maintained next to the weights
 //           (nar_pack_bf16x3): row n holds, per block of 32 k, the 32 hi values followed by the 32 lo values = one
 //           128-byte swizzle row, so ONE K-major TMA box brings both halves and no transpose pass is needed.
+// The scorer's product PD = Ec * PR[position] (nar_model.py:478, :493) never reaches HBM: its Dense layer's forward and
+// weight gradient scale A by PR where the fragment is built (EXT_SCALE_*), and its dgrad derives dEc and dPR in an
+// epilogue over position-aligned M tiles (EXT_PROD_BWD).
 #include "common.cuh"
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -46,7 +49,18 @@ constexpr int TILE_BYTES = 128 * BK * 4;     // one 128 x 32 fp32 operand tile (
 constexpr int NUM_THREADS = 256;
 constexpr int EPI_LD = BN + 4;               // floats per staged accumulator row (16-byte aligned rows)
 
-template <int MODE, bool B_MN> struct Cfg {
+// Extensions of the plain GEMM (template parameter EXT of the kernel; 0 = none):
+//   EXT_SCALE_SMEM  A scale (nar_gemm_epilogue.a_scale), its slice for the k-tile staged by TMA with the stage: a K-major
+//                   A needs the scale rows of the tile's row groups (at most SC_ROWS_K) x 32 k, an MN-major A those of
+//                   the k-tile's k groups (at most SC_ROWS_MN) x 128 m; SC_BYTES per stage either way
+//   EXT_SCALE_GMEM  A scale read from global memory at the fragment: any group size (those whose slices do not fit)
+//   EXT_PROD_BWD    scorer-product backward epilogue (nar_gemm_epilogue.pred): position-aligned M tiles
+constexpr int EXT_SCALE_SMEM = 1, EXT_SCALE_GMEM = 2, EXT_PROD_BWD = 3;
+constexpr int SC_ROWS_K = 32, SC_ROWS_MN = 8;
+constexpr int SC_BYTES = 4096;
+static_assert(SC_ROWS_K * BK * 4 == SC_BYTES && SC_ROWS_MN * BM * 4 == SC_BYTES, "a_scale slice per stage");
+
+template <int MODE, bool B_MN, int SC = 0> struct Cfg {                // SC: bytes of a_scale slice per stage
   static constexpr bool SPLIT3 = MODE == 1 || MODE == 2;
   static constexpr bool BLO = MODE == 2;
   static constexpr bool PREP = B_MN || SPLIT3;                        // B goes through the transpose / split pass
@@ -59,7 +73,8 @@ template <int MODE, bool B_MN> struct Cfg {
   static constexpr int STAGES = (BLO || !PREP_TILES) ? 3 : 4;
   static constexpr int PREP_TILE_BYTES = PREP_TILES ? TILE_BYTES * 2 : 0;   // K-major B_hi | B_lo
   static constexpr int PREP_BYTES = 2 * PREP_TILE_BYTES;             // double-buffered: k-tile kt uses buffer kt & 1
-  static constexpr int BAR_OFF = STAGES * STAGE_BYTES + PREP_BYTES;
+  static constexpr int SC_OFF = STAGES * STAGE_BYTES + PREP_BYTES;    // [STAGES] a_scale slices
+  static constexpr int BAR_OFF = SC_OFF + STAGES * SC;
   static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;              // + barriers + alignment slack
   static_assert(STAGES * STAGE_BYTES >= BM * EPI_LD * 4, "the epilogue stages the accumulators in the operand ring");
   static_assert(SMEM_BYTES <= 227 * 1024, "227 KB of shared memory per block");
@@ -74,6 +89,10 @@ struct Params {
   int act, dact, accumulate;
   int k_tiles_per_split;
   int n_tiles;                 // blockIdx.x = m_blk * n_tiles + n_blk (N fastest: CTAs sharing an A tile run together)
+  // A scale (EXT_SCALE_*): A's storage is [a_rows, a_cols]; storage row i uses scale row i / group
+  const float* a_scale; int64_t ld_a_scale, a_rows, a_cols; uint32_t group;
+  // EXT_PROD_BWD: M tile m_blk = positions [m_blk * pos_per_tile, ...), `group` rows each, n_pos positions in all
+  const float* pred; float* d_pred; int64_t ld_pred, n_pos; int pos_per_tile;
 };
 
 // ---------------------------------------------------------------- PTX wrappers
@@ -286,6 +305,73 @@ __device__ __forceinline__ void epilogue_store4(const Params& p, float4 v, int64
   }
 }
 
+// A scale of the element A's storage holds at (row i, column j), read from global memory (EXT_SCALE_GMEM); 0 outside A,
+// where TMA has filled the tile with zeros
+// (A's storage rows fit in 31 bits when it is scaled)
+__device__ __forceinline__ float scale_gmem(const Params& p, int i, int j) {
+  return (i < p.a_rows && j < p.a_cols) ? __ldg(p.a_scale + (int64_t)((uint32_t)i / p.group) * p.ld_a_scale + j) : 0.f;
+}
+// EXT_SCALE_GMEM: the stage's A tile scaled in place, one 16-byte chunk (4 elements along the storage row) at a time, before
+// its fragments are read; the same single multiply as EXT_SCALE_SMEM applies in registers
+template <bool A_MN>
+__device__ __forceinline__ void scale_tile_gmem(uint8_t* sa, const Params& p, int m0, int k_elem, int tid) {
+#pragma unroll 1
+  for (int c = tid; c < TILE_BYTES / 16; c += NUM_THREADS) {
+    int row, col;                     // storage position of the chunk's first element (see tile_off)
+    if (A_MN) { const int kr = (c >> 3) & 31; row = k_elem + kr; col = m0 + (c >> 8) * 32 + (((c & 7) ^ (kr & 7)) << 2); }
+    else { const int r = c >> 3; row = m0 + r; col = k_elem + (((c & 7) ^ (r & 7)) << 2); }
+    float4* x = reinterpret_cast<float4*>(sa + c * 16);
+    float4 v = *x;
+    v.x = __fmul_rn(v.x, scale_gmem(p, row, col)); v.y = __fmul_rn(v.y, scale_gmem(p, row, col + 1));
+    v.z = __fmul_rn(v.z, scale_gmem(p, row, col + 2)); v.w = __fmul_rn(v.w, scale_gmem(p, row, col + 3));
+    *x = v;
+  }
+}
+__device__ __forceinline__ float2 ld_shared_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+  return v;
+}
+
+// EXT_PROD_BWD epilogue: `stage` holds v = dL/d(prod) of the tile's rows; thread = (position, column), walking the
+// position's rows in order so that d_pred is the same fmaf chain as nar_mul_pred_bwd's
+__device__ __forceinline__ void prod_bwd_epilogue(const Params& p, const float* stage, int m_blk, int n_blk, int tid) {
+  const int P = p.pos_per_tile, g = (int)p.group;
+  for (int idx = tid; idx < P * BN; idx += NUM_THREADS) {
+    const int pl = idx / BN, c = idx % BN;
+    const int64_t pos = (int64_t)m_blk * P + pl, col = (int64_t)n_blk * BN + c;
+    if (pos >= p.n_pos || col >= p.N) continue;
+    const float pr = __ldg(p.pred + pos * p.ld_pred + col);
+    const float* v = stage + pl * g * EPI_LD + c;
+    const float* e = p.aux + pos * g * p.ld_aux + col;
+    float* d = p.D + pos * g * p.ldd + col;
+    float acc = 0.f;
+    int j = 0;
+    for (; j + 8 <= g; j += 8) {      // eight rows of aux in flight, then the dependent chain in row order
+      float ev[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) ev[u] = e[(j + u) * p.ld_aux];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const float x = v[(j + u) * EPI_LD];
+        d[(j + u) * p.ldd] = x * pr * act_grad_from_output(ev[u], p.dact);
+        acc = fmaf(x, ev[u], acc);
+      }
+    }
+    for (; j < g; ++j) {
+      const float x = v[j * EPI_LD], ej = e[j * p.ld_aux];
+      d[j * p.ldd] = x * pr * act_grad_from_output(ej, p.dact);
+      acc = fmaf(x, ej, acc);
+    }
+    p.d_pred[pos * p.ld_pred + col] = acc;
+  }
+}
+
 // TMA for one 128 x 32 fp32 operand tile at MN coordinate mn0, K element k_elem
 template <bool MN_MAJOR>
 __device__ __forceinline__ void load_operand(uint32_t dst, const CUtensorMap* map, uint64_t* bar, int mn0, int k_elem) {
@@ -298,13 +384,18 @@ __device__ __forceinline__ void load_operand(uint32_t dst, const CUtensorMap* ma
 }
 
 // ---------------------------------------------------------------- kernel
-template <bool A_MN, bool B_MN, int MODE>
+// tmap_x: B_lo (MODE 2) or the a_scale slices (EXT_SCALE_SMEM)
+template <bool A_MN, bool B_MN, int MODE, int EXT>
 __global__ void __launch_bounds__(NUM_THREADS, (Cfg<MODE, B_MN>::CTAS_PER_SM))
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const __grid_constant__ CUtensorMap tmap_blo, const Params p) {
-  using C = Cfg<MODE, B_MN>;
+            const __grid_constant__ CUtensorMap tmap_x, const Params p) {
+  constexpr bool SC_SMEM = EXT == EXT_SCALE_SMEM, SC_GMEM = EXT == EXT_SCALE_GMEM, SCALE = SC_SMEM || SC_GMEM;
+  constexpr bool PROD_BWD = EXT == EXT_PROD_BWD;
+  using C = Cfg<MODE, B_MN, SC_SMEM ? SC_BYTES : 0>;
   constexpr bool BF16 = MODE == 4;
   static_assert(!BF16 || (!A_MN && !B_MN), "bf16x3: A K-major fp32, B the transposed (K-major) bf16 plane");
+  static_assert(!SCALE || BF16 || (MODE == 0 && A_MN && B_MN), "A scale: bf16x3, or single-pass TF32 weight gradient");
+  static_assert(!PROD_BWD || (MODE == 0 && !A_MN && !B_MN), "product backward: single-pass TF32, K-major operands");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* prep = smem + C::STAGES * C::STAGE_BYTES;
@@ -315,11 +406,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int k_tiles_total = (int)((p.K + BK - 1) / BK);
   const int kt0 = blockIdx.y * p.k_tiles_per_split;
   const int num_kt = min(kt0 + p.k_tiles_per_split, k_tiles_total) - kt0;
+  // first row of the M tile: position-aligned tiles hold pos_per_tile whole positions of `group` rows
+  const int m0 = PROD_BWD ? m_blk * p.pos_per_tile * (int)p.group : m_blk * BM;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-    if (C::BLO) tma_prefetch_desc(&tmap_blo);
+    if (C::BLO || SC_SMEM) tma_prefetch_desc(&tmap_x);
     for (int s = 0; s < C::STAGES; ++s) mbar_init(&full[s], 1);
     fence_barrier_init();
   }
@@ -328,16 +421,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   auto issue = [&](int kt) {          // thread 0: k-tile kt -> stage kt % STAGES
     const int s = kt % C::STAGES;
     uint64_t* bar = &full[s];
-    mbar_expect_tx(bar, C::STAGE_BYTES);
+    mbar_expect_tx(bar, C::STAGE_BYTES + (SC_SMEM ? SC_BYTES : 0));
     const uint32_t a_dst = smem_u32(smem + s * C::STAGE_BYTES);
     const uint32_t b_dst = a_dst + TILE_BYTES;
     const int k_elem = (kt0 + kt) * BK;
-    load_operand<A_MN>(a_dst, &tmap_a, bar, m_blk * BM, k_elem);
+    load_operand<A_MN>(a_dst, &tmap_a, bar, m0, k_elem);
     if (BF16) {
       tma_load_2d(b_dst, &tmap_b, bar, (kt0 + kt) * 64, n_blk * BN);    // 128 n-rows x (32 hi | 32 lo) bf16
     } else {
       load_operand<B_MN>(b_dst, &tmap_b, bar, n_blk * BN, k_elem);
-      if (C::BLO) load_operand<B_MN>(b_dst + TILE_BYTES, &tmap_blo, bar, n_blk * BN, k_elem);
+      if (C::BLO) load_operand<B_MN>(b_dst + TILE_BYTES, &tmap_x, bar, n_blk * BN, k_elem);
+    }
+    if (SC_SMEM) {                    // scale rows from the first group the tile's A rows (K-major) / k-rows (MN-major) touch
+      const uint32_t sc_dst = smem_u32(smem + C::SC_OFF + s * SC_BYTES);
+      if (A_MN) tma_load_2d(sc_dst, &tmap_x, bar, m0, (int)((uint32_t)k_elem / p.group));
+      else tma_load_2d(sc_dst, &tmap_x, bar, k_elem, (int)((uint32_t)m0 / p.group));
     }
   };
   // k-tile kt goes to stage kt % STAGES; the stage of kt - 1 is refilled (with kt - 1 + STAGES) during k-tile kt, once
@@ -361,14 +459,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   uint32_t a_off[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) a_off[q] = tile_off<A_MN>(r0 + (q & 1) * 8, t + (q >> 1) * 4);
+  const uint32_t sc0 = smem_u32(smem + C::SC_OFF);           // a_scale slice of stage 0 (shared address)
 
   // One k-tile; BUF = kt & 1 is a compile-time constant (the loop below is unrolled by two) so that the fragments stay
   // in registers.  The MMAs of kt are left in flight while the next k-tile waits for its TMA and stages its operands.
   auto k_tile = [&](const int kt, auto buf_tag) {
     constexpr int BUF = decltype(buf_tag)::value;
     const int s = kt % C::STAGES;
+    const int k_elem = (kt0 + kt) * BK;
+    const uint32_t sc_s = (uint32_t)s * SC_BYTES;              // this k-tile's a_scale slice (EXT_SCALE_SMEM)
     mbar_wait(&full[s], (uint32_t)(kt / C::STAGES) & 1u);
     const uint8_t* sa = smem + s * C::STAGE_BYTES;
+    if (SC_GMEM) {
+      scale_tile_gmem<A_MN>(smem + s * C::STAGE_BYTES, p, m0, k_elem, tid);
+      __syncthreads();                // fragments read elements other threads scaled
+    }
     uint8_t* sb = smem + s * C::STAGE_BYTES + TILE_BYTES;
     // the prep tiles, or (MODE 0) B's own stage: the MMAs of kt - 1, still in flight, read another stage
     uint8_t* pb = C::PREP_TILES ? prep + BUF * C::PREP_TILE_BYTES : sb;
@@ -380,6 +485,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const uint32_t b_hi = smem_u32(pb);
     const uint32_t b_lo = b_hi + TILE_BYTES;        // 3x: the prep B_lo tile
     if (BF16) {
+      // K-major A scale: rows r0 and r0 + 8 read slice row (their group minus the tile's first group), columns 2t (+1)
+      // + 8 i of it.  Recomputed per k-tile: a value kept across the k-loop does not fit in the 128 registers.
+      uint32_t sc_r[2] = {0u, 0u};
+      if (SC_SMEM)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          sc_r[h] = sc0 + sc_s + ((uint32_t)(m0 + r0 + 8 * h) / p.group - (uint32_t)m0 / p.group) * (BK * 4) + 8 * t;
       uint32_t (&ahi)[2][4] = ahi16[BUF];
       uint32_t (&al)[2][4] = alo16[BUF];
 #pragma unroll
@@ -387,7 +499,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const int r = r0 + (q & 1) * 8, k = 16 * j + 2 * t + (q >> 1) * 8;
-          const float2 x = *reinterpret_cast<const float2*>(sa + tile_off<false>(r, k));
+          float2 x = *reinterpret_cast<const float2*>(sa + tile_off<false>(r, k));
+          if (SC_SMEM) {        // __fmul_rn: the product is rounded on its own, never contracted into the split
+            const float2 f = ld_shared_f2(sc_r[q & 1] + (16 * j + (q >> 1) * 8) * 4);
+            x.x = __fmul_rn(x.x, f.x); x.y = __fmul_rn(x.y, f.y);
+          }
           split_bf16x2(x.x, x.y, ahi[j][q], al[j][q]);
         }
       wgmma_fence();
@@ -405,6 +521,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
         for (int q = 0; q < 4; ++q)
           ah[j][q] = *reinterpret_cast<const uint32_t*>(sa + (A_MN ? a_off[q] + 1024 * j : a_off[q] ^ (32 * j)));
+      if (SC_SMEM) {            // MN-major A (the weight gradient): element (m, k) is stored at row k, column m
+        const uint32_t g0 = (uint32_t)k_elem / p.group;
+#pragma unroll
+        for (int h = 0; h < 8; ++h) {                        // k = t + 4 h: fragments q >> 1 = h & 1 of k-step j = h >> 1
+          const int k = t + 4 * h;
+          const int sr = (int)((uint32_t)(k_elem + k) / p.group - g0);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int m = r0 + 8 * i;
+            const float f = ld_shared_f32(sc0 + sc_s + (sr * BM + m) * 4);
+            uint32_t& x = ah[h >> 1][(h & 1) * 2 + i];
+            x = __float_as_uint(__fmul_rn(__uint_as_float(x), f));
+          }
+        }
+      }
       if (C::SPLIT3) {
 #pragma unroll
         for (int j = 0; j < 4; ++j)
@@ -432,12 +563,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     __syncthreads();                  // ... and the other's: stage (kt - 1) % STAGES and prep buffer (kt - 1) & 1 are free
     if (tid == 0 && kt + C::STAGES - 1 < num_kt) issue(kt + C::STAGES - 1);
   };
-  int kt = 0;
-  for (; kt + 1 < num_kt; kt += 2) {
-    k_tile(kt, std::integral_constant<int, 0>());
-    k_tile(kt + 1, std::integral_constant<int, 1>());
+  if (SCALE) {                        // (the same loop without a counter kept past it: the scale leaves no register for it)
+    for (int kt = 0; kt < num_kt; kt += 2) {
+      k_tile(kt, std::integral_constant<int, 0>());
+      if (kt + 1 < num_kt) k_tile(kt + 1, std::integral_constant<int, 1>());
+    }
+  } else {
+    int kt = 0;
+    for (; kt + 1 < num_kt; kt += 2) {
+      k_tile(kt, std::integral_constant<int, 0>());
+      k_tile(kt + 1, std::integral_constant<int, 1>());
+    }
+    if (kt < num_kt) k_tile(kt, std::integral_constant<int, 0>());
   }
-  if (kt < num_kt) k_tile(kt, std::integral_constant<int, 0>());
   wgmma_wait<0>();
   fence_acc(acc);
   __syncthreads();                    // the other warpgroup's last MMAs may still read B from the operand ring
@@ -452,12 +590,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     *reinterpret_cast<float2*>(stage + (r0 + 8) * EPI_LD + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
   }
   __syncthreads();
+  if (PROD_BWD) {
+    prod_bwd_epilogue(p, stage, m_blk, n_blk, tid);
+    return;
+  }
   const int c4 = lane * 4;
   const int64_t col = (int64_t)n_blk * BN + c4;
   if (col >= p.N) return;
   for (int it = 0; it < BM / 8; ++it) {
     const int rl = it * 8 + warp;
-    const int64_t row = (int64_t)m_blk * BM + rl;
+    const int64_t row = (int64_t)m0 + rl;
     if (row >= p.M) break;
     const float4 v = *reinterpret_cast<const float4*>(stage + rl * EPI_LD + c4);
     float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -532,10 +674,23 @@ pack_bf16x3_kernel(const PackDesc* __restrict__ descs) {
   }
 }
 
-template <bool A_MN, bool B_MN, int MODE>
+// a_scale slices for EXT_SCALE_SMEM: scale [n_groups, cols] (row stride ld), boxes of SC_ROWS_K groups x 32 columns (K-major
+// A) or SC_ROWS_MN groups x 128 columns (MN-major A), unswizzled.  Out-of-range groups / columns read zeros.
+static int make_scale_map(const nar_ctx* ctx, CUtensorMap* map, const float* ptr, int64_t n_groups, int64_t cols, int64_t ld, bool a_mn) {
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)n_groups};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+  cuuint32_t box[2] = {a_mn ? (cuuint32_t)BM : (cuuint32_t)BK, a_mn ? (cuuint32_t)SC_ROWS_MN : (cuuint32_t)SC_ROWS_K};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = reinterpret_cast<EncodeTiledFn>(ctx->encode_tiled)(
+      map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? NAR_OK : NAR_ERR_INVALID;
+}
+
+template <bool A_MN, bool B_MN, int MODE, int EXT = 0>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tbl, const Params& p, dim3 grid, cudaStream_t st) {
-  auto kern = gemm_kernel<A_MN, B_MN, MODE>;
-  constexpr int smem = Cfg<MODE, B_MN>::SMEM_BYTES;
+  auto kern = gemm_kernel<A_MN, B_MN, MODE, EXT>;
+  constexpr int smem = Cfg<MODE, B_MN, EXT == EXT_SCALE_SMEM ? SC_BYTES : 0>::SMEM_BYTES;
   static bool attr_set = false;     // per instantiation
   if (!attr_set) {
     NAR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -594,7 +749,27 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   if (bf16 && (!a_kmajor || !epi->b_bf16 || epi->accumulate || epi->split_k > 1)) return NAR_ERR_INVALID;
   const bool blo = epi->precision == 3 && epi->b_lo != nullptr;
   const int mode = bf16 ? 4 : (epi->precision == 1 ? 0 : (blo ? 2 : 1));
-  const int64_t n_tiles = (N + BN - 1) / BN, m_tiles = (M + BM - 1) / BM;
+  const bool scale = epi->a_scale != nullptr, prod_bwd = epi->pred != nullptr;
+  const int64_t a_rows = a_kmajor ? M : K, a_cols = a_kmajor ? K : M;       // A's storage
+  if (scale) {
+    // implemented: bf16x3 (K-major A), and single-pass TF32 with both operands MN-major (the weight gradient)
+    if (!(mode == 4 || (mode == 0 && !a_kmajor && !b_kmajor)) || prod_bwd) return NAR_ERR_INVALID;
+    if (epi->a_scale_group < 1 || a_rows > 0x7fffffffLL || a_cols > 0x7fffffffLL || epi->a_scale_group > a_rows ||
+        epi->ld_a_scale < a_cols || (epi->ld_a_scale & 3) != 0 ||
+        (reinterpret_cast<uintptr_t>(epi->a_scale) & 15u) != 0) return NAR_ERR_INVALID;
+  } else if (epi->a_scale_group != 0 || epi->ld_a_scale != 0) {
+    return NAR_ERR_INVALID;
+  }
+  if (prod_bwd) {
+    const int64_t g = epi->pred_group;
+    if (mode != 0 || !a_kmajor || !b_kmajor || epi->accumulate || epi->split_k > 1 || epi->bias || epi->act) return NAR_ERR_INVALID;
+    if (g < 1 || g > BM || M % g != 0 || !epi->d_pred || !epi->aux || epi->ld_aux < N || epi->ld_pred < N) return NAR_ERR_INVALID;
+  } else if (epi->d_pred || epi->pred_group != 0 || epi->ld_pred != 0) {
+    return NAR_ERR_INVALID;
+  }
+  // position-aligned M tiles: pos_per_tile whole positions of pred_group rows each (the rest of the 128 rows unused)
+  const int64_t pos_per_tile = prod_bwd ? BM / epi->pred_group : 0, n_pos = prod_bwd ? M / epi->pred_group : 0;
+  const int64_t n_tiles = (N + BN - 1) / BN, m_tiles = prod_bwd ? (n_pos + pos_per_tile - 1) / pos_per_tile : (M + BM - 1) / BM;
   if (n_tiles * m_tiles > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
   const int k_tiles = (int)((K + BK - 1) / BK);
   const bool amn = !a_kmajor, bmn = !b_kmajor;
@@ -628,8 +803,25 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   p.M = M; p.N = N; p.K = K; p.D = D; p.ldd = ldd; p.bias = epi->bias; p.aux = epi->aux; p.ld_aux = epi->ld_aux;
   p.act = epi->act; p.dact = epi->dact; p.accumulate = epi->accumulate; p.k_tiles_per_split = per;
   p.n_tiles = (int)n_tiles;
+  p.a_scale = epi->a_scale; p.ld_a_scale = epi->ld_a_scale; p.a_rows = a_rows; p.a_cols = a_cols;
+  p.group = (uint32_t)(scale ? epi->a_scale_group : (prod_bwd ? epi->pred_group : 1));
+  p.pred = epi->pred; p.d_pred = epi->d_pred; p.ld_pred = epi->ld_pred; p.n_pos = n_pos; p.pos_per_tile = (int)pos_per_tile;
   dim3 grid((unsigned)(n_tiles * m_tiles), (unsigned)split, 1);
   cudaStream_t st = as_stream(stream);
+  if (scale) {
+    // the staged slice holds the groups one tile's rows (K-major A: 128) or one k-tile's rows (MN-major A: 32) touch
+    const int64_t span = (a_kmajor ? BM - 1 : BK - 1) / epi->a_scale_group + 2;
+    if (span <= (a_kmajor ? SC_ROWS_K : SC_ROWS_MN)) {
+      rc = make_scale_map(ctx, &tbl, epi->a_scale, (a_rows + epi->a_scale_group - 1) / epi->a_scale_group, a_cols, epi->ld_a_scale,
+                          !a_kmajor);
+      if (rc) return rc;
+      if (mode == 4) return launch<false, false, 4, EXT_SCALE_SMEM>(ta, tb, tbl, p, grid, st);
+      return launch<true, true, 0, EXT_SCALE_SMEM>(ta, tb, tbl, p, grid, st);
+    }
+    if (mode == 4) return launch<false, false, 4, EXT_SCALE_GMEM>(ta, tb, tbl, p, grid, st);
+    return launch<true, true, 0, EXT_SCALE_GMEM>(ta, tb, tbl, p, grid, st);
+  }
+  if (prod_bwd) return launch<false, false, 0, EXT_PROD_BWD>(ta, tb, tbl, p, grid, st);
   if (mode == 4) return launch<false, false, 4>(ta, tb, tbl, p, grid, st);
 #define NAR_GEMM_CASE(a, b) \
   if (amn == a && bmn == b) { \

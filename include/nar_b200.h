@@ -175,6 +175,20 @@ typedef struct {
                              fp32): operand B as the pre-split transposed plane written by nar_pack_bf16x3 - [N, ld_bf16]
                              bf16, row n = per block of 32 k the 32 hi values then the 32 lo values; B / ldb are ignored */
   int64_t ld_bf16;        /* elements per row of b_bf16 (>= ceil(K/32)*64, multiple of 8) */
+  const float* a_scale;   /* optional A scale, defined on A's storage: the stored element A[i*lda + j] enters the MMA as
+                             A[i*lda + j] * a_scale[(i / a_scale_group)*ld_a_scale + j] (one fp32 multiply, rounded), so
+                             a K-major A is scaled per (row group, k) and an MN-major A per (k group, m).  Implemented for
+                             precision 4 and for precision 1 with both operands MN-major (the weight gradient); NULL: none */
+  int64_t ld_a_scale;     /* multiple of 4, >= A's storage row length */
+  int64_t a_scale_group;  /* >= 1 */
+  const float* pred;      /* optional scorer-product backward epilogue (precision 1, K-major A and B, no split-K / bias /
+                             act / accumulate / a_scale): with g = pred_group (1..128, M a multiple of g), row r of the result
+                             v is the gradient of prod[r] = aux[r] * pred[r / g] (aux = the candidate rows, e.g. the CAR
+                             output); D[r] = v[r] * pred[r/g] * dact'(aux[r]) and d_pred[l] = sum over the g rows of
+                             position l, in row order, of v * aux (fmaf chain).  M tiles hold whole positions.  NULL: none */
+  float* d_pred;
+  int64_t ld_pred;        /* row stride of pred and d_pred (>= N) */
+  int64_t pred_group;
 } nar_gemm_epilogue;
 
 /* bf16x3 weight planes for n matrices in one launch: W[i] [K[i], N[i]] fp32 (row stride ldw[i], i.e. stored [in, out]) ->

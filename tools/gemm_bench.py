@@ -5,7 +5,8 @@ Two groups of cases: operand-major / precision variants at 24000 x 1024 x 1024, 
 the shapes bench.py's roofline times (R = 23 600 candidate rows, C = 1024): CAR layer 2 forward (bf16x3, bias + tanh),
 dgrad (single-pass TF32, leaky derivative from a separate aux) and split-K wgrad (single-pass TF32, both operands
 MN-major, split chosen by the library), and the scorer's first layer
-(C -> 128) forward / dgrad / wgrad.  Each step case also reports the share of the data-sheet peak of the tensor path it
+(C -> 128) forward / dgrad / wgrad, also with the scorer product (51 candidates per position) as separate kernels
+(mul_pred + forward, dgrad + mul_pred_bwd) against folded into the GEMMs (A scaled by PR, product backward epilogue).  Each step case also reports the share of the data-sheet peak of the tensor path it
 issues on (bf16 for bf16x3, counting its 3 MMAs per product; TF32 otherwise) and the rate at which TMA fills shared
 memory with operand tiles."""
 import json
@@ -92,6 +93,22 @@ def step_cases(dev):
     c0 = torch.randn(128, device=dev) * 0.1
     dM0 = torch.zeros(C, 128, device=dev)
     M0plane = ops.pack_bf16x3(M0, C, 128)
+    # the scorer product PD = Ec * PR[position] at G1's 51 candidates per position: separate kernels vs folded into M1
+    n_cand = 51
+    L = R // n_cand
+    Rp = L * n_cand
+    Ec = torch.tanh(H1[:Rp])
+    PR = torch.tanh(torch.randn(L, C, device=dev))
+    dEc = torch.empty(Rp, C, device=dev)
+    dPR = torch.empty(L, C, device=dev)
+
+    def mul_pred_fwd():
+        ops.mul_pred(Ec, PR, L, n_cand, C, PD)
+        ops.gemm(PD, None, Z1, Rp, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0))
+
+    def dgrad_mul_pred_bwd():
+        ops.gemm(dZ1, M0, dPD, Rp, C, 128, precision=1)
+        ops.mul_pred_bwd(dPD, Ec, PR, L, n_cand, C, dEc, dPR, cand_act=ops.ACT_TANH)
     return [
         ('step L2 fwd   bf16x3 +bias tanh', lambda: ops.gemm(H1, None, E, R, C, C, ldb=0, bias=b2, act=ops.ACT_TANH, precision=4, b_bf16=W2plane, ld_bf16=W2plane.stride(0)), [R, C, C], E, 4),
         ('step L2 dgrad 1x +dact leaky aux sep', lambda: ops.gemm(dE, W2, dH1, R, C, C, precision=1, dact=ops.ACT_LEAKY, aux=H1), [R, C, C], dH1, 1),
@@ -99,6 +116,11 @@ def step_cases(dev):
         ('step M1 fwd   bf16x3 +bias leaky', lambda: ops.gemm(PD, None, Z1, R, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0)), [R, 128, C], Z1, 4),
         ('step M1 dgrad 1x', lambda: ops.gemm(dZ1, M0, dPD, R, C, 128, precision=1), [R, C, 128], dPD, 1),
         ('step M1 wgrad 1x split-K', lambda: ops.gemm(PD, dZ1, dM0, C, 128, R, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), [C, 128, R], dM0, 1),
+        ('step M1 mul_pred + fwd bf16x3', mul_pred_fwd, [Rp, 128, C], Z1, 4),
+        ('step M1 fwd bf16x3 A scaled by PR', lambda: ops.gemm(Ec, None, Z1, Rp, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0), a_scale=PR, a_scale_group=n_cand), [Rp, 128, C], Z1, 4),
+        ('step M1 dgrad 1x + mul_pred_bwd', dgrad_mul_pred_bwd, [Rp, C, 128], dEc, 1),
+        ('step M1 dgrad 1x product backward epilogue', lambda: ops.gemm(dZ1, M0, dEc, Rp, C, 128, precision=1, dact=ops.ACT_TANH, aux=Ec, pred=PR, d_pred=dPR, pred_group=n_cand), [Rp, C, 128], dEc, 1),
+        ('step M1 wgrad 1x split-K A scaled by PR', lambda: ops.gemm(Ec, dZ1, dM0, C, 128, Rp, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1, a_scale=PR, a_scale_group=n_cand), [C, 128, Rp], dM0, 1),
     ]
 
 
