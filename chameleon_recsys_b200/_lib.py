@@ -168,6 +168,8 @@ _SIGNATURES = {
     'nar_eval_metrics_popcount': (C.c_int, [vp, i64, i64, vp, vp]),
     'nar_eval_by_position': (C.c_int, [vp, i64, i64, i64, i64, i64, i64, i32, vp, i64, vp, i64, vp, i64, vp, i64, vp, vp,
                                        i64, vp, vp, vp]),
+    'nar_eval_session_logs_layout': (C.c_int, [i64, i64, i64, i32, vp]),
+    'nar_eval_session_logs_pack': (C.c_int, [vp, vp, vp, i64, vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = sorted(_SIGNATURES.keys())

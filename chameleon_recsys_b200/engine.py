@@ -650,10 +650,11 @@ class NarEngine:
         self._refresh()
 
     def eval_step(self, features, labels, buffer, pop_norm, top_n: int, metrics: Optional[torch.Tensor] = None,
-                  step_id: Optional[int] = None, keep: bool = False) -> dict:
+                  step_id: Optional[int] = None, keep: bool = False, before_sync=None) -> dict:
         """One evaluation batch: negatives with this engine's (eval) sampling hparams, forward, loss, then
         rank_items_by_predicted_prob (nar_model.py:777-795) and the streaming HR@n / MRR@n sums (:835-885).
-        ``metrics`` [3] float64 device accumulator {hits, sum of reciprocal ranks, valid labels} (counts stay exact)."""
+        ``metrics`` [3] float64 device accumulator {hits, sum of reciprocal ranks, valid labels} (counts stay exact).
+        ``before_sync``: called once the batch is queued, before the host waits for its loss (host work to overlap)."""
         st = self.stage(features, labels, buffer, pop_norm, slot='eval')
         if step_id is not None:
             self.prepare(st, step_id)
@@ -673,6 +674,8 @@ class NarEngine:
         if self.world > 1:
             torch.distributed.all_reduce(self.loss_dev, group=self.pg)
         self.loss_host.copy_(self.loss_dev, non_blocking=True)
+        if before_sync is not None:
+            before_sync()
         torch.cuda.current_stream().synchronize()
         out['xe_loss'] = float(self.loss_host[0]); out['reg_loss'] = float(self.loss_host[1]); out['nov_reg_loss'] = float(self.loss_host[2])
         out['total_loss'] = out['xe_loss'] + out['reg_loss'] - out['nov_reg_loss']

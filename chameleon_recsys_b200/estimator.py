@@ -28,6 +28,8 @@ from .nar_model import ItemsStateUpdaterHook, NARModuleModel
 # Global vars updated by the Estimator hook (nar_trainer_gcom.py:410-415)
 clicked_items_state: Optional[ClickedItemsState] = None
 eval_sessions_metrics_log: list = []
+sessions_negative_items_log: Optional[list] = None                # a list: log every eval session's negatives
+sessions_chameleon_recommendations_log: Optional[list] = None     # a list: log every eval session's ranked candidates
 
 
 @dataclass
@@ -91,6 +93,11 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
         raise RuntimeError('clicked_items_state is not set (nar_trainer_gcom.py:486-489 creates it before the Estimator)')
     hooks = [ItemsStateUpdaterHook(mode, model, eval_metrics_top_n=eval_metrics_top_n, clicked_items_state=state,
                                    eval_sessions_metrics_log=eval_sessions_metrics_log,
+                                   sessions_negative_items_log=_first_set(
+                                       params.get('sessions_negative_items_log'), sessions_negative_items_log),
+                                   sessions_chameleon_recommendations_log=_first_set(
+                                       params.get('sessions_chameleon_recommendations_log'),
+                                       sessions_chameleon_recommendations_log),
                                    content_article_embeddings_matrix=params['content_article_embeddings_matrix'],
                                    articles_metadata=params['articles_metadata'],
                                    eval_negative_sample_relevance=params.get('eval_negative_sample_relevance'),
@@ -111,11 +118,15 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
 
     # ModeKeys.EVAL (nar_trainer_gcom.py:323-332): loss + eval_metric_ops {hitrate_at_n, mrr_at_n}; each "update op" is
     # one call of model.evaluate, the values are read from the device accumulator at the end
-    def eval_update(feats, labs, feed, metrics, step_id=None):
+    def eval_update(feats, labs, feed, metrics, step_id=None, before_sync=None):
         return model.evaluate(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'],
-                              metrics=metrics, step_id=step_id)
+                              metrics=metrics, step_id=step_id, before_sync=before_sync)
     return EstimatorSpec(mode, loss=None, eval_metric_ops={'hitrate_at_n': eval_update, 'mrr_at_n': eval_update},
                          evaluation_hooks=hooks, model=model)
+
+
+def _first_set(a, b):
+    return a if a is not None else b              # (an empty list is a log that is switched on)
 
 
 class Estimator:
@@ -375,16 +386,20 @@ class Estimator:
         metrics = torch.zeros(3, device=spec.model.engine.dev, dtype=torch.float64)
         update = spec.eval_metric_ops['hitrate_at_n']
         n, loss_sum = 0, 0.0
+        # per-session logs: the previous batch's pinned copy becomes list entries while the GPU runs this batch
+        logs = [h.session_logs for h in spec.evaluation_hooks if getattr(h, 'session_logs', None) is not None]
+        overlap = {'before_sync': lambda: [sl.drain() for sl in logs]} if logs else {}
         while nxt is not None:
             features, labels = nxt
             feed = {}
             for h in spec.evaluation_hooks:
                 feed.update(h.before_run(None))
-            out = update(features, labels, feed, metrics, step_id=n + 1)
+            out = update(features, labels, feed, metrics, step_id=n + 1, **overlap)
             run_values = {'clicked_items': features['item_clicked'], 'clicked_timestamps': features['event_timestamp'],
                           'last_item_label': labels['label_last_item'], 'stage': out['stage'],
                           'eval_batch_negative_items': out['negatives'], 'session_ids': features.get('session_id'),
-                          'predicted_item_ids': out.get('predicted_item_ids')}
+                          'predicted_item_ids': out.get('predicted_item_ids'),
+                          'predicted_item_probs': out.get('predicted_item_probs')}
             for h in spec.evaluation_hooks:
                 h.after_run(None, run_values)
             loss_sum += out['total_loss']

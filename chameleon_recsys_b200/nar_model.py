@@ -109,11 +109,11 @@ class NARModuleModel:
         return out
 
     def evaluate(self, features: Dict[str, np.ndarray], labels: Dict[str, np.ndarray], pop_recent_items_buffer: np.ndarray,
-                 articles_recent_pop_norm: np.ndarray, metrics=None, step_id=None) -> dict:
+                 articles_recent_pop_norm: np.ndarray, metrics=None, step_id=None, before_sync=None) -> dict:
         """One EVAL batch (the eval_metric_ops update): loss, ``predicted_item_ids`` / ``predicted_item_probs``
         (nar_model.py:520-524) and the HR@n / MRR@n accumulators (:835-885) for ``metrics_top_n``."""
         out = self.engine.eval_step(features, labels, pop_recent_items_buffer, articles_recent_pop_norm,
-                                    top_n=self.metrics_top_n, metrics=metrics, step_id=step_id)
+                                    top_n=self.metrics_top_n, metrics=metrics, step_id=step_id, before_sync=before_sync)
         self._publish(features, labels, out)
         self.predicted_item_ids = out.get('predicted_item_ids')
         self.predicted_item_probs = out.get('predicted_item_probs')
@@ -159,6 +159,16 @@ class ItemsStateUpdaterHook:
         self.eval_metrics_top_n = eval_metrics_top_n
         self.clicked_items_state = clicked_items_state
         self.eval_sessions_metrics_log = eval_sessions_metrics_log
+        # the per-session logs (nar_model.py:1529-1581): each is on iff its list was given; a session_logs.SessionLogs
+        # object packs them on the GPU and appends to the lists
+        self.sessions_negative_items_log = sessions_negative_items_log
+        self.sessions_chameleon_recommendations_log = sessions_chameleon_recommendations_log
+        self.session_logs_on = mode == ModeKeys.EVAL and (sessions_negative_items_log is not None or
+                                                          sessions_chameleon_recommendations_log is not None)
+        self.session_logs = None
+        if self.session_logs_on and model.engine.world > 1:
+            raise NotImplementedError('the per-session evaluation logs run on one process; data-parallel evaluation of '
+                                      'them is not implemented')
         # NDCG, coverage, novelty and diversity of the model and every baseline (create_eval_metrics, nar_model.py:
         # 1696-1721): an eval_metrics.EvalMetrics accumulator, row 0 the model, rows 1.. the baselines' rows
         self.eval_negative_sample_relevance = eval_negative_sample_relevance
@@ -222,6 +232,13 @@ class ItemsStateUpdaterHook:
                                                   self.clicked_items_state.num_items, self.eval_metrics_top_n,
                                                   self.model.engine.dev)
                 self.by_position.begin()
+            if self.session_logs_on:
+                if self.session_logs is None:
+                    from .session_logs import SessionLogs
+                    self.session_logs = SessionLogs(self.clicked_items_state.num_items, self.model.engine.dev,
+                                                    self.sessions_negative_items_log,
+                                                    self.sessions_chameleon_recommendations_log)
+                self.session_logs.begin()
 
     def before_run(self, run_context=None) -> dict:
         """-> feed dict (nar_model.py:1458-1467)."""
@@ -235,8 +252,17 @@ class ItemsStateUpdaterHook:
         it, then learn from it (nar_model.py:1609-1632).  With the extended metrics on also 'predicted_item_ids' (the
         model's ranked candidates [L, 1+K] on the device, None without queries): the model's and the baselines' top-n
         lists are measured with the popularity the batch was fed with, before the state learns from the batch
-        (:1591-1603).  The hit rate by session position takes the same lists."""
+        (:1591-1603).  The hit rate by session position takes the same lists.  With a per-session log on also
+        'predicted_item_probs' [L, 1+K] and 'session_ids'."""
         ext, bp = self.extended, self.by_position           # set in EVAL only
+        if self.session_logs is not None:
+            st = run_values['stage']
+            t, pred = st['t'], run_values.get('predicted_item_ids')
+            self.session_logs.add(run_values.get('session_ids'), t['label_next'], t['pos_idx'], t['sess_off'], st['L'],
+                                  negatives=run_values['eval_batch_negative_items'], pred_ids=pred,
+                                  pred_probs=run_values.get('predicted_item_probs'),
+                                  cand=None if pred is None else self.model.engine.buffer(st, 'row_item').view(-1)[st['L']:],
+                                  cand_stride=1 if pred is None else pred.shape[1], pop=t['pop_norm'])
         if ext is not None or bp is not None:
             st = run_values['stage']
             pred = run_values.get('predicted_item_ids')
@@ -303,4 +329,6 @@ class ItemsStateUpdaterHook:
 
     def end(self, session=None):
         if self.mode == ModeKeys.EVAL:
+            if self.session_logs is not None:
+                self.session_logs.end()
             self.clicked_items_state.restore_state_checkpoint()     # nar_model.py:1693

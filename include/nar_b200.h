@@ -547,6 +547,26 @@ int nar_eval_by_position(const int64_t* ids, int64_t row_stride, int64_t q_strid
                          int64_t num_items, int64_t* hits, int64_t* total, int64_t ld, float* norm_pop, int* err,
                          void* stream);
 
+/* ---- per-session evaluation logs (csrc/session_logs.cu, spec oracle/session_logs_ref.py; the reference hook's
+ *      sessions_negative_items_log and sessions_chameleon_recommendations_log, nar_model.py:1529-1581).
+ * flags bit 0: the negatives log, bit 1: the recommendations log.  A query is a compact row r < L whose label
+ * label_next[pos_idx[r]] is nonzero; queries are numbered in row order (session-major), Q of them.  The packed buffer:
+ *   int32 {Q, err, 0, 0}, int32 counts [B] (queries of each session), then from 16-byte aligned offsets and with
+ *   Kp = K rounded up to 2, Wp = 1 + K rounded up to 4 (padding columns are 0):
+ *   bit 0: neg [rows, Kp] int64 = negatives[pos_idx[r], :] of each query;
+ *   bit 1: labels [rows] int64 = cand[r * cand_stride]; ids [rows, Wp] int64 = pred_ids[r, :]; probs [rows, Wp] float32 =
+ *          pred_probs[r, :] rounded to 7 decimals as ndarray.round does in float32 (rint(x * 1e7) / 1e7); pops
+ *          [rows, Wp] float32 = pop[ids] rounded the same way.
+ * Only the first Q rows of a section are written.  nar_eval_session_logs_layout: offsets [9] = byte offsets of {counts,
+ * neg, labels, ids, probs, pops}, the total bytes, Kp, Wp, for sections of `rows` rows.  nar_eval_session_logs_pack writes
+ * the buffer `out` (16-byte aligned, laid out for rows = L) in one launch; err is set to 1 (never cleared) when an id of
+ * pred_ids lies outside [0, num_items) (its popularity is written as 0).                                             */
+int nar_eval_session_logs_layout(int64_t B, int64_t rows, int64_t K, int32_t flags, int64_t* offsets);
+int nar_eval_session_logs_pack(const int64_t* pred_ids, const float* pred_probs, const int64_t* cand, int64_t cand_stride,
+                               const int32_t* pos_idx, const int32_t* sess_off, const float* pop, const int64_t* negatives,
+                               const int64_t* label_next, int64_t B, int64_t K, int64_t L, int64_t num_items, int32_t flags,
+                               void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
