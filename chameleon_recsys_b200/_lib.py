@@ -88,7 +88,10 @@ class GemmEpilogue(C.Structure):
                 ('ld_aux', C.c_int64), ('accumulate', C.c_int32), ('split_k', C.c_int32),
                 ('precision', C.c_int32), ('b_lo', C.c_void_p), ('b_bf16', C.c_void_p), ('ld_bf16', C.c_int64),
                 ('a_scale', C.c_void_p), ('ld_a_scale', C.c_int64), ('a_scale_group', C.c_int64),
-                ('pred', C.c_void_p), ('d_pred', C.c_void_p), ('ld_pred', C.c_int64), ('pred_group', C.c_int64)]
+                ('pred', C.c_void_p), ('d_pred', C.c_void_p), ('ld_pred', C.c_int64), ('pred_group', C.c_int64),
+                ('car_pp', C.c_void_p), ('car_pc', C.c_void_p), ('car_pi', C.c_void_p), ('car_pos_idx', C.c_void_p),
+                ('car_neg_uidx', C.c_void_p), ('car_dpp', C.c_void_p), ('car_dpc', C.c_void_p), ('car_dpi', C.c_void_p),
+                ('ld_car', C.c_int64), ('car_k', C.c_int64)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -103,11 +106,10 @@ _SIGNATURES = {
     'nar_ctx_destroy': (C.c_int, [vp]),
     'nar_gather_features': (C.c_int, [vp, C.POINTER(FeaturePlanC), vp, vp, C.POINTER(RowLayout), vp, vp, vp, vp]),
     'nar_gather_features_bwd': (C.c_int, [vp, C.POINTER(FeaturePlanC), vp, vp, C.POINTER(RowLayout), vp, vp, vp, vp, vp, vp]),
-    'nar_build_base_rows': (C.c_int, [vp, i64, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp, i64, vp]),
+    'nar_build_base_rows': (C.c_int, [vp, i64, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp]),
     'nar_sample_negatives_uidx': (C.c_int, [vp, vp, i64, i64, i64, i64, vp, i64, i64, i64, u64, u32, vp, vp,
                                             C.POINTER(vp), C.POINTER(vp), vp, i64, vp]),
     'nar_car_combine': (C.c_int, [vp, vp, vp, vp, vp, i64, i64, i64, C.c_int, vp, vp]),
-    'nar_car_segsum': (C.c_int, [vp, i64, i64, i64, i64, vp, i64, vp, vp, vp, vp, vp, vp]),
     'nar_engine_create': (C.c_int, [vp, C.POINTER(ModelCfg), C.POINTER(vp)]),
     'nar_engine_destroy': (C.c_int, [vp]),
     'nar_engine_update_cfg': (C.c_int, [vp, C.POINTER(ModelCfg)]),

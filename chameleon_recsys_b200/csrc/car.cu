@@ -6,11 +6,10 @@
 // first Dense layer splits exactly into
 //     pre(l, k) = ctx(l) * W1[ctx rows] + b1  +  item(u(l,k)) * W1[item rows]  =  PC[l] + PI[u]
 // with PC computed once per position and PI once per distinct id (two small GEMMs instead of one over all L*(1+K)
-// rows).  This file holds the two HBM-bound kernels around those GEMMs:
+// rows).  This file holds the HBM-bound kernel after those GEMMs:
 //   car_combine_kernel  H1[l, j] = leaky( j == 0 ? PP[l] : PC[l] + PI[u(l, j-1)] )        (forward)
-//   car_segsum_kernel   dPP[l] = dH1[l, 0] ; dPC[l] = sum_k dH1[l, 1+k] ; dPI[u] = sum over the rows that drew u
-// The backward sums run in a fixed order (k ascending; positions ascending through the inverse map Mt built by
-// build_base_rows_kernel), so the result is bit-reproducible - no float atomics.
+// The backward (dPP, dPC = sum over a position's negatives, dPI = sum over the rows that drew u) is formed in the epilogue
+// of the layer-2 dgrad (gemm_wgmma.cu, EXT_CAR_BWD), which recomputes pre from the same operands: dH1 never reaches HBM.
 #include "common.cuh"
 
 namespace nar {
@@ -55,109 +54,6 @@ car_combine_kernel(const float* __restrict__ PP, const float* __restrict__ PC, c
   }
 }
 
-// CTAs [0, L): position sums (dPP copy + dPC over the K negatives).  CTAs [L, L+U): one unique-table entry each.
-__global__ void __launch_bounds__(NT)
-car_segsum_kernel(const float* __restrict__ dH1c, int64_t L, int K, int C, int64_t U, const uint16_t* __restrict__ Mt,
-                  int64_t ld_mt, const int32_t* __restrict__ pos_idx, const int32_t* __restrict__ neg_uidx,
-                  float* __restrict__ dPP, float* __restrict__ dPC, float* __restrict__ dPI) {
-  const int n_cand = K + 1;
-  if ((int64_t)blockIdx.x < L) {
-    const int64_t l = blockIdx.x;
-    const float* in = dH1c + l * n_cand * (int64_t)C;
-    for (int c = threadIdx.x * 4; c < C; c += NT * 4) {
-      *reinterpret_cast<float4*>(dPP + l * C + c) = ld4(in + c);
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      int k = 1;
-      for (; k + 8 <= n_cand; k += 8) {             // 8 loads in flight, added in k order
-        float4 v[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) v[q] = ld4(in + (int64_t)(k + q) * C + c);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) add4(acc, v[q]);
-      }
-      for (; k < n_cand; ++k) add4(acc, ld4(in + (int64_t)k * C + c));
-      *reinterpret_cast<float4*>(dPC + l * C + c) = acc;
-    }
-    return;
-  }
-  // ---- unique entry u: rows (l, k) that drew it, positions ascending.  The rows of a chunk of 256 positions are
-  // compacted into a list (ballot + warp prefix: order kept), then summed 8 at a time: 8 independent 128-bit loads in
-  // flight per thread, added in list order (a popular article is drawn by hundreds of positions - one dependent load
-  // after the other made this kernel 4x slower than the GEMM it follows).
-  __shared__ int s_row[NT * 2], s_warp[NT / 32], s_cnt, s_k0[NT], s_nn[NT];
-  const int64_t u = (int64_t)blockIdx.x - L;
-  const bool pad_slot = (u == U - 1);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  float4 acc[4];                                     // C <= 4 * NT * 4 columns (host checks)
-#pragma unroll
-  for (int i = 0; i < 4; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  auto add_rows = [&](int cnt) {
-    for (int e0 = 0; e0 < cnt; e0 += 8) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = (i * NT + threadIdx.x) * 4;
-        if (c < C) {
-          float4 v[8];
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            v[q] = e0 + q < cnt ? ld4(dH1c + (int64_t)s_row[e0 + q] * C + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) add4(acc[i], v[q]);
-        }
-      }
-    }
-  };
-  for (int64_t l0 = 0; l0 < L; l0 += NT) {
-    const int64_t l = l0 + threadIdx.x;
-    int k0 = 0, n = 0;
-    if (l < L) {
-      if (!pad_slot) {
-        const int m = Mt[u * ld_mt + l];
-        if (m) { k0 = m - 1; n = 1; }
-      } else {
-        // padding negatives (id 0) are the trailing ones of a click: count them from the back
-        const int32_t* uu = neg_uidx + (int64_t)pos_idx[l] * K;
-        int kk = K;
-        while (kk > 0 && uu[kk - 1] == (int32_t)(U - 1)) --kk;
-        k0 = kk; n = K - kk;
-      }
-    }
-    if (!pad_slot) {
-      // ordered compaction of the chunk
-      const unsigned b = __ballot_sync(0xffffffffu, n > 0);
-      if (lane == 0) s_warp[w] = __popc(b);
-      __syncthreads();
-      int base = 0;
-      for (int i = 0; i < w; ++i) base += s_warp[i];
-      if (n > 0) s_row[base + __popc(b & ((1u << lane) - 1u))] = (int)(l * n_cand + 1 + k0);
-      if (threadIdx.x == 0) { int t = 0; for (int i = 0; i < NT / 32; ++i) t += s_warp[i]; s_cnt = t; }
-      __syncthreads();
-      add_rows(s_cnt);
-      __syncthreads();
-    } else {
-      // rare (the pool ran out of candidates): position after position, its trailing padding rows in k order
-      s_k0[threadIdx.x] = k0; s_nn[threadIdx.x] = n;
-      __syncthreads();
-      for (int t = 0; t < NT; ++t) {
-        const int nn = s_nn[t], kk = s_k0[t];              // block-uniform
-        for (int p0 = 0; p0 < nn; p0 += 2 * NT) {
-          const int m = min(2 * NT, nn - p0);
-          __syncthreads();
-          for (int q = threadIdx.x; q < m; q += NT) s_row[q] = (int)((l0 + t) * n_cand + 1 + kk + p0 + q);
-          __syncthreads();
-          add_rows(m);
-        }
-      }
-      __syncthreads();
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int c = (i * NT + threadIdx.x) * 4;
-    if (c < C) *reinterpret_cast<float4*>(dPI + u * C + c) = acc[i];
-  }
-}
-
 }  // namespace car
 }  // namespace nar
 
@@ -168,20 +64,6 @@ extern "C" int nar_car_combine(const float* PP, const float* PC, const float* PI
   if (L <= 0) return NAR_OK;
   nar::car::car_combine_kernel<<<(unsigned)L, nar::car::NT, (size_t)K * sizeof(int32_t), as_stream(stream)>>>(
       PP, PC, PI, pos_idx, neg_uidx, (int)K, (int)C, act, H1c);
-  NAR_LAUNCH_CHECK();
-  return NAR_OK;
-}
-
-extern "C" int nar_car_segsum(const float* dH1c, int64_t L, int64_t K, int64_t C, int64_t U, const uint16_t* Mt, int64_t ld_mt,
-                              const int32_t* pos_idx, const int32_t* neg_uidx, float* dPP, float* dPC, float* dPI, void* stream) {
-  if (!dH1c || !Mt || !pos_idx || !neg_uidx || !dPP || !dPC || !dPI) return NAR_ERR_INVALID;
-  if ((C & 3) || C > 4 * nar::car::NT * 4 || K <= 0 || U <= 0 || ld_mt < L) return NAR_ERR_INVALID;
-  if (L <= 0) {
-    NAR_CHECK_CUDA(cudaMemsetAsync(dPI, 0, (size_t)U * C * sizeof(float), as_stream(stream)));
-    return NAR_OK;
-  }
-  nar::car::car_segsum_kernel<<<(unsigned)(L + U), nar::car::NT, 0, as_stream(stream)>>>(dH1c, L, (int)K, (int)C, U, Mt, ld_mt,
-                                                                                       pos_idx, neg_uidx, dPP, dPC, dPI);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

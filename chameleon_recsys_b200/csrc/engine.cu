@@ -11,8 +11,9 @@
 //   dedup mode     XB [2L+U, Fp] base rows: L clicked, L positives, U unique-negative ITEM rows (csrc/car.cu):
 //                  PP = XB[L:2L] W1 + b1 ; PI = XB[2L:, item cols] W1[item rows] ; PC = XB[:L, ctx cols] W1[ctx rows] + b1
 //                  H1[L + l*n_cand + j] = leaky(j == 0 ? PP[l] : PC[l] + PI[u(l, j-1)])
-//                  backward: DB = [dH1(in) | dPP | dPI | dPC] by fixed-order segment sums, then ONE wgrad / dgrad
-//                  over the 2L+U base rows (+ the context block), instead of two GEMMs over all R rows.
+//                  backward: DB = [dH1(in) | dPP | dPI | dPC], the last three formed in the candidate rows' layer-2
+//                  dgrad epilogue (no dH1 of the candidate rows), then ONE wgrad / dgrad over the 2L+U base rows (+ the
+//                  context block), instead of two GEMMs over all R rows.
 // Streams: the caller's stream carries the critical path (forward, dgrad chain); everything only Adam needs (weight /
 // bias gradients) and the forward session branch run on an engine-owned auxiliary stream behind events.
 #include "common.cuh"
@@ -47,7 +48,7 @@ struct Carver {
 struct PrepBufs {
   void* sampler_ws; int64_t sampler_bytes;
   int64_t* neg; int32_t* neg_uidx; float* stats; int32_t* row_pos; int64_t* row_item;
-  int32_t* base_pos; int64_t* base_item; uint16_t* Mt; int64_t ld_mt, U;
+  int32_t* base_pos; int64_t* base_item; int64_t U;
 };
 
 struct StepBufs {
@@ -110,10 +111,8 @@ int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_
   pb->row_pos = cv.take<int32_t>(Rcap);
   pb->row_item = cv.take<int64_t>(Rcap);
   pb->U = K * 20 + 1;
-  pb->ld_mt = align_up(L_cap > 0 ? L_cap : 1, 8);
   pb->base_pos = cv.take<int32_t>(c.dedup ? 2 * L_cap + pb->U : 1);
   pb->base_item = cv.take<int64_t>(c.dedup ? 2 * L_cap + pb->U : 1);
-  pb->Mt = cv.take<uint16_t>(c.dedup ? pb->U * pb->ld_mt : 1);
   (void)B;
   return cv.off;
 }
@@ -155,7 +154,6 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
     if (c.keep_prob < 1.f)
       for (int i = 0; i < c.layers; ++i) sb->HOd[i] = cv.take<float>(L_cap * Hp);
     if (c.dedup) {
-      sb->dH1 = cv.take<float>(Rc * C);                    // candidate rows only; the input rows' dH1 is DB[0:L]
       sb->DB = cv.take<float>((3 * L_cap + U) * C);
       sb->dX = cv.take<float>(NB * Fp);
     } else {
@@ -251,6 +249,17 @@ struct Seq {
     ep.dact = NAR_ACT_TANH; ep.aux = cand; ep.ld_aux = n_in; ep.split_k = 1; ep.precision = c.bwd_precision;
     ep.pred = pred; ep.d_pred = dpred; ep.ld_pred = n_in; ep.pred_group = group;
     chk(nar_gemm_tf32(e->ctx, M, n_in, n_out, dY, lddy, 1, W(off_W), ldw, 1, dX, n_in, &ep, st));
+  }
+  // through CAR layer 1 of the candidate rows (dedup): v = dY W^T is the gradient of H1c = leaky(pre) (nar_car_combine);
+  // dPP = v * leaky'(pre) of the positives, dPC / dPI += the sums over the negatives (zeroed by the caller)
+  void dgrad_car(const float* dY, int64_t lddy, int64_t off_W, int64_t ldw, const float* PP, const float* PC, const float* PI,
+                 const int32_t* pos_idx, const int32_t* neg_uidx, float* dPP, float* dPC, float* dPI, int64_t M, int64_t n_in,
+                 int64_t n_out, cudaStream_t st) {
+    nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
+    ep.dact = NAR_ACT_LEAKY_RELU; ep.split_k = 1; ep.precision = c.bwd_precision;
+    ep.car_pp = PP; ep.car_pc = PC; ep.car_pi = PI; ep.car_pos_idx = pos_idx; ep.car_neg_uidx = neg_uidx;
+    ep.car_dpp = dPP; ep.car_dpc = dPC; ep.car_dpi = dPI; ep.ld_car = n_in; ep.car_k = c.K;
+    chk(nar_gemm_tf32(e->ctx, M, n_in, n_out, dY, lddy, 1, W(off_W), ldw, 1, nullptr, 0, &ep, st));
   }
   void bgrad(const float* dY, int64_t ld, int64_t rows, int64_t cols, int64_t off_b, cudaStream_t st) {
     chk(nar_colsum_add(dY, rows, cols, ld, G(off_b), st));
@@ -458,13 +467,18 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   // (NAR_BWD_CHAINS=1.  With two chains S keeps its own weight gradients on its stream: sharing the ONE auxiliary stream
   // in enqueue order made the big layer-2 wgrad of C wait behind the last small wgrad of S: 1.22 -> 1.27 ms per G1 step.)
   { const char* v = getenv("NAR_BWD_CHAINS"); s.two_chains = s.use_aux && v && atoi(v) != 0; }
+  // the candidate rows' layer-2 weight gradient needs only dEc: queued on the auxiliary stream before S, the longest
+  // kernel of that stream starts as soon as dEc exists
+  { cudaStream_t st = s.fork(); s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st); s.bgrad(dEc, C, Rc, C, c.off_b2, st); }
   { cudaStream_t ss = s.fork2(); session_backward(ss); }
   // ---- C: CAR layer 2 of the candidate rows (shared weights: the clicked rows follow once S has produced their dE)
-  { cudaStream_t st = s.fork(); s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st); s.bgrad(dEc, C, Rc, C, c.off_b2, st); }
-  float* dH1c = c.dedup ? sb.dH1 : sb.dH1 + L * C;
-  s.dgrad(dEc, C, c.off_W2, C, dH1c, C, Rc, C, C, NAR_ACT_LEAKY_RELU, H1c, C, 0, main);
   float* DBin = sb.DB; float* DBpp = sb.DB + L * C; float* DBpi = sb.DB + 2 * L * C; float* DBpc = sb.DB + NB * C;
-  if (c.dedup) s.chk(nar_car_segsum(sb.dH1, L, K, C, U, pb.Mt, pb.ld_mt, io->pos_idx, pb.neg_uidx, DBpp, DBpc, DBpi, main));
+  if (c.dedup) {
+    s.chk((int)cudaMemsetAsync(DBpi, 0, (size_t)(U + L) * C * sizeof(float), main));       // dPI | dPC: red.add targets
+    s.dgrad_car(dEc, C, c.off_W2, C, sb.PP, sb.PC, sb.PI, io->pos_idx, pb.neg_uidx, DBpp, DBpc, DBpi, Rc, C, C, main);
+  } else {
+    s.dgrad(dEc, C, c.off_W2, C, sb.dH1 + L * C, C, Rc, C, C, NAR_ACT_LEAKY_RELU, H1c, C, 0, main);
+  }
   s.join2();                                       // dE[0:L] is final
   { cudaStream_t st = s.fork(); s.wgrad(sb.H1, C, sb.dE, C, c.off_W2, C, C, C, L, st); s.bgrad(sb.dE, C, L, C, c.off_b2, st); }
   if (c.dedup) {
@@ -762,8 +776,8 @@ extern "C" int nar_engine_prepare(nar_engine* e, const nar_step_io* io, void* st
   if (rc) return rc;
   if (c.dedup) {
     rc = nar_build_base_rows(io->pos_idx, L, io->item_clicked, io->label_next, uitems, n_unique, pb.U, pb.neg_uidx, K, pb.base_pos,
-                             pb.base_item, pb.Mt, pb.ld_mt, st);
-    e->launches += 2;
+                             pb.base_item, st);
+    ++e->launches;
   }
   return rc;
 }
@@ -816,9 +830,9 @@ extern "C" int nar_engine_buffer(const nar_engine* e, const nar_step_io* io, con
   const Ent tab[] = {
       {"neg", pb.neg, io->Bg * io->T, K}, {"neg_uidx", pb.neg_uidx, io->Bg * io->T, K}, {"stats", pb.stats, 1, 24},
       {"row_pos", pb.row_pos, R, 1}, {"row_item", pb.row_item, R, 1}, {"base_pos", pb.base_pos, NB, 1},
-      {"base_item", pb.base_item, NB, 1}, {"Mt", pb.Mt, pb.U, pb.ld_mt},
+      {"base_item", pb.base_item, NB, 1},
       {"X", sb.X, c.dedup ? NB : R, c.Fp}, {"dX", sb.dX, c.dedup ? NB : R, c.Fp}, {"H1", sb.H1, R, c.C}, {"E", sb.E, R, c.C},
-      {"dE", sb.dE, R, c.C}, {"dH1", sb.dH1, c.dedup ? Rc : R, c.C}, {"F1", sb.F1, L, 512}, {"PR", sb.PR, L, c.C},
+      {"dE", sb.dE, R, c.C}, {"dH1", sb.dH1, R, c.C}, {"F1", sb.F1, L, 512}, {"PR", sb.PR, L, c.C},
       {"logits", sb.logits, L, n_cand}, {"PD", sb.PD, Rc, c.C}, {"Z1", sb.Z1, Rc, 128}, {"Z2", sb.Z2, Rc, 64}, {"Z3", sb.Z3, Rc, 32}, {"PP", sb.PP, L, c.C},
       {"PI", sb.PI, pb.U, c.C}, {"PC", sb.PC, L, c.C}, {"DB", sb.DB, 3 * L + pb.U, c.C},
       {"HO0", sb.HO[0], L, c.Hp}, {"HO1", sb.HO[1], L, c.Hp}, {"HO2", sb.HO[2], L, c.Hp}, {"HO3", sb.HO[3], L, c.Hp},

@@ -541,32 +541,21 @@ build_rows_kernel(const int32_t* __restrict__ pos_idx, int64_t L, const int64_t*
 
 // Base rows of the per-unique-id CAR layer 1 (engine.cu): [0,L) clicked items, [L,2L) positives, then one row per
 // entry of the step's unique-negative table (U = table capacity + 1: unused entries and the last "padding negative"
-// slot hold item 0; their context columns are written as 0).  Also fills the inverse map used by the deterministic
-// backward segment sum: Mt[u][l] = k+1 when position l drew unique item u as its k-th negative (a click's non-padding
-// negatives are distinct, so a (u, l) cell has at most one writer).  Mt must be zero on entry.
+// slot hold item 0; their context columns are written as 0).
 __global__ void __launch_bounds__(256)
 build_base_rows_kernel(const int32_t* __restrict__ pos_idx, int64_t L, const int64_t* __restrict__ item_clicked,
                        const int64_t* __restrict__ label_next, const int64_t* __restrict__ uitems,
-                       const int32_t* __restrict__ n_unique_p, int64_t U, const int32_t* __restrict__ neg_uidx, int64_t K,
-                       int32_t* __restrict__ base_pos, int64_t* __restrict__ base_item, uint16_t* __restrict__ Mt,
-                       int64_t ld_mt) {
-  const int64_t n_base = 2 * L + U, total = n_base + L * K;
+                       const int32_t* __restrict__ n_unique_p, int64_t U, int32_t* __restrict__ base_pos,
+                       int64_t* __restrict__ base_item) {
+  const int64_t n_base = 2 * L + U;
   const int n_unique = n_unique_p[0];
   const int32_t pos0 = pos_idx[0];
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    if (i < n_base) {
-      int32_t pos; int64_t item;
-      if (i < L) { pos = pos_idx[i]; item = item_clicked[pos]; }
-      else if (i < 2 * L) { pos = pos_idx[i - L]; item = label_next[pos]; }
-      else { const int64_t u = i - 2 * L; pos = pos0; item = u < n_unique ? uitems[u] : 0; }
-      base_pos[i] = pos; base_item[i] = item;
-    } else {
-      const int64_t e = i - n_base, l = e / K, k = e - l * K;
-      const int32_t u = neg_uidx[(int64_t)pos_idx[l] * K + k];
-      // the padding slot U-1 may be drawn several times by one click (trailing id-0 negatives): its rows are found
-      // by scanning neg_uidx instead (car_segsum_kernel), so it has no cell here
-      if (u >= 0 && u < U - 1) Mt[(int64_t)u * ld_mt + l] = (uint16_t)(k + 1);
-    }
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_base; i += (int64_t)gridDim.x * blockDim.x) {
+    int32_t pos; int64_t item;
+    if (i < L) { pos = pos_idx[i]; item = item_clicked[pos]; }
+    else if (i < 2 * L) { pos = pos_idx[i - L]; item = label_next[pos]; }
+    else { const int64_t u = i - 2 * L; pos = pos0; item = u < n_unique ? uitems[u] : 0; }
+    base_pos[i] = pos; base_item[i] = item;
   }
 }
 
@@ -575,17 +564,15 @@ build_base_rows_kernel(const int32_t* __restrict__ pos_idx, int64_t L, const int
 
 extern "C" int nar_build_base_rows(const int32_t* pos_idx, int64_t L, const int64_t* item_clicked, const int64_t* label_next_item,
                                    const int64_t* unique_items, const int32_t* n_unique, int64_t U, const int32_t* neg_uidx,
-                                   int64_t K, int32_t* base_pos, int64_t* base_item, uint16_t* Mt, int64_t ld_mt, void* stream) {
-  if (!pos_idx || !item_clicked || !label_next_item || !unique_items || !n_unique || !neg_uidx || !base_pos || !base_item || !Mt)
+                                   int64_t K, int32_t* base_pos, int64_t* base_item, void* stream) {
+  if (!pos_idx || !item_clicked || !label_next_item || !unique_items || !n_unique || !neg_uidx || !base_pos || !base_item)
     return NAR_ERR_INVALID;
-  if (K <= 0 || K >= 65535 || U <= 0 || ld_mt < L) return NAR_ERR_INVALID;
+  if (K <= 0 || U <= 0) return NAR_ERR_INVALID;
   if (L <= 0) return NAR_OK;
-  NAR_CHECK_CUDA(cudaMemsetAsync(Mt, 0, (size_t)U * (size_t)ld_mt * sizeof(uint16_t), as_stream(stream)));
-  const int64_t total = 2 * L + U + L * K;
+  const int64_t total = 2 * L + U;
   int64_t g = (total + 255) / 256; if (g > NAR_GRID_SMS * 8) g = NAR_GRID_SMS * 8;
   nar::feat::build_base_rows_kernel<<<(unsigned)g, 256, 0, as_stream(stream)>>>(pos_idx, L, item_clicked, label_next_item,
-                                                                              unique_items, n_unique, U, neg_uidx, K,
-                                                                              base_pos, base_item, Mt, ld_mt);
+                                                                              unique_items, n_unique, U, base_pos, base_item);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

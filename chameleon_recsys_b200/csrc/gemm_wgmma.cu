@@ -55,7 +55,9 @@ constexpr int EPI_LD = BN + 4;               // floats per staged accumulator ro
 //                   the k-tile's k groups (at most SC_ROWS_MN) x 128 m; SC_BYTES per stage either way
 //   EXT_SCALE_GMEM  A scale read from global memory at the fragment: any group size (those whose slices do not fit)
 //   EXT_PROD_BWD    scorer-product backward epilogue (nar_gemm_epilogue.pred): position-aligned M tiles
-constexpr int EXT_SCALE_SMEM = 1, EXT_SCALE_GMEM = 2, EXT_PROD_BWD = 3;
+//   EXT_CAR_BWD     CAR layer-1 backward epilogue (nar_gemm_epilogue.car_*): the gradients of PP / PC / PI, no D
+//                   (TF32 or 3xTF32 with B split in-kernel, K-major operands)
+constexpr int EXT_SCALE_SMEM = 1, EXT_SCALE_GMEM = 2, EXT_PROD_BWD = 3, EXT_CAR_BWD = 4;
 constexpr int SC_ROWS_K = 32, SC_ROWS_MN = 8;
 constexpr int SC_BYTES = 4096;
 static_assert(SC_ROWS_K * BK * 4 == SC_BYTES && SC_ROWS_MN * BM * 4 == SC_BYTES, "a_scale slice per stage");
@@ -93,6 +95,10 @@ struct Params {
   const float* a_scale; int64_t ld_a_scale, a_rows, a_cols; uint32_t group;
   // EXT_PROD_BWD: M tile m_blk = positions [m_blk * pos_per_tile, ...), `group` rows each, n_pos positions in all
   const float* pred; float* d_pred; int64_t ld_pred, n_pos; int pos_per_tile;
+  // EXT_CAR_BWD: row r = slot r % (car_k + 1) of position r / (car_k + 1); [L | L | U, ld_car] pre-activation parts and
+  // their gradients
+  const float *car_pp, *car_pc, *car_pi; const int32_t *car_pos_idx, *car_neg_uidx;
+  float *car_dpp, *car_dpc, *car_dpi; int64_t ld_car; int car_k;
 };
 
 // ---------------------------------------------------------------- PTX wrappers
@@ -372,6 +378,86 @@ __device__ __forceinline__ void prod_bwd_epilogue(const Params& p, const float* 
   }
 }
 
+// EXT_CAR_BWD row of the tile (thread tid < BM): its position l (-1 past M) and the unique-table index u of a negative
+// (slot j >= 1; -1 for the positive).  Loaded before the main loop, so that the two dependent index loads complete under
+// it; the epilogue reads them from shared memory (s_l / s_u).
+__device__ __forceinline__ void car_bwd_row(const Params& p, int m0, int tid, int32_t& l, int32_t& u) {
+  l = -1; u = -1;
+  const int row = m0 + tid, n_cand = p.car_k + 1;
+  if (tid >= BM || row >= p.M) return;
+  l = row / n_cand;
+  const int j = row - l * n_cand;
+  if (j > 0) u = __ldg(p.car_neg_uidx + (int64_t)__ldg(p.car_pos_idx + l) * p.car_k + j - 1);
+}
+
+// EXT_CAR_BWD epilogue: `stage` holds v = dL/dH1 of the tile's rows, H1 = act(pre) with pre = PP[l] for the positive and
+// PC[l] + PI[u] for a negative - the same fp32 add of the same operands as car_combine_kernel, so act'(pre) is bit for
+// bit the factor the plain dgrad takes from H1.  g = v * act'(pre):
+//   positive   dPP[l] = g (the row's only writer)
+//   negative   dPI[u] += g (red.add: a popular u is drawn by many positions), and g stays in `stage` for
+//   dPC[l] += the sum of the tile's negative rows of l in ascending row order, one red.add per (position, column).  With
+//              1 + K <= 128 a position's rows lie in at most two M tiles, so dPC gets at most two adds onto zero and is
+//              bit-reproducible (commutative); dPI is not (float atomics in launch order).
+__device__ __forceinline__ void car_bwd_epilogue(const Params& p, float* stage, const int32_t* s_l, const int32_t* s_u, int m0,
+                                                 int n_blk, int tid) {
+  constexpr int RB = 8;               // rows per batch: their L2 gathers are all in flight before the dependent arithmetic
+  const int warp = tid >> 5, c4 = (tid & 31) * 4;
+  const int64_t col = (int64_t)n_blk * BN + c4;
+  const int64_t ld = p.ld_car;
+  if (col < p.N) {                    // N % 4 == 0 (host checks)
+#pragma unroll 1
+    for (int it0 = 0; it0 < BM / 8; it0 += RB) {
+      float4 a[RB], b[RB];
+#pragma unroll
+      for (int q = 0; q < RB; ++q) {
+        const int rl = (it0 + q) * 8 + warp;
+        const int l = s_l[rl], u = s_u[rl];
+        if (l < 0) continue;
+        if (u < 0) {
+          a[q] = __ldg(reinterpret_cast<const float4*>(p.car_pp + l * ld + col));
+        } else {
+          a[q] = __ldg(reinterpret_cast<const float4*>(p.car_pi + u * ld + col));
+          b[q] = __ldg(reinterpret_cast<const float4*>(p.car_pc + l * ld + col));
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < RB; ++q) {
+        const int rl = (it0 + q) * 8 + warp;
+        const int l = s_l[rl], u = s_u[rl];
+        if (l < 0) continue;
+        const float4 pre = u < 0 ? a[q] : make_float4(a[q].x + b[q].x, a[q].y + b[q].y, a[q].z + b[q].z, a[q].w + b[q].w);
+        float4* sv = reinterpret_cast<float4*>(stage + rl * EPI_LD + c4);
+        float4 g = *sv;
+        g.x *= act_grad_from_output(apply_act(pre.x, p.dact), p.dact);
+        g.y *= act_grad_from_output(apply_act(pre.y, p.dact), p.dact);
+        g.z *= act_grad_from_output(apply_act(pre.z, p.dact), p.dact);
+        g.w *= act_grad_from_output(apply_act(pre.w, p.dact), p.dact);
+        if (u < 0) {
+          *reinterpret_cast<float4*>(p.car_dpp + l * ld + col) = g;
+        } else {
+          atomicAdd(reinterpret_cast<float4*>(p.car_dpi + u * ld + col), g);     // red.global.add.v4.f32
+          *sv = g;
+        }
+      }
+    }
+  }
+  __syncthreads();                    // the per-position sums read other warps' rows of `stage`
+  const int n_cand = p.car_k + 1;
+  const int last = (int)min((int64_t)m0 + BM, p.M) - 1, l0 = m0 / n_cand;
+  const int n_pos = last / n_cand - l0 + 1;
+  for (int idx = tid; idx < n_pos * BN; idx += NUM_THREADS) {
+    const int c = idx % BN, l = l0 + idx / BN;
+    const int64_t colc = (int64_t)n_blk * BN + c;
+    const int r_beg = max(l * n_cand + 1, m0), r_end = min((l + 1) * n_cand, last + 1);
+    if (colc >= p.N || r_beg >= r_end) continue;
+    const float* v = stage + (r_beg - m0) * EPI_LD + c;
+    float acc = v[0];
+#pragma unroll 8
+    for (int r = 1; r < r_end - r_beg; ++r) acc += v[r * EPI_LD];
+    atomicAdd(p.car_dpc + l * ld + colc, acc);
+  }
+}
+
 // TMA for one 128 x 32 fp32 operand tile at MN coordinate mn0, K element k_elem
 template <bool MN_MAJOR>
 __device__ __forceinline__ void load_operand(uint32_t dst, const CUtensorMap* map, uint64_t* bar, int mn0, int k_elem) {
@@ -390,12 +476,14 @@ __global__ void __launch_bounds__(NUM_THREADS, (Cfg<MODE, B_MN>::CTAS_PER_SM))
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_x, const Params p) {
   constexpr bool SC_SMEM = EXT == EXT_SCALE_SMEM, SC_GMEM = EXT == EXT_SCALE_GMEM, SCALE = SC_SMEM || SC_GMEM;
-  constexpr bool PROD_BWD = EXT == EXT_PROD_BWD;
+  constexpr bool PROD_BWD = EXT == EXT_PROD_BWD, CAR_BWD = EXT == EXT_CAR_BWD;
   using C = Cfg<MODE, B_MN, SC_SMEM ? SC_BYTES : 0>;
   constexpr bool BF16 = MODE == 4;
   static_assert(!BF16 || (!A_MN && !B_MN), "bf16x3: A K-major fp32, B the transposed (K-major) bf16 plane");
   static_assert(!SCALE || BF16 || (MODE == 0 && A_MN && B_MN), "A scale: bf16x3, or single-pass TF32 weight gradient");
   static_assert(!PROD_BWD || (MODE == 0 && !A_MN && !B_MN), "product backward: single-pass TF32, K-major operands");
+  static_assert(!CAR_BWD || ((MODE == 0 || MODE == 1) && !A_MN && !B_MN), "CAR backward: TF32 / 3xTF32, K-major operands");
+  static_assert(!CAR_BWD || C::STAGES * C::STAGE_BYTES >= (BM * EPI_LD + 2 * BM) * 4, "CAR backward: row slots behind the staged rows");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* prep = smem + C::STAGES * C::STAGE_BYTES;
@@ -442,6 +530,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   // the MMAs of kt - 1 are done, so STAGES - 1 k-tiles are ahead of the one being multiplied
   if (tid == 0)
     for (int kt = 0; kt < C::STAGES - 1 && kt < num_kt; ++kt) issue(kt);
+  int32_t car_l = -1, car_u = -1;
+  if (CAR_BWD) car_bwd_row(p, m0, tid, car_l, car_u);
 
   // wgmma fragments: warp w (of 8) owns tile rows [16w, 16w + 16); lane = 4 g + t.  A: rows 16w + g (+8), k t (+4)
   // for tf32, k 2t (+8) for bf16 pairs.  D: rows 16w + g (+8), columns 8j + 2t (+1).
@@ -583,6 +673,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   // ===== epilogue: the accumulators go through shared memory (the operand ring is idle now) so that each warp then
   // handles 128 contiguous bytes of one row of D / aux per instruction
   float* stage = reinterpret_cast<float*>(smem);
+  int32_t* s_l = reinterpret_cast<int32_t*>(stage + BM * EPI_LD);      // EXT_CAR_BWD: [BM] positions | [BM] slots
+  int32_t* s_u = s_l + BM;
+  if (CAR_BWD && tid < BM) { s_l[tid] = car_l; s_u[tid] = car_u; }
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int c = 8 * j + 2 * t;
@@ -592,6 +685,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   __syncthreads();
   if (PROD_BWD) {
     prod_bwd_epilogue(p, stage, m_blk, n_blk, tid);
+    return;
+  }
+  if (CAR_BWD) {
+    car_bwd_epilogue(p, stage, s_l, s_u, m0, n_blk, tid);
     return;
   }
   const int c4 = lane * 4;
@@ -739,11 +836,13 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
                              const nar_gemm_epilogue* epi, void* stream) {
   using namespace nar::gemm;
   if (!ctx || !ctx->encode_tiled) return NAR_ERR_NO_DEVICE;
-  if (!A || !D || !epi || (!B && epi->precision != 4)) return NAR_ERR_INVALID;
+  if (!A || !epi || (!B && epi->precision != 4)) return NAR_ERR_INVALID;
+  const bool car_bwd = epi->car_pp != nullptr;       // writes the CAR layer-1 gradients instead of D
+  if (car_bwd ? D != nullptr : !D) return NAR_ERR_INVALID;
   if (M <= 0 || N <= 0 || K <= 0) return NAR_OK;     // empty problem: nothing to do
   if ((ldd & 3) != 0 || (reinterpret_cast<uintptr_t>(D) & 15u) != 0) return NAR_ERR_INVALID;
   if (epi->bias && (reinterpret_cast<uintptr_t>(epi->bias) & 15u) != 0) return NAR_ERR_INVALID;
-  if (epi->dact && (!epi->aux || (epi->ld_aux & 3) != 0 || (reinterpret_cast<uintptr_t>(epi->aux) & 15u) != 0)) return NAR_ERR_INVALID;
+  if (epi->dact && !car_bwd && (!epi->aux || (epi->ld_aux & 3) != 0 || (reinterpret_cast<uintptr_t>(epi->aux) & 15u) != 0)) return NAR_ERR_INVALID;
   if (epi->precision != 1 && epi->precision != 3 && epi->precision != 4) return NAR_ERR_INVALID;
   const bool bf16 = epi->precision == 4;
   if (bf16 && (!a_kmajor || !epi->b_bf16 || epi->accumulate || epi->split_k > 1)) return NAR_ERR_INVALID;
@@ -765,6 +864,20 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
     if (mode != 0 || !a_kmajor || !b_kmajor || epi->accumulate || epi->split_k > 1 || epi->bias || epi->act) return NAR_ERR_INVALID;
     if (g < 1 || g > BM || M % g != 0 || !epi->d_pred || !epi->aux || epi->ld_aux < N || epi->ld_pred < N) return NAR_ERR_INVALID;
   } else if (epi->d_pred || epi->pred_group != 0 || epi->ld_pred != 0) {
+    return NAR_ERR_INVALID;
+  }
+  if (car_bwd) {
+    const int64_t kk = epi->car_k, ld = epi->ld_car;
+    auto al16 = [](const void* q) { return q && (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
+    if ((mode != 0 && mode != 1) || !a_kmajor || !b_kmajor || epi->accumulate || epi->split_k > 1 || epi->bias || epi->act ||
+        epi->aux || scale || prod_bwd) return NAR_ERR_INVALID;
+    // row, position and table indices in 32 bits
+    if (kk < 1 || kk > 0x7fffffffLL - 1 || M > 0x7fffffffLL - BM || M % (kk + 1) != 0 || (N & 3) != 0 || ld < N || (ld & 3) != 0)
+      return NAR_ERR_INVALID;
+    if (!al16(epi->car_pp) || !al16(epi->car_pc) || !al16(epi->car_pi) || !al16(epi->car_dpp) || !al16(epi->car_dpc) ||
+        !al16(epi->car_dpi) || !epi->car_pos_idx || !epi->car_neg_uidx) return NAR_ERR_INVALID;
+  } else if (epi->car_pc || epi->car_pi || epi->car_pos_idx || epi->car_neg_uidx || epi->car_dpp || epi->car_dpc || epi->car_dpi ||
+             epi->ld_car != 0 || epi->car_k != 0) {
     return NAR_ERR_INVALID;
   }
   // position-aligned M tiles: pos_per_tile whole positions of pred_group rows each (the rest of the 128 rows unused)
@@ -806,6 +919,9 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   p.a_scale = epi->a_scale; p.ld_a_scale = epi->ld_a_scale; p.a_rows = a_rows; p.a_cols = a_cols;
   p.group = (uint32_t)(scale ? epi->a_scale_group : (prod_bwd ? epi->pred_group : 1));
   p.pred = epi->pred; p.d_pred = epi->d_pred; p.ld_pred = epi->ld_pred; p.n_pos = n_pos; p.pos_per_tile = (int)pos_per_tile;
+  p.car_pp = epi->car_pp; p.car_pc = epi->car_pc; p.car_pi = epi->car_pi; p.car_pos_idx = epi->car_pos_idx;
+  p.car_neg_uidx = epi->car_neg_uidx; p.car_dpp = epi->car_dpp; p.car_dpc = epi->car_dpc; p.car_dpi = epi->car_dpi;
+  p.ld_car = epi->ld_car; p.car_k = (int)epi->car_k;
   dim3 grid((unsigned)(n_tiles * m_tiles), (unsigned)split, 1);
   cudaStream_t st = as_stream(stream);
   if (scale) {
@@ -822,6 +938,10 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
     return launch<true, true, 0, EXT_SCALE_GMEM>(ta, tb, tbl, p, grid, st);
   }
   if (prod_bwd) return launch<false, false, 0, EXT_PROD_BWD>(ta, tb, tbl, p, grid, st);
+  if (car_bwd) {                      // the engine's backward precision: single-pass TF32, or 3xTF32 splitting B in-kernel
+    if (mode == 0) return launch<false, false, 0, EXT_CAR_BWD>(ta, tb, tbl, p, grid, st);
+    return launch<false, false, 1, EXT_CAR_BWD>(ta, tb, tbl, p, grid, st);
+  }
   if (mode == 4) return launch<false, false, 4>(ta, tb, tbl, p, grid, st);
 #define NAR_GEMM_CASE(a, b) \
   if (amn == a && bmn == b) { \

@@ -494,7 +494,7 @@ class NarEngine:
         return st
 
     _INT_BUFFERS = {'neg': torch.int64, 'row_item': torch.int64, 'base_item': torch.int64, 'neg_uidx': torch.int32,
-                    'row_pos': torch.int32, 'base_pos': torch.int32, 'Mt': torch.int16}
+                    'row_pos': torch.int32, 'base_pos': torch.int32}
 
     def buffer(self, st: dict, name: str) -> torch.Tensor:
         """Device view of a named intermediate of the step staged in ``st`` (see nar_engine_buffer)."""

@@ -126,13 +126,11 @@ int nar_build_rows(const int32_t* pos_idx, int64_t L, const int64_t* item_clicke
 
 /* base rows of the per-unique-id CAR layer 1 (csrc/car.cu): n_base = 2L + U rows = the L clicked items, the L positives,
  * then one ITEM-ONLY row per entry of the step's unique-negative table (unique_items / n_unique as returned by
- * nar_sample_negatives_uidx; U = table capacity K*20 plus one trailing slot for the padding negative, id 0).  Also
- * writes the inverse map Mt [U, ld_mt] uint16: Mt[u][l] = k+1 when position l drew unique entry u as its k-th
- * negative (neg_uidx [B*T, K]), 0 otherwise - what nar_car_segsum walks to sum gradients in a fixed order.         */
+ * nar_sample_negatives_uidx; U = table capacity K*20 plus one trailing slot for the padding negative, id 0).         */
 int nar_build_base_rows(const int32_t* pos_idx, int64_t L, const int64_t* item_clicked, const int64_t* label_next_item,
                         const int64_t* unique_items, const int32_t* n_unique /*[1] device*/, int64_t U,
                         const int32_t* neg_uidx, int64_t K, int32_t* base_pos /*[2L+U]*/, int64_t* base_item /*[2L+U]*/,
-                        uint16_t* Mt, int64_t ld_mt, void* stream);
+                        void* stream);
 
 /* normalisation statistics of recency / novelty over the first n_norm nonzero buffer entries
  * (nar_model.py:1062-1089, :1150-1193, :1011-1039).  stats[g][8], g = 0 input / 1 positive /
@@ -189,6 +187,23 @@ typedef struct {
   float* d_pred;
   int64_t ld_pred;        /* row stride of pred and d_pred (>= N) */
   int64_t pred_group;
+  const float* car_pp;    /* optional CAR layer-1 backward epilogue (precision 1, or 3 without b_lo; K-major A and B, no split-K / bias / act /
+                             accumulate / aux / a_scale / pred; D must be NULL; N a multiple of 4): row r of the result v is
+                             the gradient of H1c[r] = dact(pre) for candidate j = r % (car_k+1) of position l = r / (car_k+1),
+                             pre = j == 0 ? car_pp[l] : car_pc[l] + car_pi[u], u = car_neg_uidx[car_pos_idx[l]*car_k + j-1]
+                             (the rows nar_car_combine writes).  With g = v * dact'(pre): car_dpp[l] = g of j == 0;
+                             car_dpc[l] += sum of g over j >= 1 and car_dpi[u] += g, float atomics into buffers the caller
+                             zeroes (car_dpc is bit-reproducible for car_k < 128, car_dpi is not).  All [rows, ld_car], 16-byte
+                             aligned.  NULL: none */
+  const float* car_pc;
+  const float* car_pi;
+  const int32_t* car_pos_idx;
+  const int32_t* car_neg_uidx;
+  float* car_dpp;
+  float* car_dpc;
+  float* car_dpi;
+  int64_t ld_car;         /* row stride of the six car_ tensors (>= N, multiple of 4) */
+  int64_t car_k;          /* negatives per position (K) */
 } nar_gemm_epilogue;
 
 /* bf16x3 weight planes for n matrices in one launch: W[i] [K[i], N[i]] fp32 (row stride ldw[i], i.e. stored [in, out]) ->
@@ -248,9 +263,7 @@ int nar_sample_negatives_uidx(nar_ctx* ctx, const int64_t* all_items_global, int
 int nar_car_combine(const float* PP /*[L,C]*/, const float* PC /*[L,C]*/, const float* PI /*[U,C]*/,
                     const int32_t* pos_idx, const int32_t* neg_uidx, int64_t L, int64_t K, int64_t C, int act,
                     float* H1c, void* stream);
-/* backward: dPP[l] = dH1c[l,0]; dPC[l] = sum_k dH1c[l,1+k]; dPI[u] = sum of the rows that drew u (fixed order).   */
-int nar_car_segsum(const float* dH1c, int64_t L, int64_t K, int64_t C, int64_t U, const uint16_t* Mt, int64_t ld_mt,
-                   const int32_t* pos_idx, const int32_t* neg_uidx, float* dPP, float* dPC, float* dPI, void* stream);
+/* (its backward is the layer-2 dgrad's epilogue: nar_gemm_epilogue.car_pp)                                          */
 
 /* ---- scorer + loss (replaces tf.multiply + matching_dense_layer_1..4 :478-500, softmax
  *      :515, log :660, masked mean :664).                                                  */

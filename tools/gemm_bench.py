@@ -3,7 +3,8 @@
 
 Two groups of cases: operand-major / precision variants at 24000 x 1024 x 1024, and the training step's own GEMMs at
 the shapes bench.py's roofline times (R = 23 600 candidate rows, C = 1024): CAR layer 2 forward (bf16x3, bias + tanh),
-dgrad (single-pass TF32, leaky derivative from a separate aux) and split-K wgrad (single-pass TF32, both operands
+dgrad (single-pass TF32, leaky derivative from a separate aux, and with the CAR layer-1 gradients formed in its epilogue
+instead of a stored dH1) and split-K wgrad (single-pass TF32, both operands
 MN-major, split chosen by the library), and the scorer's first layer
 (C -> 128) forward / dgrad / wgrad, also with the scorer product (51 candidates per position) as separate kernels
 (mul_pred + forward, dgrad + mul_pred_bwd) against folded into the GEMMs (A scaled by PR, product backward epilogue).  Each step case also reports the share of the data-sheet peak of the tensor path it
@@ -106,12 +107,28 @@ def step_cases(dev):
         ops.mul_pred(Ec, PR, L, n_cand, C, PD)
         ops.gemm(PD, None, Z1, Rp, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0))
 
+    # CAR layer 1 per unique id at G1 (462 positions x 51 candidate rows, 1001 table slots): the layer-2 dgrad with its
+    # gradients of PP / PC / PI formed in the epilogue (dPI | dPC zeroed first, as the step does)
+    Lg, Kg = 462, 50
+    Rg, Ug = Lg * (Kg + 1), Kg * 20 + 1
+    PP, PC = torch.randn(Lg, C, device=dev), torch.randn(Lg, C, device=dev)
+    PI = torch.randn(Ug, C, device=dev)
+    pos_idx = torch.arange(Lg, dtype=torch.int32, device=dev)
+    neg_uidx = torch.multinomial(1.0 / torch.arange(1, Ug, device=dev, dtype=torch.float64).expand(Lg, Ug - 1), Kg).to(torch.int32)
+    DB = torch.empty(Lg + Ug + Lg, C, device=dev)                     # dPP | dPI | dPC, as in the step's DB
+    car = dict(pp=PP, pc=PC, pi=PI, pos_idx=pos_idx, neg_uidx=neg_uidx, dpp=DB[:Lg], dpi=DB[Lg:Lg + Ug], dpc=DB[Lg + Ug:], k=Kg)
+
+    def car_dgrad():
+        DB[Lg:].zero_()
+        ops.gemm(dE[:Rg], W2, None, Rg, C, C, precision=1, dact=ops.ACT_LEAKY, car=car)
+
     def dgrad_mul_pred_bwd():
         ops.gemm(dZ1, M0, dPD, Rp, C, 128, precision=1)
         ops.mul_pred_bwd(dPD, Ec, PR, L, n_cand, C, dEc, dPR, cand_act=ops.ACT_TANH)
     return [
         ('step L2 fwd   bf16x3 +bias tanh', lambda: ops.gemm(H1, None, E, R, C, C, ldb=0, bias=b2, act=ops.ACT_TANH, precision=4, b_bf16=W2plane, ld_bf16=W2plane.stride(0)), [R, C, C], E, 4),
         ('step L2 dgrad 1x +dact leaky aux sep', lambda: ops.gemm(dE, W2, dH1, R, C, C, precision=1, dact=ops.ACT_LEAKY, aux=H1), [R, C, C], dH1, 1),
+        ('step L2 dgrad 1x CAR layer-1 backward epilogue (G1 462 x 51 rows)', car_dgrad, [Rg, C, C], DB, 1),
         ('step L2 wgrad 1x split-K', lambda: ops.gemm(H1, dE, dW2, C, C, R, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), [C, C, R], dW2, 1),
         ('step M1 fwd   bf16x3 +bias leaky', lambda: ops.gemm(PD, None, Z1, R, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0)), [R, 128, C], Z1, 4),
         ('step M1 dgrad 1x', lambda: ops.gemm(dZ1, M0, dPD, R, C, 128, precision=1), [R, C, 128], dPD, 1),
