@@ -76,7 +76,7 @@ struct nar_engine {
   nar_ctx* ctx;
   nar_model_cfg cfg;
   PlaneSet planes;
-  cudaStream_t aux, aux2;
+  cudaStream_t aux;
   cudaEvent_t ev[N_EVENTS];
   int ev_i;
   float* WhT[NAR_MAX_LAYERS];
@@ -175,26 +175,12 @@ struct Seq {
 
   cudaEvent_t next_event() { cudaEvent_t v = e->ev[e->ev_i]; e->ev_i = (e->ev_i + 1) % N_EVENTS; return v; }
   // stream that deferred work (weight / bias gradients, forward session branch) runs on, after everything queued on main so far
-  cudaStream_t fork() { return fork(main); }
-  cudaStream_t fork(cudaStream_t from) {           // deferred work of a chain that itself runs on `from`
+  cudaStream_t fork() {
     if (!use_aux) return main;
     cudaEvent_t v = next_event();
-    if (cudaEventRecord(v, from) != cudaSuccess || cudaStreamWaitEvent(aux, v, 0) != cudaSuccess) rc = rc ? rc : (int)cudaGetLastError();
+    if (cudaEventRecord(v, main) != cudaSuccess || cudaStreamWaitEvent(aux, v, 0) != cudaSuccess) rc = rc ? rc : (int)cudaGetLastError();
     aux_dirty = true;
     return aux;
-  }
-  // second auxiliary stream: an independent CHAIN (the session backward) next to the main stream's
-  bool two_chains = false;
-  cudaStream_t fork2() {
-    if (!use_aux || !two_chains) return main;
-    cudaEvent_t v = next_event();
-    if (cudaEventRecord(v, main) != cudaSuccess || cudaStreamWaitEvent(e->aux2, v, 0) != cudaSuccess) rc = rc ? rc : (int)cudaGetLastError();
-    return e->aux2;
-  }
-  void join2() {
-    if (!use_aux || !two_chains) return;
-    cudaEvent_t v = next_event();
-    if (cudaEventRecord(v, e->aux2) != cudaSuccess || cudaStreamWaitEvent(main, v, 0) != cudaSuccess) rc = rc ? rc : (int)cudaGetLastError();
   }
   void join() {
     if (!use_aux || !aux_dirty) return;
@@ -219,8 +205,8 @@ struct Seq {
       const PlaneSet& ps = e->planes;
       int i = 0;
       for (; i < ps.n; ++i) if (ps.off_W[i] == off_W && ps.K[i] == Kd && ps.N[i] == N) break;
-      if (i == ps.n) { ep.precision = 3; ep.b_lo = c.params_lo + off_W; }      // no plane for this block: 3xTF32
-      else { ep.b_bf16 = ps.buf + ps.dst[i]; ep.ld_bf16 = ps.ld_out[i]; }
+      if (i == ps.n) { if (!rc) rc = NAR_ERR_INVALID; return; }   // planes_build registers every forward block: a miss is a bug
+      ep.b_bf16 = ps.buf + ps.dst[i]; ep.ld_bf16 = ps.ld_out[i];
     }
     chk(nar_gemm_tf32(e->ctx, M, N, Kd, X, ldx, 1, W(off_W), ldw, 0, Y, ldy, &ep, st));
   }
@@ -264,15 +250,19 @@ struct Seq {
   void bgrad(const float* dY, int64_t ld, int64_t rows, int64_t cols, int64_t off_b, cudaStream_t st) {
     chk(nar_colsum_add(dY, rows, cols, ld, G(off_b), st));
   }
+  // training-step dropout at site tensor_id (masks of oracle/dropout_ref.py, keyed by each row's position); dst may be src
+  void dropout(const float* src, float* dst, int64_t rows, int64_t cols, const int32_t* row_pos, int tensor_id, cudaStream_t st) {
+    chk(nar_dropout_rows(src, dst, rows, cols, cols, row_pos, io->L, c.K + 1, c.K, tensor_id, c.keep_prob, c.dropout_seed,
+                         (uint32_t)(io->global_step + 1), st));
+  }
 };
 
 // CAR (nar_model.py:374-405) of the L clicked rows sb.X[0:L] on the main stream, then the session branch - RNN (:408,
 // :1308-1342) + FC1 / FC2 (:410-438) -> sb.PR - forked onto the auxiliary stream, so that it runs under whatever the
 // caller queues next on main (the candidate rows); the caller joins before reading sb.PR.  (Moving the two CAR GEMMs
-// into the session branch as well was measured neutral and is not used: DESIGN.md section 6.)
-// dropout(src, dst, rows, cols, row_pos, tensor_id, stream) is only called when `drop` is set.
-template <class Dropout>
-void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop, Dropout&& dropout) {
+// into the session branch as well was measured neutral and is not used: DESIGN.md section 6.)  `drop`: training-step
+// dropout on the RNN outputs and FC1.
+void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
   const nar_model_cfg& c = s.c;
   const nar_step_io* io = s.io;
   const int64_t B = io->B, C = c.C, Hp = c.Hp, Fp = c.Fp;
@@ -292,11 +282,11 @@ void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop, Drop
       s.chk(nar_ugrnn_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.CD[i], st));
     }
     // DropoutWrapper(output_keep_prob) (nar_model.py:1330-1333): the cell's OUTPUT is dropped, its state is not
-    if (drop) dropout(sb.HO[i], sb.HOd[i], L, Hp, io->pos_idx, 8 + i, st);
+    if (drop) s.dropout(sb.HO[i], sb.HOd[i], L, Hp, io->pos_idx, 8 + i, st);
     rnn_in = drop ? sb.HOd[i] : sb.HO[i]; n_in = Hp;
   }
   s.fwd(rnn_in, Hp, c.off_W3, 512, c.off_b3, sb.F1, 512, L, 512, Hp, NAR_ACT_LEAKY_RELU, st);
-  if (drop) dropout(sb.F1, sb.F1, L, 512, io->pos_idx, 4, st);                                  // nar_model.py:417-419
+  if (drop) s.dropout(sb.F1, sb.F1, L, 512, io->pos_idx, 4, st);                                // nar_model.py:417-419
   s.fwd(sb.F1, 512, c.off_W4, C, c.off_b4, sb.PR, C, L, C, 512, NAR_ACT_TANH, st);
 }
 
@@ -315,18 +305,7 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   // dropout (training steps only): masks are per candidate row, so every row must be materialised
   const bool drop = train && c.keep_prob < 1.f;
   if (drop && c.dedup) return NAR_ERR_INVALID;
-  const uint32_t dstep = (uint32_t)(io->global_step + 1);
   Seq s(e, io, main);
-  // NAR_DEBUG_DROP_ONLY=<tensor id> (diagnostics, mirrored by the oracle): dropout at that site only
-  int drop_only = -1;
-  if (drop) { const char* v = getenv("NAR_DEBUG_DROP_ONLY"); if (v) drop_only = atoi(v); }
-  auto dropout = [&](const float* src, float* dst, int64_t rows, int64_t cols, const int32_t* rpos, int tid, cudaStream_t st) {
-    if (drop_only >= 0 && drop_only != tid) {
-      if (src != dst) cudaMemcpyAsync(dst, src, (size_t)rows * cols * sizeof(float), cudaMemcpyDeviceToDevice, st);
-      return;
-    }
-    s.chk(nar_dropout_rows(src, dst, rows, cols, cols, rpos, L, n_cand, K, tid, c.keep_prob, c.dropout_seed, dstep, st));
-  };
   const float inv_count = 1.0f / (float)(io->L_global > 0 ? io->L_global : 1);
   const int64_t U = pb.U, NB = 2 * L + U;
 
@@ -341,10 +320,10 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   const int32_t* g_pos = c.dedup ? pb.base_pos : pb.row_pos;
   const int64_t* g_item = c.dedup ? pb.base_item : pb.row_item;
   s.chk(nar_gather_features(e->ctx, &plan, g_pos, g_item, &rl, io->event_ts, io->max_ts, sb.X, main));
-  if (drop) dropout(sb.X, sb.X, R, Fp, pb.row_pos, 0, main);          // nar_model.py:338-340, :351-353, :367-369
+  if (drop) s.dropout(sb.X, sb.X, R, Fp, pb.row_pos, 0, main);        // nar_model.py:338-340, :351-353, :367-369
 
   float* H1c = sb.H1 + L * C; float* Ec = sb.E + L * C;
-  clicked_rows_forward(s, sb, L, drop, dropout);
+  clicked_rows_forward(s, sb, L, drop);
   if (c.dedup) {
     s.fwd(sb.X + L * Fp, Fp, c.off_W1, C, c.off_b1, sb.PP, C, L, C, Fp, NAR_ACT_NONE, main);                       // positives: full rows
     s.fwd(sb.X + 2 * L * Fp, Fp, c.off_W1, C, -1, sb.PI, C, U, C, c0, NAR_ACT_NONE, main);                          // item half, once per unique id
@@ -406,32 +385,35 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   } else {
     s.chk(nar_act_bwd(dEc, Ec, Rc * C, NAR_ACT_TANH, dEc, main));
   }
-  // ---- two independent chains from here on:
+  // ---- the two branches that share CAR layer 2's weights, one after the other on the main stream:
   //   S  session branch: FC2 / FC1 (nar_model.py:410-426) -> BPTT -> d(E) of the L clicked rows - a dozen small kernels
-  //   C  candidates: CAR layer-2 backward over the L*(1+K) candidate rows - the big GEMMs (+ the segment sums)
-  // S runs on a second auxiliary stream next to C; they meet before the clicked rows' CAR backward.
-  auto session_backward = [&](cudaStream_t ss) {
-    s.chk(nar_act_bwd(sb.dPR, sb.PR, L * C, NAR_ACT_TANH, sb.dPR, ss));
-    { cudaStream_t st = s.two_chains ? ss : s.fork(ss); s.wgrad(sb.F1, 512, sb.dPR, C, c.off_W4, C, 512, C, L, st); s.bgrad(sb.dPR, C, L, C, c.off_b4, st); }
-    s.dgrad(sb.dPR, C, c.off_W4, C, sb.dF1, 512, L, 512, C, NAR_ACT_LEAKY_RELU, sb.F1, 512, 0, ss);
-    if (drop) dropout(sb.dF1, sb.dF1, L, 512, io->pos_idx, 4, ss);     // F1 holds the dropped activations: re-apply the mask to the gradient
+  //   C  candidates: CAR layer-2 dgrad over the L*(1+K) candidate rows - the big GEMM (+ the CAR layer-1 sums)
+  // then the clicked rows' CAR backward, which needs S's dE.  The candidate rows' layer-2 weight gradient needs only dEc:
+  // queued on the auxiliary stream before S, the longest kernel of that stream starts as soon as dEc exists.
+  { cudaStream_t st = s.fork(); s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st); s.bgrad(dEc, C, Rc, C, c.off_b2, st); }
+  // ---- S
+  {
+    s.chk(nar_act_bwd(sb.dPR, sb.PR, L * C, NAR_ACT_TANH, sb.dPR, main));
+    { cudaStream_t st = s.fork(); s.wgrad(sb.F1, 512, sb.dPR, C, c.off_W4, C, 512, C, L, st); s.bgrad(sb.dPR, C, L, C, c.off_b4, st); }
+    s.dgrad(sb.dPR, C, c.off_W4, C, sb.dF1, 512, L, 512, C, NAR_ACT_LEAKY_RELU, sb.F1, 512, 0, main);
+    if (drop) s.dropout(sb.dF1, sb.dF1, L, 512, io->pos_idx, 4, main); // F1 holds the dropped activations: re-apply the mask to the gradient
     const float* rnn_out = drop ? sb.HOd[c.layers - 1] : sb.HO[c.layers - 1];
-    { cudaStream_t st = s.two_chains ? ss : s.fork(ss); s.wgrad(rnn_out, Hp, sb.dF1, 512, c.off_W3, 512, Hp, 512, L, st); s.bgrad(sb.dF1, 512, L, 512, c.off_b3, st); }
-    s.dgrad(sb.dF1, 512, c.off_W3, 512, sb.dHO, Hp, L, Hp, 512, NAR_ACT_NONE, nullptr, 0, 0, ss);
+    { cudaStream_t st = s.fork(); s.wgrad(rnn_out, Hp, sb.dF1, 512, c.off_W3, 512, Hp, 512, L, st); s.bgrad(sb.dF1, 512, L, 512, c.off_b3, st); }
+    s.dgrad(sb.dF1, 512, c.off_W3, 512, sb.dHO, Hp, L, Hp, 512, NAR_ACT_NONE, nullptr, 0, 0, main);
     float* dho = sb.dHO;
     for (int i = c.layers - 1; i >= 0; --i) {
-      if (drop) dropout(dho, dho, L, Hp, io->pos_idx, 8 + i, ss);       // gradient of the dropped cell output
+      if (drop) s.dropout(dho, dho, L, Hp, io->pos_idx, 8 + i, main);   // gradient of the dropped cell output
       const float* x_in = i == 0 ? sb.E : (drop ? sb.HOd[i - 1] : sb.HO[i - 1]);
       const int64_t n_in = i == 0 ? C : Hp;
       if (c.rnn_cell == 1) {
         const int64_t W3 = 3 * Hp;
-        s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, ss));
-        s.chk(nar_transpose_f32(s.W(c.off_Whc[i]), Hp, Hp, Hp, e->WhcT[i], Hp, ss));
+        s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, main));
+        s.chk(nar_transpose_f32(s.W(c.off_Whc[i]), Hp, Hp, Hp, e->WhcT[i], Hp, main));
         s.chk(nar_gru_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.UO[i], sb.CD[i], e->WhT[i], e->WhcT[i], io->sess_off, B, Hp, sb.dGX[i],
-                          sb.HPV[i], ss));
+                          sb.HPV[i], main));
         const float* dg = sb.dGX[i]; const float* dc = sb.dGX[i] + 2 * Hp;
         {
-          cudaStream_t st = s.two_chains ? ss : s.fork(ss);
+          cudaStream_t st = s.fork();
           s.wgrad(x_in, n_in, dg, W3, c.off_Wx[i], 2 * Hp, n_in, 2 * Hp, L, st);
           s.wgrad(x_in, n_in, dc, W3, c.off_Wxc[i], Hp, n_in, Hp, L, st);
           s.wgrad(sb.HPV[i], Hp, dg, W3, c.off_Wh[i], 2 * Hp, Hp, 2 * Hp, L, st);
@@ -442,35 +424,28 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
         // d(input) = d_gx[:, :2Hp] Wxg^T + d_gx[:, 2Hp:] Wxc^T (two GEMMs into one buffer), then through the CAR tanh for layer 0
         float* dxin = i == 0 ? sb.dE : sb.dHOb[i];
         const int64_t ldx = i == 0 ? C : Hp;
-        s.dgrad(dg, W3, c.off_Wx[i], 2 * Hp, dxin, ldx, L, n_in, 2 * Hp, NAR_ACT_NONE, nullptr, 0, 0, ss);
-        s.dgrad(dc, W3, c.off_Wxc[i], Hp, dxin, ldx, L, n_in, Hp, NAR_ACT_NONE, nullptr, 0, 1, ss);
-        if (i == 0) s.chk(nar_act_bwd(sb.dE, sb.E, L * C, NAR_ACT_TANH, sb.dE, ss));
+        s.dgrad(dg, W3, c.off_Wx[i], 2 * Hp, dxin, ldx, L, n_in, 2 * Hp, NAR_ACT_NONE, nullptr, 0, 0, main);
+        s.dgrad(dc, W3, c.off_Wxc[i], Hp, dxin, ldx, L, n_in, Hp, NAR_ACT_NONE, nullptr, 0, 1, main);
+        if (i == 0) s.chk(nar_act_bwd(sb.dE, sb.E, L * C, NAR_ACT_TANH, sb.dE, main));
         else dho = sb.dHOb[i];
         continue;
       }
-      s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, ss));
-      s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], ss));
+      s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, main));
+      s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
       {
-        cudaStream_t st = s.two_chains ? ss : s.fork(ss);
+        cudaStream_t st = s.fork();
         s.wgrad(x_in, n_in, sb.dGX[i], 2 * Hp, c.off_Wx[i], 2 * Hp, n_in, 2 * Hp, L, st);
         s.wgrad(sb.HPV[i], Hp, sb.dGX[i], 2 * Hp, c.off_Wh[i], 2 * Hp, Hp, 2 * Hp, L, st);
         s.bgrad(sb.dGX[i], 2 * Hp, L, 2 * Hp, c.off_rb[i], st);
       }
       if (i == 0) {
-        s.dgrad(sb.dGX[0], 2 * Hp, c.off_Wx[0], 2 * Hp, sb.dE, C, L, C, 2 * Hp, NAR_ACT_TANH, sb.E, C, 0, ss);   // clicked rows of dE (pre-tanh)
+        s.dgrad(sb.dGX[0], 2 * Hp, c.off_Wx[0], 2 * Hp, sb.dE, C, L, C, 2 * Hp, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
       } else {
-        s.dgrad(sb.dGX[i], 2 * Hp, c.off_Wx[i], 2 * Hp, sb.dHOb[i], Hp, L, Hp, 2 * Hp, NAR_ACT_NONE, nullptr, 0, 0, ss);
+        s.dgrad(sb.dGX[i], 2 * Hp, c.off_Wx[i], 2 * Hp, sb.dHOb[i], Hp, L, Hp, 2 * Hp, NAR_ACT_NONE, nullptr, 0, 0, main);
         dho = sb.dHOb[i];
       }
     }
-  };
-  // (NAR_BWD_CHAINS=1.  With two chains S keeps its own weight gradients on its stream: sharing the ONE auxiliary stream
-  // in enqueue order made the big layer-2 wgrad of C wait behind the last small wgrad of S: 1.22 -> 1.27 ms per G1 step.)
-  { const char* v = getenv("NAR_BWD_CHAINS"); s.two_chains = s.use_aux && v && atoi(v) != 0; }
-  // the candidate rows' layer-2 weight gradient needs only dEc: queued on the auxiliary stream before S, the longest
-  // kernel of that stream starts as soon as dEc exists
-  { cudaStream_t st = s.fork(); s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st); s.bgrad(dEc, C, Rc, C, c.off_b2, st); }
-  { cudaStream_t ss = s.fork2(); session_backward(ss); }
+  }
   // ---- C: CAR layer 2 of the candidate rows (shared weights: the clicked rows follow once S has produced their dE)
   float* DBin = sb.DB; float* DBpp = sb.DB + L * C; float* DBpi = sb.DB + 2 * L * C; float* DBpc = sb.DB + NB * C;
   if (c.dedup) {
@@ -479,7 +454,6 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   } else {
     s.dgrad(dEc, C, c.off_W2, C, sb.dH1 + L * C, C, Rc, C, C, NAR_ACT_LEAKY_RELU, H1c, C, 0, main);
   }
-  s.join2();                                       // dE[0:L] is final
   { cudaStream_t st = s.fork(); s.wgrad(sb.H1, C, sb.dE, C, c.off_W2, C, C, C, L, st); s.bgrad(sb.dE, C, L, C, c.off_b2, st); }
   if (c.dedup) {
     s.dgrad(sb.dE, C, c.off_W2, C, DBin, C, L, C, C, NAR_ACT_LEAKY_RELU, sb.H1, C, 0, main);
@@ -496,7 +470,7 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
     s.dgrad(sb.dE, C, c.off_W2, C, sb.dH1, C, L, C, C, NAR_ACT_LEAKY_RELU, sb.H1, C, 0, main);
     { cudaStream_t st = s.fork(); s.wgrad(sb.X, Fp, sb.dH1, C, c.off_W1, C, Fp, C, R, st); s.bgrad(sb.dH1, C, R, C, c.off_b1, st); }
     s.dgrad(sb.dH1, C, c.off_W1, C, sb.dX, Fp, R, Fp, C, NAR_ACT_NONE, nullptr, 0, 0, main);
-    if (drop) dropout(sb.dX, sb.dX, R, Fp, pb.row_pos, 0, main);
+    if (drop) s.dropout(sb.dX, sb.dX, R, Fp, pb.row_pos, 0, main);
   }
   s.chk(nar_gather_features_bwd(e->ctx, &plan, g_pos, g_item, &rl, io->event_ts, io->max_ts, sb.dX, s.G(c.off_gamma),
                                 s.G(c.off_beta), main));
@@ -603,7 +577,7 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
   if (s.rc) return s.rc;
 
   // ---- clicked rows + session branch (aux), the context half of layer 1 per position (main)
-  clicked_rows_forward(s, sb, L, false, [](const float*, float*, int64_t, int64_t, const int32_t*, int, cudaStream_t) {});
+  clicked_rows_forward(s, sb, L, false);
   s.fwd(sb.X + c0, Fp, c.off_W1 + c0 * C, C, c.off_b1, rb.PC, C, L, C, Fp - c0, NAR_ACT_NONE, main);
   s.join();
   if (gather_q) {
@@ -648,13 +622,15 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
 
 }  // namespace
 
-void planes_build(nar_engine* e) {
+// NAR_ERR_INVALID when the forward blocks do not fit MAX_PLANES
+int planes_build(nar_engine* e) {
   const nar_model_cfg& c = e->cfg;
   PlaneSet& ps = e->planes;
   ps.n = 0;
   int64_t total = 0;
+  bool overflow = false;
   auto add = [&](int64_t off, int64_t K, int64_t N, int64_t ldw) {
-    if (ps.n >= MAX_PLANES) return;
+    if (ps.n >= MAX_PLANES) { overflow = true; return; }
     const int i = ps.n++;
     ps.off_W[i] = off; ps.K[i] = (int32_t)K; ps.N[i] = (int32_t)N; ps.ldw[i] = (int32_t)ldw;
     ps.ld_out[i] = (int32_t)((K + 31) / 32 * 64);
@@ -670,12 +646,14 @@ void planes_build(nar_engine* e) {
     add(c.off_Wx[i], n_in, 2 * Hp, 2 * Hp);
     if (c.rnn_cell == 1) add(c.off_Wxc[i], n_in, Hp, Hp);
   }
+  if (overflow) return NAR_ERR_INVALID;
   if (!ps.buf) {
     cudaMalloc(&ps.buf, (size_t)total * sizeof(uint16_t));
     cudaMemset(ps.buf, 0, (size_t)total * sizeof(uint16_t));
     cudaMalloc(&ps.descs, MAX_PLANES * 32);
   }
   for (int i = 0; i < ps.n; ++i) { ps.W[i] = c.params + ps.off_W[i]; ps.out[i] = ps.buf + ps.dst[i]; }
+  return NAR_OK;
 }
 
 int planes_refresh(nar_engine* e, cudaStream_t st) {
@@ -699,15 +677,14 @@ extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_eng
   e->ctx = ctx; e->cfg = *cfg;
   { const char* v = getenv("NAR_FUSED_SCORER_PRODUCT"); e->fused_product = !(v && atoi(v) == 0); }
   NAR_CHECK_CUDA(cudaSetDevice(ctx->device));
-  if (cudaStreamCreateWithFlags(&e->aux, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&e->aux2, cudaStreamNonBlocking) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
+  if (cudaStreamCreateWithFlags(&e->aux, cudaStreamNonBlocking) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   for (int i = 0; i < N_EVENTS; ++i)
     if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   for (int i = 0; i < cfg->layers; ++i) {
     if (cudaMalloc(&e->WhT[i], (size_t)2 * cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
     if (cfg->rnn_cell == 1 && cudaMalloc(&e->WhcT[i], (size_t)cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   }
-  planes_build(e);
+  if (planes_build(e) != NAR_OK) { delete e; return NAR_ERR_INVALID; }
   if (!e->planes.buf || !e->planes.descs) { delete e; return NAR_ERR_NO_DEVICE; }
   *out = e;
   return NAR_OK;
@@ -721,7 +698,6 @@ extern "C" int nar_engine_refresh(nar_engine* e, void* stream) {
 extern "C" int nar_engine_destroy(nar_engine* e) {
   if (!e) return NAR_OK;
   cudaStreamSynchronize(e->aux);
-  if (e->aux2) { cudaStreamSynchronize(e->aux2); cudaStreamDestroy(e->aux2); }
   for (int i = 0; i < NAR_MAX_LAYERS; ++i) { if (e->WhT[i]) cudaFree(e->WhT[i]); if (e->WhcT[i]) cudaFree(e->WhcT[i]); }
   for (int i = 0; i < N_EVENTS; ++i) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
   if (e->aux) cudaStreamDestroy(e->aux);
@@ -736,8 +712,7 @@ extern "C" int nar_engine_update_cfg(nar_engine* e, const nar_model_cfg* cfg) {
   if (cfg->layers != e->cfg.layers || cfg->Hp != e->cfg.Hp || cfg->C != e->cfg.C || cfg->Fp != e->cfg.Fp ||
       cfg->rnn_cell != e->cfg.rnn_cell) return NAR_ERR_INVALID;        // structural changes need a new engine
   e->cfg = *cfg;
-  planes_build(e);                      // the parameter buffer may have changed (share_params)
-  return NAR_OK;
+  return planes_build(e);               // the parameter buffer may have changed (share_params)
 }
 
 extern "C" int nar_engine_workspace_bytes(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_t L_cap, int32_t train,

@@ -205,10 +205,6 @@ class NarOracle:
         if self.mask_override is not None:
             m = self.mask_override[tensor_id if t is None else (tensor_id, t)]
             return x * torch.as_tensor(np.asarray(m)).to(self.dtype) / self.keep_prob
-        import os
-        only = os.environ.get('NAR_DEBUG_DROP_ONLY')            # diagnostics: dropout at one site only (feature rows = 0)
-        if only is not None and int(only) != (0 if tensor_id in (1, 2, 3) else tensor_id):
-            return x
         from . import dropout_ref
         n_cols = x.shape[-1]
         if feature_rows:

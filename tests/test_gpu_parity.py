@@ -4,7 +4,7 @@ against the oracle / fp64 references on the same seeded inputs.
 Tolerances (north_star): sampled negatives bit-exact; loss and logits within 1e-3 relative.  Gradients are compared at
 IDENTICAL leaky_relu slope choices (tools/gpu_step_check.py hands the engine's activation signs to the oracle): a 1e-5
 forward difference that flips one pre-activation across the kink moves the oracle's own bias gradients by up to 10 %
-(tools/debug_drop.py, DESIGN.md section 3), which says nothing about either implementation.  Additional bars we
+(DESIGN.md section 3), which says nothing about either implementation.  Additional bars we
 hold ourselves to: feature rows 1e-5, 3xTF32 GEMM 2e-5, TF32 GEMM 3e-3, gradients 3e-2 of the tensor max
 (backward GEMMs run single-pass TF32), Adam update within 0.2*lr where the gradient is far above eps.
 """
