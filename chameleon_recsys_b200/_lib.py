@@ -131,6 +131,8 @@ _SIGNATURES = {
     'nar_ugrnn_bwd': (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]),
     'nar_gru_fwd': (C.c_int, [vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, vp, vp, vp]),
     'nar_gru_bwd': (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]),
+    'nar_lstm_fwd': (C.c_int, [vp, vp, vp, vp, i64, i64, vp, vp, vp]),
+    'nar_lstm_bwd': (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]),
     'nar_sample_negatives_workspace': (C.c_int, [i64, i64, i64, i64, C.POINTER(i64)]),
     'nar_sample_negatives': (C.c_int, [vp, vp, i64, i64, i64, i64, vp, i64, i64, i64, u64, u32, vp, vp, i64, vp]),
     'nar_mul_pred': (C.c_int, [vp, vp, i64, i64, i64, vp, vp]),

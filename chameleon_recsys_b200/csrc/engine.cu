@@ -97,6 +97,9 @@ bool fused_product(const nar_engine* e) {
   return e->fused_product && c.ranking == 0 && c.K + 1 <= 128 && c.fwd_precision == 4 && c.bwd_precision == 1;
 }
 
+// gate blocks per unit: UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o)
+int64_t gate_blocks(const nar_model_cfg& c) { return c.rnn_cell == 2 ? 4 : c.rnn_cell == 1 ? 3 : 2; }
+
 int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_t L_cap, void* base, PrepBufs* pb) {
   const nar_model_cfg& c = e->cfg;
   const int64_t K = c.K, n_cand = K + 1, Rcap = L_cap * (n_cand + 1);
@@ -126,7 +129,7 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
   if (c.dedup) { sb->X = cv.take<float>(NB * Fp); } else { sb->X = cv.take<float>(R * Fp); }
   sb->H1 = cv.take<float>(R * C);
   sb->E = cv.take<float>(R * C);
-  const int64_t gw = c.rnn_cell == 1 ? 3 : 2;           // gate blocks per unit: UGRNN (gate | candidate), GRU (r | u | candidate)
+  const int64_t gw = gate_blocks(c);
   for (int i = 0; i < c.layers; ++i) {
     sb->GX[i] = cv.take<float>(L_cap * gw * Hp); sb->HO[i] = cv.take<float>(L_cap * Hp);
     sb->GT[i] = cv.take<float>(L_cap * Hp); sb->CD[i] = cv.take<float>(L_cap * Hp);
@@ -277,6 +280,11 @@ void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
       s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wxc[i], Hp, c.off_bc[i], sb.GX[i] + 2 * Hp, 3 * Hp, L, Hp, n_in, NAR_ACT_NONE, st);
       s.chk(nar_gru_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), s.W(c.off_Whc[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.UO[i],
                         sb.CD[i], sb.RH[i], st));
+    } else if (c.rnn_cell == 2) {
+      // LSTMCell: gx = x Wx + b (i | j | f | o), then the recurrence (csrc/lstm.cu), which leaves the activated gates in gx
+      // and the cell state in CD
+      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 4 * Hp, c.off_rb[i], sb.GX[i], 4 * Hp, L, 4 * Hp, n_in, NAR_ACT_NONE, st);
+      s.chk(nar_lstm_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.CD[i], st));
     } else {
       s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 2 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
       s.chk(nar_ugrnn_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.CD[i], st));
@@ -430,6 +438,24 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
         else dho = sb.dHOb[i];
         continue;
       }
+      if (c.rnn_cell == 2) {
+        const int64_t W4 = 4 * Hp;
+        s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, W4, W4, e->WhT[i], Hp, main));
+        s.chk(nar_lstm_bwd(e->ctx, dho, sb.HO[i], sb.CD[i], sb.GX[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
+        {
+          cudaStream_t st = s.fork();
+          s.wgrad(x_in, n_in, sb.dGX[i], W4, c.off_Wx[i], W4, n_in, W4, L, st);
+          s.wgrad(sb.HPV[i], Hp, sb.dGX[i], W4, c.off_Wh[i], W4, Hp, W4, L, st);
+          s.bgrad(sb.dGX[i], W4, L, W4, c.off_rb[i], st);
+        }
+        if (i == 0) {
+          s.dgrad(sb.dGX[0], W4, c.off_Wx[0], W4, sb.dE, C, L, C, W4, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
+        } else {
+          s.dgrad(sb.dGX[i], W4, c.off_Wx[i], W4, sb.dHOb[i], Hp, L, Hp, W4, NAR_ACT_NONE, nullptr, 0, 0, main);
+          dho = sb.dHOb[i];
+        }
+        continue;
+      }
       s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, main));
       s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
       {
@@ -490,7 +516,7 @@ struct RecBufs {
 int64_t rec_carve(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int64_t qb, int64_t nb, int gather_q, void* base,
                   RecBufs* rb) {
   const nar_model_cfg& c = e->cfg;
-  const int64_t C = c.C, Hp = c.Hp, Fp = c.Fp, gw = c.rnn_cell == 1 ? 3 : 2, P = qb * nb;
+  const int64_t C = c.C, Hp = c.Hp, Fp = c.Fp, gw = gate_blocks(c), P = qb * nb;
   memset(rb, 0, sizeof(*rb));
   StepBufs& sb = rb->sb;
   Carver cv(base);
@@ -643,7 +669,8 @@ int planes_build(nar_engine* e) {
   add(c.off_M[0], C, 128, c.ld_M[0]); add(c.off_M[1], 128, 64, c.ld_M[1]); add(c.off_M[2], 64, 32, c.ld_M[2]);
   for (int i = 0; i < c.layers; ++i) {
     const int64_t n_in = i == 0 ? C : Hp;
-    add(c.off_Wx[i], n_in, 2 * Hp, 2 * Hp);
+    const int64_t wx = c.rnn_cell == 2 ? 4 * Hp : 2 * Hp;
+    add(c.off_Wx[i], n_in, wx, wx);
     if (c.rnn_cell == 1) add(c.off_Wxc[i], n_in, Hp, Hp);
   }
   if (overflow) return NAR_ERR_INVALID;
@@ -667,7 +694,7 @@ int planes_refresh(nar_engine* e, cudaStream_t st) {
 extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_engine** out) {
   if (!ctx || !cfg || !out) return NAR_ERR_INVALID;
   *out = nullptr;
-  if (cfg->layers < 1 || cfg->layers > NAR_MAX_LAYERS || cfg->rnn_cell < 0 || cfg->rnn_cell > 1 || cfg->ranking < 0 || cfg->ranking > 1)
+  if (cfg->layers < 1 || cfg->layers > NAR_MAX_LAYERS || cfg->rnn_cell < 0 || cfg->rnn_cell > 2 || cfg->ranking < 0 || cfg->ranking > 1)
     return NAR_ERR_UNSUPPORTED;
   if ((cfg->C & 3) || (cfg->Hp & 3) || (cfg->Fp & 3) || (cfg->ctx_col0 & 3) || cfg->ctx_col0 <= 0 || cfg->ctx_col0 >= cfg->Fp)
     return NAR_ERR_INVALID;
@@ -681,7 +708,8 @@ extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_eng
   for (int i = 0; i < N_EVENTS; ++i)
     if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   for (int i = 0; i < cfg->layers; ++i) {
-    if (cudaMalloc(&e->WhT[i], (size_t)2 * cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
+    const size_t wht = (size_t)(cfg->rnn_cell == 2 ? 4 : 2) * cfg->Hp * cfg->Hp;     // transposed recurrent block [2Hp | 4Hp, Hp]
+    if (cudaMalloc(&e->WhT[i], wht * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
     if (cfg->rnn_cell == 1 && cudaMalloc(&e->WhcT[i], (size_t)cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   }
   if (planes_build(e) != NAR_OK) { delete e; return NAR_ERR_INVALID; }

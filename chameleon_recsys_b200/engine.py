@@ -41,8 +41,9 @@ class NarEngine:
                  dropout_seed: Optional[int] = None):
         if not torch.cuda.is_available():
             raise NarError('NarEngine needs a CUDA (sm_90a) device; there is no CPU fallback')
-        if rnn_cell not in ('ugrnn', 'gru'):
-            raise ValueError("rnn_cell=%r: 'ugrnn' (the reference's UGRNNCell, nar_model.py:1318) or 'gru' (GRUCell, :1315)" % rnn_cell)
+        if rnn_cell not in ('ugrnn', 'gru', 'lstm'):
+            raise ValueError("rnn_cell=%r: 'ugrnn' (the reference's UGRNNCell, nar_model.py:1318), 'gru' (GRUCell, :1315) or "
+                             "'lstm' (LSTMCell, :1316)" % rnn_cell)
         if rnn_cell != getattr(layout, 'rnn_cell', 'ugrnn'):
             raise ValueError('ParamLayout was built for rnn_cell=%r' % getattr(layout, 'rnn_cell', 'ugrnn'))
         self.rnn_cell = rnn_cell
@@ -151,7 +152,7 @@ class NarEngine:
         lay, pl = self.layout, self.plan
         c = ModelCfg()
         c.num_items, c.C, c.Hp, c.Fp, c.ctx_col0 = self.V, self.C, self.Hp, pl.Fp, pl.ctx_col0
-        c.layers, c.rnn_cell, c.ranking = self.layers, 1 if self.rnn_cell == 'gru' else 0, 0 if self.ranking == 'mlp' else 1
+        c.layers, c.rnn_cell, c.ranking = self.layers, {'ugrnn': 0, 'gru': 1, 'lstm': 2}[self.rnn_cell], 0 if self.ranking == 'mlp' else 1
         c.fwd_precision, c.bwd_precision = self.fwd_prec, self.bwd_prec
         c.dedup, c.use_aux_stream = int(self.dedup), int(self.use_aux_stream)
         c.keep_prob, c.novelty_reg_factor = self.keep_prob, self.nov_factor

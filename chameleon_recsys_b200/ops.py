@@ -180,6 +180,22 @@ def ugrnn_bwd(d_hout, h_out, gate, cand, WhT, sess_off, B, Hp, d_gx, h_prev):
                                 _p(d_gx), _p(h_prev), _stream()), 'nar_ugrnn_bwd')
 
 
+def lstm_fwd(gx, Wh, sess_off, B, Hp, h_out, c_out):
+    """gx [L,4Hp] (pre-activations i | j | f | o of the input) is overwritten with the activated gates."""
+    global LAUNCHES
+    LAUNCHES += 1
+    ctx = context()
+    check(ctx.lib.nar_lstm_fwd(ctx.handle, _p(gx), _p(Wh), _p(sess_off), B, Hp, _p(h_out), _p(c_out), _stream()), 'nar_lstm_fwd')
+
+
+def lstm_bwd(d_hout, h_out, c_out, act, WhT, sess_off, B, Hp, d_gx, h_prev):
+    global LAUNCHES
+    LAUNCHES += 1
+    ctx = context()
+    check(ctx.lib.nar_lstm_bwd(ctx.handle, _p(d_hout), _p(h_out), _p(c_out), _p(act), _p(WhT), _p(sess_off), B, Hp, _p(d_gx),
+                               _p(h_prev), _stream()), 'nar_lstm_bwd')
+
+
 def sample_negatives_workspace(Bg, T1, buf_len, K) -> int:
     lib = _lib.load()
     n = C.c_int64(0)

@@ -271,7 +271,23 @@ class ParamLayout:
                                      col_map=np.arange(H), part_of=ck, part_rows=(n_in, n_in + H), row_map=np.arange(H)))
             noreg.append(ParamTensor('rnn%d/bc' % i, base + 'candidate/bias', (H,), INIT_ZEROS, False, rows=1, ld=Hp,
                                      col_map=np.arange(H)))
-        for i in range(self.layers if rnn_cell != 'gru' else 0):
+        lstm_cols = np.concatenate([k * Hp + np.arange(H) for k in range(4)])
+        for i in range(self.layers if rnn_cell == 'lstm' else 0):
+            # tf.nn.rnn_cell.LSTMCell(H, state_is_tuple=True) (nar_model.py:1316, commented alternative): lstm_cell/kernel
+            # [in+H, 4H] (i | j | f | o), lstm_cell/bias [4H] (zeros; forget_bias 1.0 is a constant inside the cell); the four
+            # column blocks go to Hp-wide blocks, the rows split into input and recurrent parts
+            n_in = C if i == 0 else H
+            n_in_p = C if i == 0 else Hp
+            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/lstm_cell/'.format(i)
+            noreg.append(ParamTensor('rnn%d/Wx' % i, base + 'kernel', (n_in + H, 4 * H), INIT_XAVIER, False,
+                                     rows=n_in_p, ld=4 * Hp, col_map=lstm_cols, part_of=base + 'kernel',
+                                     part_rows=(0, n_in), row_map=np.arange(n_in)))
+            noreg.append(ParamTensor('rnn%d/Wh' % i, base + 'kernel', (n_in + H, 4 * H), INIT_XAVIER, False,
+                                     rows=Hp, ld=4 * Hp, col_map=lstm_cols, part_of=base + 'kernel',
+                                     part_rows=(n_in, n_in + H), row_map=np.arange(H)))
+            noreg.append(ParamTensor('rnn%d/b' % i, base + 'bias', (4 * H,), INIT_ZEROS, False,
+                                     rows=1, ld=4 * Hp, col_map=lstm_cols))
+        for i in range(self.layers if rnn_cell not in ('gru', 'lstm') else 0):
             n_in = C if i == 0 else H
             n_in_p = C if i == 0 else Hp
             base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/ugrnn_cell/'.format(i)

@@ -239,6 +239,18 @@ int nar_gru_bwd(nar_ctx* ctx, const float* d_hout, const float* h_out, const flo
                 const float* c_out, const float* WhgT, const float* WhcT, const int32_t* sess_off, int64_t B, int64_t Hp,
                 float* d_gx, float* h_prev, void* stream);
 
+/* LSTM recurrence (tf.nn.rnn_cell.LSTMCell(H, state_is_tuple=True), nar_model.py:1316; rnn_cell='lstm'; no peepholes, no
+ * cell clip, no projection, forget_bias 1.0): gx [L,4Hp] = x*Wx + b (i | j | f | o pre-activations of the input),
+ * Wh [Hp,4Hp]:  c' = sigmoid(f + h*Wh_f + 1) * c + sigmoid(i + h*Wh_i) * tanh(j + h*Wh_j) ; h' = sigmoid(o + h*Wh_o) * tanh(c').
+ * gx is overwritten in place with the activated gates (sigmoid(i) | tanh(j) | sigmoid(f+1) | sigmoid(o)); per row: output
+ * h_out = h', cell state c_out = c'.                                                                                       */
+int nar_lstm_fwd(nar_ctx* ctx, float* gx, const float* Wh, const int32_t* sess_off, int64_t B, int64_t Hp, float* h_out,
+                 float* c_out, void* stream);
+/* act [L,4Hp] = the activated gates nar_lstm_fwd left in gx; d_gx [L,4Hp] = dL/d(pre-activations); h_prev [L,Hp] = h entering
+ * the step (dWh = h_prev^T d_gx); WhT [4Hp,Hp] is the transposed recurrent block.                                          */
+int nar_lstm_bwd(nar_ctx* ctx, const float* d_hout, const float* h_out, const float* c_out, const float* act, const float* WhT,
+                 const int32_t* sess_off, int64_t B, int64_t Hp, float* d_gx, float* h_prev, void* stream);
+
 /* ---- negative sampler (replaces nar_model.py:1220-1304: tf.random_shuffle x(2+clicks),
  *      tf.unique, unsorted_segment_min, tf.setdiff1d inside nested tf.map_fn).  RNG spec:
  *      oracle/sampler_ref.py.  all_items_global [Bg,T1] builds the pool; negatives are
@@ -394,7 +406,7 @@ int nar_tf32_lo(const float* x, int64_t n, float* lo, void* stream);
 typedef struct {
   /* dimensions */
   int64_t num_items, C /*CAR_embedding_size*/, Hp /*rnn_units padded to 4*/, Fp /*feature row width*/, ctx_col0;
-  int32_t layers, rnn_cell /*0 = UGRNNCell (nar_model.py:1318), 1 = GRUCell (:1315)*/, ranking /*0 = MLP scorer (:444-500), 1 = cosine*/;
+  int32_t layers, rnn_cell /*0 = UGRNNCell (nar_model.py:1318), 1 = GRUCell (:1315), 2 = LSTMCell (:1316)*/, ranking /*0 = MLP scorer (:444-500), 1 = cosine*/;
   int32_t fwd_precision, bwd_precision;       /* nar_gemm_epilogue.precision of the forward (3 or 4) / backward (1 or 3) GEMMs */
   int32_t dedup;                              /* 1: per-unique-id CAR layer 1 (csrc/car.cu); 0: every candidate row materialised */
   int32_t use_aux_stream;                     /* 1: weight / bias gradients (and the forward session branch) on the auxiliary stream */
@@ -411,7 +423,7 @@ typedef struct {
   int64_t n_params, reg_end;
   int64_t off_W1, off_b1, off_W2, off_b2, off_W3, off_b3, off_W4, off_b4, off_gamma, off_beta;
   int64_t off_M[4], off_c[4], ld_M[4];        /* matching_dense_layer_1..4 kernels / biases, leading dimensions */
-  int64_t off_Wx[NAR_MAX_LAYERS], off_Wh[NAR_MAX_LAYERS], off_rb[NAR_MAX_LAYERS];     /* UGRNN: [in|H, 2Hp] (gate | candidate); GRU: gates (r | u) */
+  int64_t off_Wx[NAR_MAX_LAYERS], off_Wh[NAR_MAX_LAYERS], off_rb[NAR_MAX_LAYERS];     /* UGRNN: [in|H, 2Hp] (gate | candidate); GRU: gates (r | u); LSTM: [in|H, 4Hp] (i | j | f | o) */
   int64_t off_Wxc[NAR_MAX_LAYERS], off_Whc[NAR_MAX_LAYERS], off_bc[NAR_MAX_LAYERS];  /* GRU only: candidate blocks [in|H, Hp] */
   /* feature plan: static part (segments, tables, metadata, created_at_ts, gamma / beta, column map) */
   nar_feature_plan plan;

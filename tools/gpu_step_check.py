@@ -17,12 +17,13 @@ from chameleon_recsys_b200.clicked_items_state import batch_clicks_for_state_upd
 from chameleon_recsys_b200.engine import NarEngine  # noqa: E402
 from chameleon_recsys_b200.harness import make_problem, warm_state  # noqa: E402
 from oracle import sampler_ref  # noqa: E402
+from oracle.lstm_ref import LstmOracle  # noqa: E402
 from oracle.nar_oracle import NarOracle  # noqa: E402
 
 
 def make_oracle(pb, dtype=torch.float64):
     hp = pb.hp
-    return NarOracle(pb.session_features_config, pb.articles_features_config, pb.internal_features_config,
+    return (LstmOracle if hp.rnn_cell == 'lstm' else NarOracle)(pb.session_features_config, pb.articles_features_config, pb.internal_features_config,
                      pb.content_article_embeddings_matrix, pb.articles_metadata,
                      negative_samples=hp.train_total_negative_samples, softmax_temperature=hp.softmax_temperature,
                      reg_weight_decay=hp.reg_l2, recent_clicks_for_normalization=hp.recent_clicks_for_normalization,
