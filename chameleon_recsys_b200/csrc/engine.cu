@@ -55,7 +55,9 @@ struct StepBufs {
   float *X, *dX, *H1, *E, *dE, *dH1, *F1, *PR, *logits, *PD, *dPD, *Z1, *Z2, *Z3, *dZ1, *dZ2, *dZ3, *dPR, *dF1, *dHO;
   float *GX[NAR_MAX_LAYERS], *HO[NAR_MAX_LAYERS], *GT[NAR_MAX_LAYERS], *CD[NAR_MAX_LAYERS], *dGX[NAR_MAX_LAYERS],
         *HPV[NAR_MAX_LAYERS], *dHOb[NAR_MAX_LAYERS], *HOd[NAR_MAX_LAYERS],   // HOd: RNN outputs after DropoutWrapper
-        *UO[NAR_MAX_LAYERS], *RH[NAR_MAX_LAYERS];                          // GRU: update gate, r * previous state
+        *UO[NAR_MAX_LAYERS], *RH[NAR_MAX_LAYERS];
+  // per cell: GT = UGRNN gate / GRU r (LSTM: none); CD = UGRNN and GRU candidate / LSTM cell state; UO = GRU u;
+  // RH = GRU r * previous state.  The LSTM's activated gates replace its pre-activations in GX.
   float *PP, *PI, *PC, *DB;        // dedup: layer-1 pre-activations and their gradients
 };
 
@@ -97,8 +99,10 @@ bool fused_product(const nar_engine* e) {
   return e->fused_product && c.ranking == 0 && c.K + 1 <= 128 && c.fwd_precision == 4 && c.bwd_precision == 1;
 }
 
-// gate blocks per unit: UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o)
-int64_t gate_blocks(const nar_model_cfg& c) { return c.rnn_cell == 2 ? 4 : c.rnn_cell == 1 ? 3 : 2; }
+// gate blocks per unit (GX width): UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o)
+int64_t gate_blocks(const nar_model_cfg& c) { return c.rnn_cell == NAR_CELL_LSTM ? 4 : c.rnn_cell == NAR_CELL_GRU ? 3 : 2; }
+// blocks per unit of the Wx / Wh parameter blocks (and WhT): the GRU's candidate lives in Wxc / Whc
+int64_t wh_blocks(const nar_model_cfg& c) { return c.rnn_cell == NAR_CELL_LSTM ? 4 : 2; }
 
 int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_t L_cap, void* base, PrepBufs* pb) {
   const nar_model_cfg& c = e->cfg;
@@ -132,8 +136,9 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
   const int64_t gw = gate_blocks(c);
   for (int i = 0; i < c.layers; ++i) {
     sb->GX[i] = cv.take<float>(L_cap * gw * Hp); sb->HO[i] = cv.take<float>(L_cap * Hp);
-    sb->GT[i] = cv.take<float>(L_cap * Hp); sb->CD[i] = cv.take<float>(L_cap * Hp);
-    if (c.rnn_cell == 1) { sb->UO[i] = cv.take<float>(L_cap * Hp); sb->RH[i] = cv.take<float>(L_cap * Hp); }
+    if (c.rnn_cell != NAR_CELL_LSTM) sb->GT[i] = cv.take<float>(L_cap * Hp);
+    sb->CD[i] = cv.take<float>(L_cap * Hp);
+    if (c.rnn_cell == NAR_CELL_GRU) { sb->UO[i] = cv.take<float>(L_cap * Hp); sb->RH[i] = cv.take<float>(L_cap * Hp); }
   }
   sb->F1 = cv.take<float>(L_cap * 512);
   sb->PR = cv.take<float>(L_cap * C);
@@ -273,20 +278,19 @@ void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
   s.fwd(sb.H1, C, c.off_W2, C, c.off_b2, sb.E, C, L, C, C, NAR_ACT_TANH, s.main);
   cudaStream_t st = s.fork();
   const float* rnn_in = sb.E; int64_t n_in = C;
+  const int64_t wx = wh_blocks(c) * Hp, gw = gate_blocks(c) * Hp;
   for (int i = 0; i < c.layers; ++i) {
-    if (c.rnn_cell == 1) {
-      // GRUCell: gx = (x Wxg + bg | x Wxc + bc), then the recurrence (csrc/gru.cu)
-      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 3 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
+    // input projection gx = x Wx + b, then the recurrence (csrc/rnn.cu)
+    s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], wx, c.off_rb[i], sb.GX[i], gw, L, wx, n_in, NAR_ACT_NONE, st);
+    if (c.rnn_cell == NAR_CELL_GRU) {
+      // GRUCell: gx = (x Wxg + bg | x Wxc + bc), the candidate's projection from its own block
       s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wxc[i], Hp, c.off_bc[i], sb.GX[i] + 2 * Hp, 3 * Hp, L, Hp, n_in, NAR_ACT_NONE, st);
       s.chk(nar_gru_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), s.W(c.off_Whc[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.UO[i],
                         sb.CD[i], sb.RH[i], st));
-    } else if (c.rnn_cell == 2) {
-      // LSTMCell: gx = x Wx + b (i | j | f | o), then the recurrence (csrc/lstm.cu), which leaves the activated gates in gx
-      // and the cell state in CD
-      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 4 * Hp, c.off_rb[i], sb.GX[i], 4 * Hp, L, 4 * Hp, n_in, NAR_ACT_NONE, st);
+    } else if (c.rnn_cell == NAR_CELL_LSTM) {
+      // LSTMCell (i | j | f | o): the recurrence leaves the activated gates in gx and the cell state in CD
       s.chk(nar_lstm_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.CD[i], st));
     } else {
-      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], 2 * Hp, c.off_rb[i], sb.GX[i], 2 * Hp, L, 2 * Hp, n_in, NAR_ACT_NONE, st);
       s.chk(nar_ugrnn_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.CD[i], st));
     }
     // DropoutWrapper(output_keep_prob) (nar_model.py:1330-1333): the cell's OUTPUT is dropped, its state is not
@@ -413,7 +417,7 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
       if (drop) s.dropout(dho, dho, L, Hp, io->pos_idx, 8 + i, main);   // gradient of the dropped cell output
       const float* x_in = i == 0 ? sb.E : (drop ? sb.HOd[i - 1] : sb.HO[i - 1]);
       const int64_t n_in = i == 0 ? C : Hp;
-      if (c.rnn_cell == 1) {
+      if (c.rnn_cell == NAR_CELL_GRU) {
         const int64_t W3 = 3 * Hp;
         s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, main));
         s.chk(nar_transpose_f32(s.W(c.off_Whc[i]), Hp, Hp, Hp, e->WhcT[i], Hp, main));
@@ -438,36 +442,23 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
         else dho = sb.dHOb[i];
         continue;
       }
-      if (c.rnn_cell == 2) {
-        const int64_t W4 = 4 * Hp;
-        s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, W4, W4, e->WhT[i], Hp, main));
+      // UGRNN and LSTM: gx, Wx, Wh and the bias are all wh_blocks(c) * Hp wide
+      const int64_t wx = wh_blocks(c) * Hp;
+      s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, wx, wx, e->WhT[i], Hp, main));
+      if (c.rnn_cell == NAR_CELL_LSTM)
         s.chk(nar_lstm_bwd(e->ctx, dho, sb.HO[i], sb.CD[i], sb.GX[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
-        {
-          cudaStream_t st = s.fork();
-          s.wgrad(x_in, n_in, sb.dGX[i], W4, c.off_Wx[i], W4, n_in, W4, L, st);
-          s.wgrad(sb.HPV[i], Hp, sb.dGX[i], W4, c.off_Wh[i], W4, Hp, W4, L, st);
-          s.bgrad(sb.dGX[i], W4, L, W4, c.off_rb[i], st);
-        }
-        if (i == 0) {
-          s.dgrad(sb.dGX[0], W4, c.off_Wx[0], W4, sb.dE, C, L, C, W4, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
-        } else {
-          s.dgrad(sb.dGX[i], W4, c.off_Wx[i], W4, sb.dHOb[i], Hp, L, Hp, W4, NAR_ACT_NONE, nullptr, 0, 0, main);
-          dho = sb.dHOb[i];
-        }
-        continue;
-      }
-      s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, main));
-      s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
+      else
+        s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
       {
         cudaStream_t st = s.fork();
-        s.wgrad(x_in, n_in, sb.dGX[i], 2 * Hp, c.off_Wx[i], 2 * Hp, n_in, 2 * Hp, L, st);
-        s.wgrad(sb.HPV[i], Hp, sb.dGX[i], 2 * Hp, c.off_Wh[i], 2 * Hp, Hp, 2 * Hp, L, st);
-        s.bgrad(sb.dGX[i], 2 * Hp, L, 2 * Hp, c.off_rb[i], st);
+        s.wgrad(x_in, n_in, sb.dGX[i], wx, c.off_Wx[i], wx, n_in, wx, L, st);
+        s.wgrad(sb.HPV[i], Hp, sb.dGX[i], wx, c.off_Wh[i], wx, Hp, wx, L, st);
+        s.bgrad(sb.dGX[i], wx, L, wx, c.off_rb[i], st);
       }
       if (i == 0) {
-        s.dgrad(sb.dGX[0], 2 * Hp, c.off_Wx[0], 2 * Hp, sb.dE, C, L, C, 2 * Hp, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
+        s.dgrad(sb.dGX[0], wx, c.off_Wx[0], wx, sb.dE, C, L, C, wx, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
       } else {
-        s.dgrad(sb.dGX[i], 2 * Hp, c.off_Wx[i], 2 * Hp, sb.dHOb[i], Hp, L, Hp, 2 * Hp, NAR_ACT_NONE, nullptr, 0, 0, main);
+        s.dgrad(sb.dGX[i], wx, c.off_Wx[i], wx, sb.dHOb[i], Hp, L, Hp, wx, NAR_ACT_NONE, nullptr, 0, 0, main);
         dho = sb.dHOb[i];
       }
     }
@@ -529,8 +520,9 @@ int64_t rec_carve(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int64_t 
   sb.E = cv.take<float>(L * C);
   for (int i = 0; i < c.layers; ++i) {
     sb.GX[i] = cv.take<float>(L * gw * Hp); sb.HO[i] = cv.take<float>(L * Hp);
-    sb.GT[i] = cv.take<float>(L * Hp); sb.CD[i] = cv.take<float>(L * Hp);
-    if (c.rnn_cell == 1) { sb.UO[i] = cv.take<float>(L * Hp); sb.RH[i] = cv.take<float>(L * Hp); }
+    if (c.rnn_cell != NAR_CELL_LSTM) sb.GT[i] = cv.take<float>(L * Hp);
+    sb.CD[i] = cv.take<float>(L * Hp);
+    if (c.rnn_cell == NAR_CELL_GRU) { sb.UO[i] = cv.take<float>(L * Hp); sb.RH[i] = cv.take<float>(L * Hp); }
   }
   sb.F1 = cv.take<float>(L * 512);
   sb.PR = cv.take<float>(L * C);
@@ -669,9 +661,9 @@ int planes_build(nar_engine* e) {
   add(c.off_M[0], C, 128, c.ld_M[0]); add(c.off_M[1], 128, 64, c.ld_M[1]); add(c.off_M[2], 64, 32, c.ld_M[2]);
   for (int i = 0; i < c.layers; ++i) {
     const int64_t n_in = i == 0 ? C : Hp;
-    const int64_t wx = c.rnn_cell == 2 ? 4 * Hp : 2 * Hp;
+    const int64_t wx = wh_blocks(c) * Hp;
     add(c.off_Wx[i], n_in, wx, wx);
-    if (c.rnn_cell == 1) add(c.off_Wxc[i], n_in, Hp, Hp);
+    if (c.rnn_cell == NAR_CELL_GRU) add(c.off_Wxc[i], n_in, Hp, Hp);
   }
   if (overflow) return NAR_ERR_INVALID;
   if (!ps.buf) {
@@ -694,7 +686,8 @@ int planes_refresh(nar_engine* e, cudaStream_t st) {
 extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_engine** out) {
   if (!ctx || !cfg || !out) return NAR_ERR_INVALID;
   *out = nullptr;
-  if (cfg->layers < 1 || cfg->layers > NAR_MAX_LAYERS || cfg->rnn_cell < 0 || cfg->rnn_cell > 2 || cfg->ranking < 0 || cfg->ranking > 1)
+  if (cfg->layers < 1 || cfg->layers > NAR_MAX_LAYERS || cfg->rnn_cell < NAR_CELL_UGRNN || cfg->rnn_cell > NAR_CELL_LSTM ||
+      cfg->ranking < 0 || cfg->ranking > 1)
     return NAR_ERR_UNSUPPORTED;
   if ((cfg->C & 3) || (cfg->Hp & 3) || (cfg->Fp & 3) || (cfg->ctx_col0 & 3) || cfg->ctx_col0 <= 0 || cfg->ctx_col0 >= cfg->Fp)
     return NAR_ERR_INVALID;
@@ -708,9 +701,9 @@ extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_eng
   for (int i = 0; i < N_EVENTS; ++i)
     if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   for (int i = 0; i < cfg->layers; ++i) {
-    const size_t wht = (size_t)(cfg->rnn_cell == 2 ? 4 : 2) * cfg->Hp * cfg->Hp;     // transposed recurrent block [2Hp | 4Hp, Hp]
+    const size_t wht = (size_t)wh_blocks(*cfg) * cfg->Hp * cfg->Hp;     // transposed recurrent block [2Hp | 4Hp, Hp]
     if (cudaMalloc(&e->WhT[i], wht * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
-    if (cfg->rnn_cell == 1 && cudaMalloc(&e->WhcT[i], (size_t)cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
+    if (cfg->rnn_cell == NAR_CELL_GRU && cudaMalloc(&e->WhcT[i], (size_t)cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   }
   if (planes_build(e) != NAR_OK) { delete e; return NAR_ERR_INVALID; }
   if (!e->planes.buf || !e->planes.descs) { delete e; return NAR_ERR_NO_DEVICE; }

@@ -180,6 +180,22 @@ def ugrnn_bwd(d_hout, h_out, gate, cand, WhT, sess_off, B, Hp, d_gx, h_prev):
                                 _p(d_gx), _p(h_prev), _stream()), 'nar_ugrnn_bwd')
 
 
+def gru_fwd(gx, Whg, Whc, sess_off, B, Hp, h_out, r_out, u_out, c_out, rh_out):
+    global LAUNCHES
+    LAUNCHES += 1
+    ctx = context()
+    check(ctx.lib.nar_gru_fwd(ctx.handle, _p(gx), _p(Whg), _p(Whc), _p(sess_off), B, Hp, _p(h_out), _p(r_out), _p(u_out),
+                              _p(c_out), _p(rh_out), _stream()), 'nar_gru_fwd')
+
+
+def gru_bwd(d_hout, h_out, r_out, u_out, c_out, WhgT, WhcT, sess_off, B, Hp, d_gx, h_prev):
+    global LAUNCHES
+    LAUNCHES += 1
+    ctx = context()
+    check(ctx.lib.nar_gru_bwd(ctx.handle, _p(d_hout), _p(h_out), _p(r_out), _p(u_out), _p(c_out), _p(WhgT), _p(WhcT),
+                              _p(sess_off), B, Hp, _p(d_gx), _p(h_prev), _stream()), 'nar_gru_bwd')
+
+
 def lstm_fwd(gx, Wh, sess_off, B, Hp, h_out, c_out):
     """gx [L,4Hp] (pre-activations i | j | f | o of the input) is overwritten with the activated gates."""
     global LAUNCHES

@@ -157,6 +157,8 @@ int nar_scatter_add_rows_f32(float* table, int64_t n_table_rows, int64_t ld, int
  *      accumulation in registers.  a_kmajor: A(m,k) = A[m*lda + k] else A[k*lda + m];
  *      b_kmajor: B(n,k) = B[n*ldb + k] else B[k*ldb + n].                                  */
 typedef enum { NAR_ACT_NONE = 0, NAR_ACT_LEAKY_RELU = 1, NAR_ACT_TANH = 2 } nar_act;
+/* session cell, nar_model_cfg.rnn_cell */
+typedef enum { NAR_CELL_UGRNN = 0, NAR_CELL_GRU = 1, NAR_CELL_LSTM = 2 } nar_rnn_cell;
 
 typedef struct {
   const float* bias;      /* [N] added before the activation, or NULL */
@@ -406,7 +408,7 @@ int nar_tf32_lo(const float* x, int64_t n, float* lo, void* stream);
 typedef struct {
   /* dimensions */
   int64_t num_items, C /*CAR_embedding_size*/, Hp /*rnn_units padded to 4*/, Fp /*feature row width*/, ctx_col0;
-  int32_t layers, rnn_cell /*0 = UGRNNCell (nar_model.py:1318), 1 = GRUCell (:1315), 2 = LSTMCell (:1316)*/, ranking /*0 = MLP scorer (:444-500), 1 = cosine*/;
+  int32_t layers, rnn_cell /*nar_rnn_cell: UGRNNCell (nar_model.py:1318), GRUCell (:1315), LSTMCell (:1316)*/, ranking /*0 = MLP scorer (:444-500), 1 = cosine*/;
   int32_t fwd_precision, bwd_precision;       /* nar_gemm_epilogue.precision of the forward (3 or 4) / backward (1 or 3) GEMMs */
   int32_t dedup;                              /* 1: per-unique-id CAR layer 1 (csrc/car.cu); 0: every candidate row materialised */
   int32_t use_aux_stream;                     /* 1: weight / bias gradients (and the forward session branch) on the auxiliary stream */

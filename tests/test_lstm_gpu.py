@@ -1,6 +1,6 @@
-"""rnn_cell='lstm' on the GPU (pytest -m gpu): the recurrence kernels (csrc/lstm.cu) against an fp64 torch recurrence at
-every accepted hidden size, then the whole training / EVAL / PREDICT / checkpoint path against the oracle
-(oracle/lstm_ref.py) at the bars the GRU cell is held to (tests/test_gpu_parity.py)."""
+"""rnn_cell='lstm' on the GPU (pytest -m gpu): the whole training / EVAL / PREDICT / checkpoint path against the oracle
+(oracle/lstm_ref.py) at the bars the GRU cell is held to (tests/test_gpu_parity.py).  The recurrence kernels (csrc/rnn.cu)
+are tested against fp64 in tests/test_rnn_cells_gpu.py."""
 import os
 import sys
 
@@ -11,81 +11,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 pytestmark = pytest.mark.gpu
-
-# session lengths per case: an empty session, single steps, mixed, long; more sessions than one CTA holds (SB = 4)
-LENGTHS = {'single': [1], 'empty_and_one': [0, 1, 0], 'mixed': [3, 0, 1, 7, 2, 1, 5, 4, 20, 1, 2]}
-
-
-def _reference(gx, Wh, lens, dH):
-    """fp64 LSTMCell recurrence over pre-activations gx [L,4H] and its autograd backward of sum(h * dH)."""
-    import torch
-    H = Wh.shape[0]
-    gxr = gx.double().clone().requires_grad_(True)
-    Whr = Wh.double().clone().requires_grad_(True)
-    hs, cs, acts = [], [], []
-    r = 0
-    for n in lens:
-        h = torch.zeros(H, dtype=torch.float64, device=gx.device)
-        c = torch.zeros_like(h)
-        for _ in range(n):
-            z = gxr[r] + h @ Whr
-            i, j, f, o = torch.sigmoid(z[:H]), torch.tanh(z[H:2 * H]), torch.sigmoid(z[2 * H:3 * H] + 1.0), torch.sigmoid(z[3 * H:])
-            c = f * c + i * j
-            h = o * torch.tanh(c)
-            hs.append(h); cs.append(c); acts.append(torch.cat([i, j, f, o]))
-            r += 1
-    Href, Cref, Aref = torch.stack(hs), torch.stack(cs), torch.stack(acts)
-    (Href * dH.double()).sum().backward()
-    return Href.detach(), Cref.detach(), Aref.detach(), gxr.grad, Whr.grad
-
-
-@pytest.mark.parametrize('Hp', [32, 64, 128, 256, 512, 1024])
-@pytest.mark.parametrize('lengths', sorted(LENGTHS))
-def test_lstm_kernels_match_fp64(Hp, lengths):
-    import torch
-    from chameleon_recsys_b200 import ops
-    lens = LENGTHS[lengths]
-    B = len(lens)
-    torch.manual_seed(Hp + B)
-    off = torch.zeros(B + 1, dtype=torch.int32)
-    off[1:] = torch.cumsum(torch.tensor(lens), 0).int()
-    L = int(off[-1])
-    gx = torch.randn(L, 4 * Hp, device='cuda') * 0.5
-    Wh = torch.randn(Hp, 4 * Hp, device='cuda') / (Hp ** 0.5)
-    dH = torch.randn(L, Hp, device='cuda')
-    Href, Cref, Aref, dgx_ref, dWh_ref = _reference(gx, Wh, lens, dH)
-    d_off = off.cuda()
-    act = gx.clone()                                             # overwritten in place with the activated gates
-    h_out = torch.zeros(L, Hp, device='cuda'); c_out = torch.zeros(L, Hp, device='cuda')
-    ops.lstm_fwd(act, Wh, d_off, B, Hp, h_out, c_out)
-    WhT = torch.zeros(4 * Hp, Hp, device='cuda')
-    ops.transpose(Wh, Hp, 4 * Hp, 4 * Hp, WhT, Hp)
-    d_gx = torch.zeros(L, 4 * Hp, device='cuda'); h_prev = torch.zeros(L, Hp, device='cuda')
-    ops.lstm_bwd(dH, h_out, c_out, act, WhT, d_off, B, Hp, d_gx, h_prev)
-    torch.cuda.synchronize()
-    assert (h_out.double() - Href).abs().max().item() < 1e-5
-    assert (c_out.double() - Cref).abs().max().item() < 1e-5
-    assert (act.double() - Aref).abs().max().item() < 1e-5
-    scale = max(dgx_ref.abs().max().item(), 1e-30)
-    assert (d_gx.double() - dgx_ref).abs().max().item() < 1e-5 * max(scale, 1.0)
-    dWh = h_prev.double().t() @ d_gx.double()                       # what the engine's weight-gradient GEMM forms
-    assert (dWh - dWh_ref).abs().max().item() < 1e-4 * max(dWh_ref.abs().max().item(), 1.0)
-
-
-def test_lstm_kernels_reject_the_sizes_the_other_cells_reject():
-    import torch
-    from chameleon_recsys_b200 import _lib, ops
-    ctx = ops.context()
-    x = torch.zeros(16, device='cuda')
-    off = torch.zeros(2, dtype=torch.int32, device='cuda')
-    for Hp in (16, 20, 1028, 2048):
-        rc = ctx.lib.nar_lstm_fwd(ctx.handle, ops._p(x), ops._p(x), ops._p(off), 1, Hp, ops._p(x), ops._p(x), ops._stream())
-        assert rc != 0, Hp
-        rc_u = ctx.lib.nar_ugrnn_fwd(ctx.handle, ops._p(x), ops._p(x), ops._p(off), 1, Hp, ops._p(x), ops._p(x), ops._p(x),
-                                     ops._stream())
-        assert rc_u != 0, Hp
-    with pytest.raises(_lib.NarError):
-        ops.lstm_fwd(x, x, off, 1, 16, x, x)
 
 
 def _check_steps(res, grad_tol=3e-2, update_tol=0.2):
