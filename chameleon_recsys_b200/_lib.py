@@ -62,7 +62,7 @@ class ModelCfg(C.Structure):
                 ('off_gamma', C.c_int64), ('off_beta', C.c_int64),
                 ('off_M', C.c_int64 * 4), ('off_c', C.c_int64 * 4), ('ld_M', C.c_int64 * 4),
                 ('off_Wx', C.c_int64 * NAR_MAX_LAYERS), ('off_Wh', C.c_int64 * NAR_MAX_LAYERS), ('off_rb', C.c_int64 * NAR_MAX_LAYERS),
-                ('off_Wxc', C.c_int64 * NAR_MAX_LAYERS), ('off_Whc', C.c_int64 * NAR_MAX_LAYERS), ('off_bc', C.c_int64 * NAR_MAX_LAYERS),
+                ('off_Whc', C.c_int64 * NAR_MAX_LAYERS),
                 ('plan', FeaturePlanC)]
 
 
@@ -192,7 +192,7 @@ def load() -> C.CDLL:
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    if lib.nar_abi_version() != 2:
+    if lib.nar_abi_version() != 3:
         raise NarError('ABI version mismatch')
     _lib = lib
     return lib

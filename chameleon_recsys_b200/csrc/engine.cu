@@ -81,8 +81,7 @@ struct nar_engine {
   cudaStream_t aux;
   cudaEvent_t ev[N_EVENTS];
   int ev_i;
-  float* WhT[NAR_MAX_LAYERS];
-  float* WhcT[NAR_MAX_LAYERS];     // GRU: transposed candidate recurrent block
+  float* WhT[NAR_MAX_LAYERS];       // transposed recurrent blocks [gate_blocks * Hp, Hp] (GRU: Whg, then Whc)
   int64_t launches;
   int fused_product;               // NAR_FUSED_SCORER_PRODUCT (default 1), read when the engine is created
 };
@@ -99,10 +98,8 @@ bool fused_product(const nar_engine* e) {
   return e->fused_product && c.ranking == 0 && c.K + 1 <= 128 && c.fwd_precision == 4 && c.bwd_precision == 1;
 }
 
-// gate blocks per unit (GX width): UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o)
+// gate blocks per unit (the width of GX, Wx and the bias): UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o)
 int64_t gate_blocks(const nar_model_cfg& c) { return c.rnn_cell == NAR_CELL_LSTM ? 4 : c.rnn_cell == NAR_CELL_GRU ? 3 : 2; }
-// blocks per unit of the Wx / Wh parameter blocks (and WhT): the GRU's candidate lives in Wxc / Whc
-int64_t wh_blocks(const nar_model_cfg& c) { return c.rnn_cell == NAR_CELL_LSTM ? 4 : 2; }
 
 int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_t L_cap, void* base, PrepBufs* pb) {
   const nar_model_cfg& c = e->cfg;
@@ -124,6 +121,19 @@ int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_
   return cv.off;
 }
 
+// the session branch's buffers for L rows (what clicked_rows_forward writes), in the same order for a step and a recommend call
+void session_carve(const nar_model_cfg& c, int64_t L, Carver& cv, StepBufs* sb) {
+  const int64_t Hp = c.Hp;
+  for (int i = 0; i < c.layers; ++i) {
+    sb->GX[i] = cv.take<float>(L * gate_blocks(c) * Hp); sb->HO[i] = cv.take<float>(L * Hp);
+    if (c.rnn_cell != NAR_CELL_LSTM) sb->GT[i] = cv.take<float>(L * Hp);
+    sb->CD[i] = cv.take<float>(L * Hp);
+    if (c.rnn_cell == NAR_CELL_GRU) { sb->UO[i] = cv.take<float>(L * Hp); sb->RH[i] = cv.take<float>(L * Hp); }
+  }
+  sb->F1 = cv.take<float>(L * 512);
+  sb->PR = cv.take<float>(L * c.C);
+}
+
 int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, StepBufs* sb) {
   const nar_model_cfg& c = e->cfg;
   const int64_t K = c.K, n_cand = K + 1, Rc = L_cap * n_cand, R = L_cap + Rc, C = c.C, Hp = c.Hp, Fp = c.Fp;
@@ -133,15 +143,7 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
   if (c.dedup) { sb->X = cv.take<float>(NB * Fp); } else { sb->X = cv.take<float>(R * Fp); }
   sb->H1 = cv.take<float>(R * C);
   sb->E = cv.take<float>(R * C);
-  const int64_t gw = gate_blocks(c);
-  for (int i = 0; i < c.layers; ++i) {
-    sb->GX[i] = cv.take<float>(L_cap * gw * Hp); sb->HO[i] = cv.take<float>(L_cap * Hp);
-    if (c.rnn_cell != NAR_CELL_LSTM) sb->GT[i] = cv.take<float>(L_cap * Hp);
-    sb->CD[i] = cv.take<float>(L_cap * Hp);
-    if (c.rnn_cell == NAR_CELL_GRU) { sb->UO[i] = cv.take<float>(L_cap * Hp); sb->RH[i] = cv.take<float>(L_cap * Hp); }
-  }
-  sb->F1 = cv.take<float>(L_cap * 512);
-  sb->PR = cv.take<float>(L_cap * C);
+  session_carve(c, L_cap, cv, sb);
   sb->logits = cv.take<float>(L_cap * n_cand);
   if (c.dedup) { sb->PP = cv.take<float>(L_cap * C); sb->PI = cv.take<float>(U * C); sb->PC = cv.take<float>(L_cap * C); }
   const bool fused = fused_product(e);
@@ -153,7 +155,7 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
     sb->dE = cv.take<float>(R * C);
     sb->dPR = cv.take<float>(L_cap * C); sb->dF1 = cv.take<float>(L_cap * 512); sb->dHO = cv.take<float>(L_cap * Hp);
     for (int i = 0; i < c.layers; ++i) {
-      sb->dGX[i] = cv.take<float>(L_cap * gw * Hp); sb->HPV[i] = cv.take<float>(L_cap * Hp); sb->dHOb[i] = cv.take<float>(L_cap * Hp);
+      sb->dGX[i] = cv.take<float>(L_cap * gate_blocks(c) * Hp); sb->HPV[i] = cv.take<float>(L_cap * Hp); sb->dHOb[i] = cv.take<float>(L_cap * Hp);
     }
     if (c.ranking == 0) {
       sb->dZ3 = cv.take<float>(Rc * 32); sb->dZ2 = cv.take<float>(Rc * 64); sb->dZ1 = cv.take<float>(Rc * 128);
@@ -278,13 +280,11 @@ void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
   s.fwd(sb.H1, C, c.off_W2, C, c.off_b2, sb.E, C, L, C, C, NAR_ACT_TANH, s.main);
   cudaStream_t st = s.fork();
   const float* rnn_in = sb.E; int64_t n_in = C;
-  const int64_t wx = wh_blocks(c) * Hp, gw = gate_blocks(c) * Hp;
+  const int64_t gw = gate_blocks(c) * Hp;
   for (int i = 0; i < c.layers; ++i) {
     // input projection gx = x Wx + b, then the recurrence (csrc/rnn.cu)
-    s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], wx, c.off_rb[i], sb.GX[i], gw, L, wx, n_in, NAR_ACT_NONE, st);
+    s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], gw, c.off_rb[i], sb.GX[i], gw, L, gw, n_in, NAR_ACT_NONE, st);
     if (c.rnn_cell == NAR_CELL_GRU) {
-      // GRUCell: gx = (x Wxg + bg | x Wxc + bc), the candidate's projection from its own block
-      s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wxc[i], Hp, c.off_bc[i], sb.GX[i] + 2 * Hp, 3 * Hp, L, Hp, n_in, NAR_ACT_NONE, st);
       s.chk(nar_gru_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), s.W(c.off_Whc[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.UO[i],
                         sb.CD[i], sb.RH[i], st));
     } else if (c.rnn_cell == NAR_CELL_LSTM) {
@@ -417,48 +417,36 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
       if (drop) s.dropout(dho, dho, L, Hp, io->pos_idx, 8 + i, main);   // gradient of the dropped cell output
       const float* x_in = i == 0 ? sb.E : (drop ? sb.HOd[i - 1] : sb.HO[i - 1]);
       const int64_t n_in = i == 0 ? C : Hp;
+      // gx, Wx and the bias are gw wide; the recurrent blocks differ per cell
+      const int64_t gw = gate_blocks(c) * Hp;
       if (c.rnn_cell == NAR_CELL_GRU) {
-        const int64_t W3 = 3 * Hp;
+        float* cand_T = e->WhT[i] + 2 * Hp * Hp;     // Whc transposed, after Whg transposed
         s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, 2 * Hp, 2 * Hp, e->WhT[i], Hp, main));
-        s.chk(nar_transpose_f32(s.W(c.off_Whc[i]), Hp, Hp, Hp, e->WhcT[i], Hp, main));
-        s.chk(nar_gru_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.UO[i], sb.CD[i], e->WhT[i], e->WhcT[i], io->sess_off, B, Hp, sb.dGX[i],
+        s.chk(nar_transpose_f32(s.W(c.off_Whc[i]), Hp, Hp, Hp, cand_T, Hp, main));
+        s.chk(nar_gru_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.UO[i], sb.CD[i], e->WhT[i], cand_T, io->sess_off, B, Hp, sb.dGX[i],
                           sb.HPV[i], main));
-        const float* dg = sb.dGX[i]; const float* dc = sb.dGX[i] + 2 * Hp;
-        {
-          cudaStream_t st = s.fork();
-          s.wgrad(x_in, n_in, dg, W3, c.off_Wx[i], 2 * Hp, n_in, 2 * Hp, L, st);
-          s.wgrad(x_in, n_in, dc, W3, c.off_Wxc[i], Hp, n_in, Hp, L, st);
-          s.wgrad(sb.HPV[i], Hp, dg, W3, c.off_Wh[i], 2 * Hp, Hp, 2 * Hp, L, st);
-          s.wgrad(sb.RH[i], Hp, dc, W3, c.off_Whc[i], Hp, Hp, Hp, L, st);
-          s.bgrad(dg, W3, L, 2 * Hp, c.off_rb[i], st);
-          s.bgrad(dc, W3, L, Hp, c.off_bc[i], st);
-        }
-        // d(input) = d_gx[:, :2Hp] Wxg^T + d_gx[:, 2Hp:] Wxc^T (two GEMMs into one buffer), then through the CAR tanh for layer 0
-        float* dxin = i == 0 ? sb.dE : sb.dHOb[i];
-        const int64_t ldx = i == 0 ? C : Hp;
-        s.dgrad(dg, W3, c.off_Wx[i], 2 * Hp, dxin, ldx, L, n_in, 2 * Hp, NAR_ACT_NONE, nullptr, 0, 0, main);
-        s.dgrad(dc, W3, c.off_Wxc[i], Hp, dxin, ldx, L, n_in, Hp, NAR_ACT_NONE, nullptr, 0, 1, main);
-        if (i == 0) s.chk(nar_act_bwd(sb.dE, sb.E, L * C, NAR_ACT_TANH, sb.dE, main));
-        else dho = sb.dHOb[i];
-        continue;
+      } else {
+        s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, gw, gw, e->WhT[i], Hp, main));
+        if (c.rnn_cell == NAR_CELL_LSTM)
+          s.chk(nar_lstm_bwd(e->ctx, dho, sb.HO[i], sb.CD[i], sb.GX[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
+        else
+          s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
       }
-      // UGRNN and LSTM: gx, Wx, Wh and the bias are all wh_blocks(c) * Hp wide
-      const int64_t wx = wh_blocks(c) * Hp;
-      s.chk(nar_transpose_f32(s.W(c.off_Wh[i]), Hp, wx, wx, e->WhT[i], Hp, main));
-      if (c.rnn_cell == NAR_CELL_LSTM)
-        s.chk(nar_lstm_bwd(e->ctx, dho, sb.HO[i], sb.CD[i], sb.GX[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
-      else
-        s.chk(nar_ugrnn_bwd(e->ctx, dho, sb.HO[i], sb.GT[i], sb.CD[i], e->WhT[i], io->sess_off, B, Hp, sb.dGX[i], sb.HPV[i], main));
       {
         cudaStream_t st = s.fork();
-        s.wgrad(x_in, n_in, sb.dGX[i], wx, c.off_Wx[i], wx, n_in, wx, L, st);
-        s.wgrad(sb.HPV[i], Hp, sb.dGX[i], wx, c.off_Wh[i], wx, Hp, wx, L, st);
-        s.bgrad(sb.dGX[i], wx, L, wx, c.off_rb[i], st);
+        s.wgrad(x_in, n_in, sb.dGX[i], gw, c.off_Wx[i], gw, n_in, gw, L, st);
+        if (c.rnn_cell == NAR_CELL_GRU) {     // dWhg = h_prev^T d_gx[:, :2Hp], dWhc = (r * h_prev)^T d_gx[:, 2Hp:]
+          s.wgrad(sb.HPV[i], Hp, sb.dGX[i], gw, c.off_Wh[i], 2 * Hp, Hp, 2 * Hp, L, st);
+          s.wgrad(sb.RH[i], Hp, sb.dGX[i] + 2 * Hp, gw, c.off_Whc[i], Hp, Hp, Hp, L, st);
+        } else {
+          s.wgrad(sb.HPV[i], Hp, sb.dGX[i], gw, c.off_Wh[i], gw, Hp, gw, L, st);
+        }
+        s.bgrad(sb.dGX[i], gw, L, gw, c.off_rb[i], st);
       }
       if (i == 0) {
-        s.dgrad(sb.dGX[0], wx, c.off_Wx[0], wx, sb.dE, C, L, C, wx, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
+        s.dgrad(sb.dGX[0], gw, c.off_Wx[0], gw, sb.dE, C, L, C, gw, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
       } else {
-        s.dgrad(sb.dGX[i], wx, c.off_Wx[i], wx, sb.dHOb[i], Hp, L, Hp, wx, NAR_ACT_NONE, nullptr, 0, 0, main);
+        s.dgrad(sb.dGX[i], gw, c.off_Wx[i], gw, sb.dHOb[i], Hp, L, Hp, gw, NAR_ACT_NONE, nullptr, 0, 0, main);
         dho = sb.dHOb[i];
       }
     }
@@ -507,7 +495,7 @@ struct RecBufs {
 int64_t rec_carve(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int64_t qb, int64_t nb, int gather_q, void* base,
                   RecBufs* rb) {
   const nar_model_cfg& c = e->cfg;
-  const int64_t C = c.C, Hp = c.Hp, Fp = c.Fp, gw = gate_blocks(c), P = qb * nb;
+  const int64_t C = c.C, Fp = c.Fp, P = qb * nb;
   memset(rb, 0, sizeof(*rb));
   StepBufs& sb = rb->sb;
   Carver cv(base);
@@ -518,14 +506,7 @@ int64_t rec_carve(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int64_t 
   sb.X = cv.take<float>((L + N) * Fp);
   sb.H1 = cv.take<float>(L * C);
   sb.E = cv.take<float>(L * C);
-  for (int i = 0; i < c.layers; ++i) {
-    sb.GX[i] = cv.take<float>(L * gw * Hp); sb.HO[i] = cv.take<float>(L * Hp);
-    if (c.rnn_cell != NAR_CELL_LSTM) sb.GT[i] = cv.take<float>(L * Hp);
-    sb.CD[i] = cv.take<float>(L * Hp);
-    if (c.rnn_cell == NAR_CELL_GRU) { sb.UO[i] = cv.take<float>(L * Hp); sb.RH[i] = cv.take<float>(L * Hp); }
-  }
-  sb.F1 = cv.take<float>(L * 512);
-  sb.PR = cv.take<float>(L * C);
+  session_carve(c, L, cv, &sb);
   rb->PC = cv.take<float>(L * C);
   rb->PCq = gather_q ? cv.take<float>(Q * C) : rb->PC;
   rb->PRq = gather_q ? cv.take<float>(Q * C) : sb.PR;
@@ -660,10 +641,8 @@ int planes_build(nar_engine* e) {
   add(c.off_W2, C, C, C); add(c.off_W3, Hp, 512, 512); add(c.off_W4, 512, C, C);
   add(c.off_M[0], C, 128, c.ld_M[0]); add(c.off_M[1], 128, 64, c.ld_M[1]); add(c.off_M[2], 64, 32, c.ld_M[2]);
   for (int i = 0; i < c.layers; ++i) {
-    const int64_t n_in = i == 0 ? C : Hp;
-    const int64_t wx = wh_blocks(c) * Hp;
-    add(c.off_Wx[i], n_in, wx, wx);
-    if (c.rnn_cell == NAR_CELL_GRU) add(c.off_Wxc[i], n_in, Hp, Hp);
+    const int64_t gw = gate_blocks(c) * Hp;
+    add(c.off_Wx[i], i == 0 ? C : Hp, gw, gw);
   }
   if (overflow) return NAR_ERR_INVALID;
   if (!ps.buf) {
@@ -701,9 +680,8 @@ extern "C" int nar_engine_create(nar_ctx* ctx, const nar_model_cfg* cfg, nar_eng
   for (int i = 0; i < N_EVENTS; ++i)
     if (cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   for (int i = 0; i < cfg->layers; ++i) {
-    const size_t wht = (size_t)wh_blocks(*cfg) * cfg->Hp * cfg->Hp;     // transposed recurrent block [2Hp | 4Hp, Hp]
+    const size_t wht = (size_t)gate_blocks(*cfg) * cfg->Hp * cfg->Hp;
     if (cudaMalloc(&e->WhT[i], wht * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
-    if (cfg->rnn_cell == NAR_CELL_GRU && cudaMalloc(&e->WhcT[i], (size_t)cfg->Hp * cfg->Hp * sizeof(float)) != cudaSuccess) { delete e; return NAR_ERR_NO_DEVICE; }
   }
   if (planes_build(e) != NAR_OK) { delete e; return NAR_ERR_INVALID; }
   if (!e->planes.buf || !e->planes.descs) { delete e; return NAR_ERR_NO_DEVICE; }
@@ -719,7 +697,7 @@ extern "C" int nar_engine_refresh(nar_engine* e, void* stream) {
 extern "C" int nar_engine_destroy(nar_engine* e) {
   if (!e) return NAR_OK;
   cudaStreamSynchronize(e->aux);
-  for (int i = 0; i < NAR_MAX_LAYERS; ++i) { if (e->WhT[i]) cudaFree(e->WhT[i]); if (e->WhcT[i]) cudaFree(e->WhcT[i]); }
+  for (int i = 0; i < NAR_MAX_LAYERS; ++i) if (e->WhT[i]) cudaFree(e->WhT[i]);
   for (int i = 0; i < N_EVENTS; ++i) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
   if (e->aux) cudaStreamDestroy(e->aux);
   if (e->planes.buf) cudaFree(e->planes.buf);
@@ -832,8 +810,7 @@ extern "C" int nar_engine_buffer(const nar_engine* e, const nar_step_io* io, con
       {"logits", sb.logits, L, n_cand}, {"PD", sb.PD, Rc, c.C}, {"Z1", sb.Z1, Rc, 128}, {"Z2", sb.Z2, Rc, 64}, {"Z3", sb.Z3, Rc, 32}, {"PP", sb.PP, L, c.C},
       {"PI", sb.PI, pb.U, c.C}, {"PC", sb.PC, L, c.C}, {"DB", sb.DB, 3 * L + pb.U, c.C},
       {"HO0", sb.HO[0], L, c.Hp}, {"HO1", sb.HO[1], L, c.Hp}, {"HO2", sb.HO[2], L, c.Hp}, {"HO3", sb.HO[3], L, c.Hp},
-      {"HOd0", sb.HOd[0], L, c.Hp}, {"HOd1", sb.HOd[1], L, c.Hp}, {"HOd2", sb.HOd[2], L, c.Hp}, {"HOd3", sb.HOd[3], L, c.Hp},
-      {"GX0", sb.GX[0], L, 2 * c.Hp}, {"dGX0", sb.dGX[0], L, 2 * c.Hp}};
+      {"HOd0", sb.HOd[0], L, c.Hp}, {"HOd1", sb.HOd[1], L, c.Hp}, {"HOd2", sb.HOd[2], L, c.Hp}, {"HOd3", sb.HOd[3], L, c.Hp}};
   for (const Ent& t : tab)
     if (strcmp(t.n, name) == 0) {
       *ptr = t.p;

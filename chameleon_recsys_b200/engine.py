@@ -174,7 +174,7 @@ class NarEngine:
         for i in range(self.layers):
             c.off_Wx[i], c.off_Wh[i], c.off_rb[i] = off('rnn%d/Wx' % i), off('rnn%d/Wh' % i), off('rnn%d/b' % i)
             if self.rnn_cell == 'gru':
-                c.off_Wxc[i], c.off_Whc[i], c.off_bc[i] = off('rnn%d/Wxc' % i), off('rnn%d/Whc' % i), off('rnn%d/bc' % i)
+                c.off_Whc[i] = off('rnn%d/Whc' % i)
         c.plan = self._plan_c_static()
         return c
 

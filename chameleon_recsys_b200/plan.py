@@ -197,8 +197,8 @@ class ParamTensor:
     # how the logical tensor maps into the internal one
     row_map: Optional[np.ndarray] = None   # internal row index for each logical row
     col_map: Optional[np.ndarray] = None   # internal col index for each logical col
-    part_of: Optional[str] = None          # logical tensor this is a slice of (RNN kernel split)
-    part_rows: Optional[Tuple[int, int]] = None
+    part_rows: Optional[Tuple[int, int]] = None   # rows of the logical tensor this one holds (RNN kernel split)
+    into: Optional[str] = None    # key of the tensor whose storage this one fills (same rows and ld, none of its own)
 
     @property
     def size(self) -> int:
@@ -250,55 +250,37 @@ class ParamLayout:
         noreg.append(ParamTensor('b1', 'main/CAR/PreCAR_representation/bias', (C,), INIT_ZEROS, False, rows=1, ld=C))
         reg.append(ParamTensor('W2', 'main/CAR/CAR_representation/kernel', (C, C), INIT_XAVIER, True, rows=C, ld=C))
         noreg.append(ParamTensor('b2', 'main/CAR/CAR_representation/bias', (C,), INIT_ZEROS, False, rows=1, ld=C))
-        # nar_model.py:1308-1342  (tf.contrib.rnn.UGRNNCell: kernel [in+H, 2H], bias [2H]; not regularised)
-        gate_cols = np.concatenate([np.arange(H), Hp + np.arange(H)])
-        for i in range(self.layers if rnn_cell == 'gru' else 0):
-            # tf.nn.rnn_cell.GRUCell (nar_model.py:1315, commented alternative): gates/kernel [in+H, 2H] (r | u), gates/bias
-            # (constant 1.0), candidate/kernel [in+H, H], candidate/bias (zeros); split into input and recurrent blocks
+        # nar_model.py:1308-1342, not regularised.  Per cell: its TF scope, then per TF kernel [in+H, n*H] and bias [n*H] the
+        # prefix, the n column blocks, the bias initialiser and the key of the recurrent block:
+        #   tf.contrib.rnn.UGRNNCell    kernel (gate | candidate)
+        #   tf.nn.rnn_cell.GRUCell      gates/kernel (r | u), bias 1.0; candidate/kernel (:1315, commented alternative)
+        #   tf.nn.rnn_cell.LSTMCell     kernel (i | j | f | o); forget_bias 1.0 is a constant inside the cell (:1316, idem)
+        # Every column block goes to an Hp-wide block.  The input rows of a layer's kernels fill one Wx [in, G*Hp] and its
+        # biases one b [G*Hp] (G = 2, 3 or 4: one input projection per layer).  The recurrent rows of each kernel are a block
+        # of their own: the GRU's candidate multiplies r*h, not h, so its Whc is a separate product.
+        cells = {'ugrnn': ('ugrnn_cell/', [('', 2, INIT_ZEROS, 'Wh')]),
+                 'gru': ('gru_cell/', [('gates/', 2, INIT_ONES, 'Wh'), ('candidate/', 1, INIT_ZEROS, 'Whc')]),
+                 'lstm': ('lstm_cell/', [('', 4, INIT_ZEROS, 'Wh')])}
+        if rnn_cell not in cells:
+            raise ValueError('rnn_cell=%r: one of %s' % (rnn_cell, sorted(cells)))
+        scope, kernels = cells[rnn_cell]
+        G = sum(n for _, n, _, _ in kernels)
+        for i in range(self.layers):
             n_in = C if i == 0 else H
             n_in_p = C if i == 0 else Hp
-            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/gru_cell/'.format(i)
-            gk, ck = base + 'gates/kernel', base + 'candidate/kernel'
-            noreg.append(ParamTensor('rnn%d/Wx' % i, gk, (n_in + H, 2 * H), INIT_XAVIER, False, rows=n_in_p, ld=2 * Hp,
-                                     col_map=gate_cols, part_of=gk, part_rows=(0, n_in), row_map=np.arange(n_in)))
-            noreg.append(ParamTensor('rnn%d/Wh' % i, gk, (n_in + H, 2 * H), INIT_XAVIER, False, rows=Hp, ld=2 * Hp,
-                                     col_map=gate_cols, part_of=gk, part_rows=(n_in, n_in + H), row_map=np.arange(H)))
-            noreg.append(ParamTensor('rnn%d/b' % i, base + 'gates/bias', (2 * H,), INIT_ONES, False, rows=1, ld=2 * Hp,
-                                     col_map=gate_cols))
-            noreg.append(ParamTensor('rnn%d/Wxc' % i, ck, (n_in + H, H), INIT_XAVIER, False, rows=n_in_p, ld=Hp,
-                                     col_map=np.arange(H), part_of=ck, part_rows=(0, n_in), row_map=np.arange(n_in)))
-            noreg.append(ParamTensor('rnn%d/Whc' % i, ck, (n_in + H, H), INIT_XAVIER, False, rows=Hp, ld=Hp,
-                                     col_map=np.arange(H), part_of=ck, part_rows=(n_in, n_in + H), row_map=np.arange(H)))
-            noreg.append(ParamTensor('rnn%d/bc' % i, base + 'candidate/bias', (H,), INIT_ZEROS, False, rows=1, ld=Hp,
-                                     col_map=np.arange(H)))
-        lstm_cols = np.concatenate([k * Hp + np.arange(H) for k in range(4)])
-        for i in range(self.layers if rnn_cell == 'lstm' else 0):
-            # tf.nn.rnn_cell.LSTMCell(H, state_is_tuple=True) (nar_model.py:1316, commented alternative): lstm_cell/kernel
-            # [in+H, 4H] (i | j | f | o), lstm_cell/bias [4H] (zeros; forget_bias 1.0 is a constant inside the cell); the four
-            # column blocks go to Hp-wide blocks, the rows split into input and recurrent parts
-            n_in = C if i == 0 else H
-            n_in_p = C if i == 0 else Hp
-            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/lstm_cell/'.format(i)
-            noreg.append(ParamTensor('rnn%d/Wx' % i, base + 'kernel', (n_in + H, 4 * H), INIT_XAVIER, False,
-                                     rows=n_in_p, ld=4 * Hp, col_map=lstm_cols, part_of=base + 'kernel',
-                                     part_rows=(0, n_in), row_map=np.arange(n_in)))
-            noreg.append(ParamTensor('rnn%d/Wh' % i, base + 'kernel', (n_in + H, 4 * H), INIT_XAVIER, False,
-                                     rows=Hp, ld=4 * Hp, col_map=lstm_cols, part_of=base + 'kernel',
-                                     part_rows=(n_in, n_in + H), row_map=np.arange(H)))
-            noreg.append(ParamTensor('rnn%d/b' % i, base + 'bias', (4 * H,), INIT_ZEROS, False,
-                                     rows=1, ld=4 * Hp, col_map=lstm_cols))
-        for i in range(self.layers if rnn_cell not in ('gru', 'lstm') else 0):
-            n_in = C if i == 0 else H
-            n_in_p = C if i == 0 else Hp
-            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/ugrnn_cell/'.format(i)
-            noreg.append(ParamTensor('rnn%d/Wx' % i, base + 'kernel', (n_in + H, 2 * H), INIT_XAVIER, False,
-                                     rows=n_in_p, ld=2 * Hp, col_map=gate_cols, part_of=base + 'kernel',
-                                     part_rows=(0, n_in), row_map=np.arange(n_in)))
-            noreg.append(ParamTensor('rnn%d/Wh' % i, base + 'kernel', (n_in + H, 2 * H), INIT_XAVIER, False,
-                                     rows=Hp, ld=2 * Hp, col_map=gate_cols, part_of=base + 'kernel',
-                                     part_rows=(n_in, n_in + H), row_map=np.arange(H)))
-            noreg.append(ParamTensor('rnn%d/b' % i, base + 'bias', (2 * H,), INIT_ZEROS, False,
-                                     rows=1, ld=2 * Hp, col_map=gate_cols))
+            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/'.format(i) + scope
+            wx, b = 'rnn%d/Wx' % i, 'rnn%d/b' % i
+            g0 = 0
+            for prefix, n, b_init, wh in kernels:
+                k, cols = base + prefix + 'kernel', np.concatenate([g * Hp + np.arange(H) for g in range(n)])
+                noreg.append(ParamTensor(wx, k, (n_in + H, n * H), INIT_XAVIER, False, rows=n_in_p, ld=G * Hp,
+                                         col_map=g0 * Hp + cols, part_rows=(0, n_in), row_map=np.arange(n_in),
+                                         into=wx if g0 else None))
+                noreg.append(ParamTensor('rnn%d/%s' % (i, wh), k, (n_in + H, n * H), INIT_XAVIER, False, rows=Hp, ld=n * Hp,
+                                         col_map=cols, part_rows=(n_in, n_in + H), row_map=np.arange(H)))
+                noreg.append(ParamTensor(b, base + prefix + 'bias', (n * H,), b_init, False, rows=1, ld=G * Hp,
+                                         col_map=g0 * Hp + cols, into=b if g0 else None))
+                g0 += n
         # nar_model.py:410-426
         reg.append(ParamTensor('W3', 'main/session_representation/FC1/kernel', (H, 512), INIT_VAR_SCALING, True,
                                rows=Hp, ld=512, row_map=np.arange(H)))
@@ -317,13 +299,17 @@ class ParamLayout:
                                      rows=1, ld=ld, col_map=np.arange(dims[li + 1])))
         self.tensors: List[ParamTensor] = reg + noreg
         off = 0
+        self.by_key: Dict[str, ParamTensor] = {}
         for t in self.tensors:
+            if t.into is not None:
+                t.offset = self.by_key[t.into].offset
+                continue
             t.offset = off
             off += round_up(t.size, 4)
             if t.reg:
                 self.reg_end = off
+            self.by_key[t.key] = t
         self.total = off
-        self.by_key: Dict[str, ParamTensor] = {t.key: t for t in self.tensors}
 
     # ---- logical <-> internal -------------------------------------------------
     def logical_names(self) -> List[str]:

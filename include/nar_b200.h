@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define NAR_ABI_VERSION 2
+#define NAR_ABI_VERSION 3
 
 typedef enum {
   NAR_OK = 0,
@@ -230,7 +230,7 @@ int nar_ugrnn_bwd(nar_ctx* ctx, const float* d_hout /*[L,Hp]*/, const float* h_o
                   const float* cand, const float* WhT /*[2Hp,Hp]*/, const int32_t* sess_off, int64_t B,
                   int64_t Hp, float* d_gx /*[L,2Hp]*/, float* h_prev /*[L,Hp]*/, void* stream);
 
-/* GRU recurrence (tf.nn.rnn_cell.GRUCell; rnn_cell='gru'): gx [L,3Hp] = x*Wxg + bg | x*Wxc + bc (r | u | c pre-activations
+/* GRU recurrence (tf.nn.rnn_cell.GRUCell; rnn_cell='gru'): gx [L,3Hp] = x*Wx + b with Wx [in,3Hp] (r | u | c pre-activations
  * of the input), Whg [Hp,2Hp], Whc [Hp,Hp]:  [r,u] = sigmoid(gx_ru + h*Whg) ; c = tanh(gx_c + (r*h)*Whc) ;
  * h' = u*h + (1-u)*c.  Outputs per row: state h_out, gates r / u, candidate c, rh = r * (state entering the step).      */
 int nar_gru_fwd(nar_ctx* ctx, const float* gx, const float* Whg, const float* Whc, const int32_t* sess_off, int64_t B,
@@ -425,8 +425,9 @@ typedef struct {
   int64_t n_params, reg_end;
   int64_t off_W1, off_b1, off_W2, off_b2, off_W3, off_b3, off_W4, off_b4, off_gamma, off_beta;
   int64_t off_M[4], off_c[4], ld_M[4];        /* matching_dense_layer_1..4 kernels / biases, leading dimensions */
-  int64_t off_Wx[NAR_MAX_LAYERS], off_Wh[NAR_MAX_LAYERS], off_rb[NAR_MAX_LAYERS];     /* UGRNN: [in|H, 2Hp] (gate | candidate); GRU: gates (r | u); LSTM: [in|H, 4Hp] (i | j | f | o) */
-  int64_t off_Wxc[NAR_MAX_LAYERS], off_Whc[NAR_MAX_LAYERS], off_bc[NAR_MAX_LAYERS];  /* GRU only: candidate blocks [in|H, Hp] */
+  /* per layer: Wx [in, G*Hp] and b [G*Hp], G gate blocks: UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o);
+   * Wh [Hp, G*Hp], except the GRU's Wh [Hp, 2Hp] (r | u) and Whc [Hp, Hp] (candidate: a product with r*h) */
+  int64_t off_Wx[NAR_MAX_LAYERS], off_Wh[NAR_MAX_LAYERS], off_rb[NAR_MAX_LAYERS], off_Whc[NAR_MAX_LAYERS];
   /* feature plan: static part (segments, tables, metadata, created_at_ts, gamma / beta, column map) */
   nar_feature_plan plan;
 } nar_model_cfg;

@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), name
     assert sorted(_lib.EXPORTED_SYMBOLS) == declared
-    assert lib.nar_abi_version() == 2
+    assert lib.nar_abi_version() == 3
     # the ctypes mirrors of the ABI structs have the C layout (a padding mismatch would corrupt every call)
     for which, cls in enumerate((_lib.FeaturePlanC, _lib.ModelCfg, _lib.StepIO, _lib.RowLayout, _lib.GemmEpilogue, _lib.Segment)):
         import ctypes

@@ -1,5 +1,6 @@
 """rnn_cell='lstm' on the CPU: the oracle's LSTM branch (oracle/lstm_ref.py) against outputs of the REFERENCE's own model
-code, a hand-sized cell step, finite differences through two layers, and the parameter layout's TF-name round trip.
+code, a hand-sized cell step, finite differences through two layers, and the parameter layout's TF-name round trip (for
+the GRU as well).
 
 tests/golden/lstm_golden.npz ran nar_model.py unmodified on the TF-1.x stand-in with an LSTMCell stand-in in place of
 UGRNNCell (= un-commenting nar_model.py:1316; generator tests/golden/make_lstm_golden.py).  That pins the cell's place
@@ -169,34 +170,44 @@ def test_finite_difference_gradients_two_layers():
 
 
 def test_param_layout_round_trip_h255():
-    """ParamLayout(rnn_cell='lstm') at H = 255 (Hp = 256), two layers: logical -> internal -> logical is exact, the four
-    TF column blocks land in Hp-wide blocks, and the padding rows / columns stay zero."""
-    pb = make_problem('tiny', profile='B', rnn_cell='lstm', rnn_units=255, rnn_num_layers=2)
-    lay = pb.layout
-    H, Hp, C = 255, 256, lay.C
-    assert lay.Hp == Hp
-    rs = np.random.RandomState(3)
-    lg = {k: rs.randn(*v.shape).astype(np.float32) for k, v in lay.init_logical(1).items()}
-    back = lay.to_logical(lay.to_internal(lg))
-    assert sorted(back) == sorted(lg)
-    for k in lg:
-        assert np.array_equal(back[k], lg[k]), k
-    flat = lay.to_internal(lg)
-    for i, n_in, n_in_p in ((0, C, C), (1, H, Hp)):
-        base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/lstm_cell/'.format(i)
-        k = lg[base + 'kernel']
-        assert k.shape == (n_in + H, 4 * H) and lg[base + 'bias'].shape == (4 * H,)
-        for key, rows, lrows in (('Wx', n_in_p, k[:n_in]), ('Wh', Hp, k[n_in:])):
-            t = lay.by_key['rnn%d/%s' % (i, key)]
-            m = flat[t.offset:t.offset + t.size].reshape(rows, 4 * Hp)
-            for g in range(4):                                   # i | j | f | o
-                assert np.array_equal(m[:lrows.shape[0], g * Hp:g * Hp + H], lrows[:, g * H:(g + 1) * H])
-                assert not m[:, g * Hp + H:(g + 1) * Hp].any()
-            assert not m[lrows.shape[0]:].any()
-        t = lay.by_key['rnn%d/b' % i]
-        b = flat[t.offset:t.offset + t.size].reshape(4, Hp)
-        assert np.array_equal(b[:, :H], lg[base + 'bias'].reshape(4, H)) and not b[:, H:].any()
-    # initialisers: Xavier kernel, zero bias, not L2-regularised
-    init = lay.init_logical(42)
-    assert not init['main/RNN/rnn/multi_rnn_cell/cell_0/lstm_cell/bias'].any()
-    assert all(not lay.by_key['rnn%d/%s' % (i, k)].reg for i in range(2) for k in ('Wx', 'Wh', 'b'))
+    """ParamLayout(rnn_cell='lstm' and 'gru') at H = 255 (Hp = 256), two layers: logical -> internal -> logical is exact,
+    every TF column block lands in its Hp-wide block (LSTM i | j | f | o; GRU r | u from gates/*, c from candidate/*), the
+    input rows and biases of a layer in one Wx / b, the recurrent rows in Wh (GRU: Wh and Whc), and the padding rows /
+    columns stay zero."""
+    # per cell and TF kernel: kernel, bias, column blocks, bias initialiser value, recurrent block, first block in Wx / b
+    cells = {'lstm': [('lstm_cell/kernel', 'lstm_cell/bias', 4, 0.0, 'Wh', 0)],
+             'gru': [('gru_cell/gates/kernel', 'gru_cell/gates/bias', 2, 1.0, 'Wh', 0),
+                     ('gru_cell/candidate/kernel', 'gru_cell/candidate/bias', 1, 0.0, 'Whc', 2)]}
+    for cell, kernels in cells.items():
+        pb = make_problem('tiny', profile='B', rnn_cell=cell, rnn_units=255, rnn_num_layers=2)
+        lay = pb.layout
+        H, Hp, C = 255, 256, lay.C
+        assert lay.Hp == Hp
+        G = sum(n for _, _, n, _, _, _ in kernels)
+        rs = np.random.RandomState(3)
+        lg = {k: rs.randn(*v.shape).astype(np.float32) for k, v in lay.init_logical(1).items()}
+        back = lay.to_logical(lay.to_internal(lg))
+        assert sorted(back) == sorted(lg)
+        for k in lg:
+            assert np.array_equal(back[k], lg[k]), (cell, k)
+        flat = lay.to_internal(lg)
+        for i, n_in, n_in_p in ((0, C, C), (1, H, Hp)):
+            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/'.format(i)
+            want = {'Wx': np.zeros((n_in_p, G * Hp), np.float32), 'b': np.zeros((1, G * Hp), np.float32)}
+            for kname, bname, n, _, wh, g0 in kernels:
+                k, b = lg[base + kname], lg[base + bname]
+                assert k.shape == (n_in + H, n * H) and b.shape == (n * H,)
+                want[wh] = np.zeros((Hp, n * Hp), np.float32)
+                for g in range(n):
+                    col = (g0 + g) * Hp
+                    want['Wx'][:n_in, col:col + H] = k[:n_in, g * H:(g + 1) * H]
+                    want['b'][0, col:col + H] = b[g * H:(g + 1) * H]
+                    want[wh][:H, g * Hp:g * Hp + H] = k[n_in:, g * H:(g + 1) * H]
+            for key, m in want.items():
+                t = lay.by_key['rnn%d/%s' % (i, key)]
+                assert (t.rows, t.ld) == m.shape and not t.reg, (cell, i, key)       # not L2-regularised
+                assert np.array_equal(flat[t.offset:t.offset + t.size].reshape(m.shape), m), (cell, i, key)
+        # bias initialisers: LSTM zeros (forget_bias 1.0 is a constant of the cell); GRU gates ones, candidate zeros
+        init = lay.init_logical(42)
+        for _, bname, n, value, _, _ in kernels:
+            assert np.array_equal(init['main/RNN/rnn/multi_rnn_cell/cell_0/' + bname], np.full(n * H, value, np.float32))
