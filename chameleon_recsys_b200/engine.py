@@ -29,6 +29,27 @@ from .plan import (SEG_ACR, SEG_CTX_EMBED, SEG_ITEM_EMB, SEG_META_EMBED, Feature
 _NP2T = {np.int64: torch.int64, np.float32: torch.float32, np.int32: torch.int32}
 
 
+def set_plan_columns(p: FeaturePlanC, pl: FeaturePlan):
+    """Write the column part of the C plan ``p`` from ``pl``: the column -> segment map and the column ranges outside the
+    wide (vector-copied) segments."""
+    if pl.Fp > len(p.col_seg):
+        raise NarError('feature rows wider than NAR_MAX_COLS')
+    cs = np.full(len(p.col_seg), 255, dtype=np.uint8)
+    wide = np.zeros(pl.Fp, dtype=bool)
+    for i, s in enumerate(pl.segments):
+        cs[s.int_col:s.int_col + s.width] = i
+        if s.kind in (SEG_ACR, SEG_ITEM_EMB):
+            wide[s.int_col:s.int_col + s.width] = True
+    C.memmove(p.col_seg, cs.ctypes.data, len(p.col_seg))
+    edges = np.flatnonzero(np.diff(np.concatenate([[True], wide, [True]]).astype(np.int8)))
+    ranges = list(zip(edges[0::2], edges[1::2]))
+    if len(ranges) > 4:
+        raise NarError('more than 4 narrow column ranges')
+    p.n_narrow = len(ranges)
+    for i, (a, b) in enumerate(ranges):
+        p.narrow_begin[i], p.narrow_end[i] = int(a), int(b)
+
+
 class NarEngine:
     def __init__(self, plan: FeaturePlan, layout: ParamLayout, content_article_embeddings_matrix: np.ndarray,
                  articles_metadata: Dict[str, np.ndarray], *, negative_samples: int, negative_sample_from_buffer: int,
@@ -409,23 +430,7 @@ class NarEngine:
         p.gamma = self.view('gamma').data_ptr()
         p.beta = self.view('beta').data_ptr()
         p.log_base_recency, p.log_base_novelty = self.lb_rec, self.lb_nov
-        # column -> segment map and the column ranges outside the wide (vector-copied) segments
-        if pl.Fp > len(p.col_seg):
-            raise NarError('feature rows wider than NAR_MAX_COLS')
-        cs = np.full(len(p.col_seg), 255, dtype=np.uint8)
-        wide = np.zeros(pl.Fp, dtype=bool)
-        for i, s in enumerate(pl.segments):
-            cs[s.int_col:s.int_col + s.width] = i
-            if s.kind in (SEG_ACR, SEG_ITEM_EMB):
-                wide[s.int_col:s.int_col + s.width] = True
-        C.memmove(p.col_seg, cs.ctypes.data, len(p.col_seg))
-        edges = np.flatnonzero(np.diff(np.concatenate([[True], wide, [True]]).astype(np.int8)))
-        ranges = list(zip(edges[0::2], edges[1::2]))
-        if len(ranges) > 4:
-            raise NarError('more than 4 narrow column ranges')
-        p.n_narrow = len(ranges)
-        for i, (a, b) in enumerate(ranges):
-            p.narrow_begin[i], p.narrow_end[i] = int(a), int(b)
+        set_plan_columns(p, pl)
         return p
 
     def feature_plan_c(self, st: dict) -> FeaturePlanC:

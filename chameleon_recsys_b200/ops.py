@@ -154,6 +154,13 @@ def build_rows(pos_idx, L, item_clicked, label_next, negatives, K, row_pos, row_
                                      _p(row_item), _stream()), 'nar_build_rows')
 
 
+def build_base_rows(pos_idx, L, item_clicked, label_next, unique_items, n_unique, U, neg_uidx, K, base_pos, base_item):
+    global LAUNCHES
+    LAUNCHES += 1
+    check(_lib.load().nar_build_base_rows(_p(pos_idx), L, _p(item_clicked), _p(label_next), _p(unique_items), _p(n_unique), U,
+                                          _p(neg_uidx), K, _p(base_pos), _p(base_item), _stream()), 'nar_build_base_rows')
+
+
 def feature_stats(buffer, n_norm, created_at_ts, pop_norm, max_ts, log_base_rec, log_base_nov, row_pos, row_item,
                   n_rows, n_input, n_cand, event_ts, stats):
     global LAUNCHES
