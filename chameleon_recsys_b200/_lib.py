@@ -110,6 +110,7 @@ _SIGNATURES = {
     'nar_sample_negatives_uidx': (C.c_int, [vp, vp, i64, i64, i64, i64, vp, i64, i64, i64, u64, u32, vp, vp,
                                             C.POINTER(vp), C.POINTER(vp), vp, i64, vp]),
     'nar_car_combine': (C.c_int, [vp, vp, vp, vp, vp, i64, i64, i64, C.c_int, vp, vp]),
+    'nar_car_combine_t': (C.c_int, [vp, vp, vp, vp, vp, i64, i64, i64, C.c_int, vp, i64, vp]),
     'nar_engine_create': (C.c_int, [vp, C.POINTER(ModelCfg), C.POINTER(vp)]),
     'nar_engine_destroy': (C.c_int, [vp]),
     'nar_engine_update_cfg': (C.c_int, [vp, C.POINTER(ModelCfg)]),
@@ -126,6 +127,8 @@ _SIGNATURES = {
     'nar_scatter_add_rows_f32': (C.c_int, [vp, i64, i64, C.c_int, vp, i64, vp, i64, vp]),
     'nar_gemm_tf32': (C.c_int, [vp, i64, i64, i64, vp, i64, C.c_int, vp, i64, C.c_int, vp, i64,
                                 C.POINTER(GemmEpilogue), vp]),
+    'nar_gemm_tf32_dt': (C.c_int, [vp, i64, i64, i64, vp, i64, C.c_int, vp, i64, C.c_int, vp, i64,
+                                   C.POINTER(GemmEpilogue), vp]),
     'nar_pack_bf16x3': (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, vp, vp]),
     'nar_ugrnn_fwd': (C.c_int, [vp, vp, vp, vp, i64, i64, vp, vp, vp, vp]),
     'nar_ugrnn_bwd': (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]),

@@ -10,7 +10,9 @@
 //   full mode      X [R, Fp] feature rows in the same order (every candidate row gathered and multiplied by W1)
 //   dedup mode     XB [2L+U, Fp] base rows: L clicked, L positives, U unique-negative ITEM rows (csrc/car.cu):
 //                  PP = XB[L:2L] W1 + b1 ; PI = XB[2L:, item cols] W1[item rows] ; PC = XB[:L, ctx cols] W1[ctx rows] + b1
-//                  H1[L + l*n_cand + j] = leaky(j == 0 ? PP[l] : PC[l] + PI[u(l, j-1)])
+//                  H1[L + l*n_cand + j] = leaky(j == 0 ? PP[l] : PC[l] + PI[u(l, j-1)]), stored transposed:
+//                  H1cT [C, ldr] behind the L_cap clicked rows of H1, so that layer 2's weight gradient reads both
+//                  operands in the major the tensor cores take (the forward reads it MN-major)
 //                  backward: DB = [dH1(in) | dPP | dPI | dPC], the last three formed in the candidate rows' layer-2
 //                  dgrad epilogue (no dH1 of the candidate rows), then ONE wgrad / dgrad over the 2L+U base rows (+ the
 //                  context block), instead of two GEMMs over all R rows.
@@ -59,6 +61,7 @@ struct StepBufs {
   // per cell: GT = UGRNN gate / GRU r (LSTM: none); CD = UGRNN and GRU candidate / LSTM cell state; UO = GRU u;
   // RH = GRU r * previous state.  The LSTM's activated gates replace its pre-activations in GX.
   float *PP, *PI, *PC, *DB;        // dedup: layer-1 pre-activations and their gradients
+  float* H1cT; int64_t ldr;        // dedup: the candidate rows of H1 transposed, [C, ldr], ldr >= L_cap * n_cand
 };
 
 }  // namespace
@@ -141,7 +144,14 @@ int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, St
   memset(sb, 0, sizeof(*sb));
   Carver cv(base);
   if (c.dedup) { sb->X = cv.take<float>(NB * Fp); } else { sb->X = cv.take<float>(R * Fp); }
-  sb->H1 = cv.take<float>(R * C);
+  if (c.dedup) {
+    // column segments of 32 rows start 128-byte aligned; H1 keeps >= R * C floats
+    sb->ldr = align_up(Rc, 32);
+    sb->H1 = cv.take<float>(L_cap * C + C * sb->ldr);
+    sb->H1cT = sb->H1 + L_cap * C;
+  } else {
+    sb->H1 = cv.take<float>(R * C);
+  }
   sb->E = cv.take<float>(R * C);
   session_carve(c, L_cap, cv, sb);
   sb->logits = cv.take<float>(L_cap * n_cand);
@@ -204,9 +214,11 @@ struct Seq {
   float* G(int64_t off) const { return c.grads + off; }
 
   // Y[M,N] = act(X[M,Kd] * W[Kd,N] + b)      (W stored [in,out]: MN-major B operand, or its bf16x3 plane)
-  // (a_scale: X's row i scaled by a_scale[i / group] as it is loaded, see fused_product)
+  // (a_scale: X's row i scaled by a_scale[i / group] as it is loaded, see fused_product; x_kmajor = 0: X is stored
+  // transposed, [Kd, ldx])
   void fwd(const float* X, int64_t ldx, int64_t off_W, int64_t ldw, int64_t off_b, float* Y, int64_t ldy, int64_t M, int64_t N,
-           int64_t Kd, int act, cudaStream_t st, const float* a_scale = nullptr, int64_t ld_scale = 0, int64_t group = 0) {
+           int64_t Kd, int act, cudaStream_t st, const float* a_scale = nullptr, int64_t ld_scale = 0, int64_t group = 0,
+           int x_kmajor = 1) {
     nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
     ep.a_scale = a_scale; ep.ld_a_scale = ld_scale; ep.a_scale_group = group;
     ep.bias = off_b >= 0 ? W(off_b) : nullptr; ep.act = act; ep.split_k = 1; ep.precision = c.fwd_precision;
@@ -218,7 +230,7 @@ struct Seq {
       if (i == ps.n) { if (!rc) rc = NAR_ERR_INVALID; return; }   // planes_build registers every forward block: a miss is a bug
       ep.b_bf16 = ps.buf + ps.dst[i]; ep.ld_bf16 = ps.ld_out[i];
     }
-    chk(nar_gemm_tf32(e->ctx, M, N, Kd, X, ldx, 1, W(off_W), ldw, 0, Y, ldy, &ep, st));
+    chk(nar_gemm_tf32(e->ctx, M, N, Kd, X, ldx, x_kmajor, W(off_W), ldw, 0, Y, ldy, &ep, st));
   }
   // dX[M,n_in] (+)= dY[M,n_out] * W^T, optionally times act'(aux)
   void dgrad(const float* dY, int64_t lddy, int64_t off_W, int64_t ldw, float* dX, int64_t lddx, int64_t M, int64_t n_in,
@@ -236,6 +248,14 @@ struct Seq {
     ep.a_scale = a_scale; ep.ld_a_scale = ld_scale; ep.a_scale_group = group;
     ep.accumulate = 1; ep.split_k = 0; ep.precision = c.bwd_precision;
     chk(nar_gemm_tf32(e->ctx, n_in, n_out, rows, X, ldx, 0, dY, lddy, 0, G(off_W), ldw, &ep, st));
+  }
+  // the same from X stored transposed (XT [n_in, ldxt]), as dW^T = dY^T * X: A = dY MN-major, B = XT K-major, so that
+  // neither operand is transposed in shared memory; the epilogue adds the tile transposed into dW [in, out]
+  void wgrad_xt(const float* XT, int64_t ldxt, const float* dY, int64_t lddy, int64_t off_W, int64_t ldw, int64_t n_in,
+                int64_t n_out, int64_t rows, cudaStream_t st) {
+    nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
+    ep.accumulate = 1; ep.split_k = 0; ep.precision = c.bwd_precision;
+    chk(nar_gemm_tf32_dt(e->ctx, n_out, n_in, rows, dY, lddy, 0, XT, ldxt, 1, G(off_W), ldw, &ep, st));
   }
   // through the scorer product and the CAR tanh: v = dY W^T; dX[r] = v[r] * pred[r / group] * tanh'(cand[r]) and
   // dpred[l] = sum over position l's rows of v * cand (nar_mul_pred_bwd's arithmetic)
@@ -340,11 +360,12 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
     s.fwd(sb.X + L * Fp, Fp, c.off_W1, C, c.off_b1, sb.PP, C, L, C, Fp, NAR_ACT_NONE, main);                       // positives: full rows
     s.fwd(sb.X + 2 * L * Fp, Fp, c.off_W1, C, -1, sb.PI, C, U, C, c0, NAR_ACT_NONE, main);                          // item half, once per unique id
     s.fwd(sb.X + c0, Fp, c.off_W1 + c0 * C, C, c.off_b1, sb.PC, C, L, C, Fp - c0, NAR_ACT_NONE, main);             // context half, once per position
-    s.chk(nar_car_combine(sb.PP, sb.PC, sb.PI, io->pos_idx, pb.neg_uidx, L, K, C, NAR_ACT_LEAKY_RELU, H1c, main));
+    s.chk(nar_car_combine_t(sb.PP, sb.PC, sb.PI, io->pos_idx, pb.neg_uidx, L, K, C, NAR_ACT_LEAKY_RELU, sb.H1cT, sb.ldr, main));
+    s.fwd(sb.H1cT, sb.ldr, c.off_W2, C, c.off_b2, Ec, C, Rc, C, C, NAR_ACT_TANH, main, nullptr, 0, 0, 0);
   } else {
     s.fwd(sb.X + L * Fp, Fp, c.off_W1, C, c.off_b1, H1c, C, Rc, C, Fp, NAR_ACT_LEAKY_RELU, main);
+    s.fwd(H1c, C, c.off_W2, C, c.off_b2, Ec, C, Rc, C, C, NAR_ACT_TANH, main);
   }
-  s.fwd(H1c, C, c.off_W2, C, c.off_b2, Ec, C, Rc, C, C, NAR_ACT_TANH, main);
   s.join();
 
   // ---- scorer + loss (nar_model.py:444-517, :639-667), optional novelty regulariser (:673-683)
@@ -402,7 +423,12 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   //   C  candidates: CAR layer-2 dgrad over the L*(1+K) candidate rows - the big GEMM (+ the CAR layer-1 sums)
   // then the clicked rows' CAR backward, which needs S's dE.  The candidate rows' layer-2 weight gradient needs only dEc:
   // queued on the auxiliary stream before S, the longest kernel of that stream starts as soon as dEc exists.
-  { cudaStream_t st = s.fork(); s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st); s.bgrad(dEc, C, Rc, C, c.off_b2, st); }
+  {
+    cudaStream_t st = s.fork();
+    if (c.dedup) s.wgrad_xt(sb.H1cT, sb.ldr, dEc, C, c.off_W2, C, C, C, Rc, st);
+    else s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st);
+    s.bgrad(dEc, C, Rc, C, c.off_b2, st);
+  }
   // ---- S
   {
     s.chk(nar_act_bwd(sb.dPR, sb.PR, L * C, NAR_ACT_TANH, sb.dPR, main));
@@ -805,7 +831,7 @@ extern "C" int nar_engine_buffer(const nar_engine* e, const nar_step_io* io, con
       {"neg", pb.neg, io->Bg * io->T, K}, {"neg_uidx", pb.neg_uidx, io->Bg * io->T, K}, {"stats", pb.stats, 1, 24},
       {"row_pos", pb.row_pos, R, 1}, {"row_item", pb.row_item, R, 1}, {"base_pos", pb.base_pos, NB, 1},
       {"base_item", pb.base_item, NB, 1},
-      {"X", sb.X, c.dedup ? NB : R, c.Fp}, {"dX", sb.dX, c.dedup ? NB : R, c.Fp}, {"H1", sb.H1, R, c.C}, {"E", sb.E, R, c.C},
+      {"X", sb.X, c.dedup ? NB : R, c.Fp}, {"dX", sb.dX, c.dedup ? NB : R, c.Fp}, {"H1", sb.H1, R, c.C}, {"H1cT", sb.H1cT, c.C, sb.ldr}, {"E", sb.E, R, c.C},
       {"dE", sb.dE, R, c.C}, {"dH1", sb.dH1, R, c.C}, {"F1", sb.F1, L, 512}, {"PR", sb.PR, L, c.C},
       {"logits", sb.logits, L, n_cand}, {"PD", sb.PD, Rc, c.C}, {"Z1", sb.Z1, Rc, 128}, {"Z2", sb.Z2, Rc, 64}, {"Z3", sb.Z3, Rc, 32}, {"PP", sb.PP, L, c.C},
       {"PI", sb.PI, pb.U, c.C}, {"PC", sb.PC, L, c.C}, {"DB", sb.DB, 3 * L + pb.U, c.C},

@@ -57,7 +57,9 @@ constexpr int EPI_LD = BN + 4;               // floats per staged accumulator ro
 //   EXT_PROD_BWD    scorer-product backward epilogue (nar_gemm_epilogue.pred): position-aligned M tiles
 //   EXT_CAR_BWD     CAR layer-1 backward epilogue (nar_gemm_epilogue.car_*): the gradients of PP / PC / PI, no D
 //                   (TF32 or 3xTF32 with B split in-kernel, K-major operands)
-constexpr int EXT_SCALE_SMEM = 1, EXT_SCALE_GMEM = 2, EXT_PROD_BWD = 3, EXT_CAR_BWD = 4;
+//   EXT_TRANS_D     D written transposed, D[n * ldd + m] (nar_gemm_tf32_dt): a weight gradient computed as
+//                   dW^T = dY^T * X, A = dY MN-major and B = X^T K-major, lands in dW [in, out] with no prep pass on B
+constexpr int EXT_SCALE_SMEM = 1, EXT_SCALE_GMEM = 2, EXT_PROD_BWD = 3, EXT_CAR_BWD = 4, EXT_TRANS_D = 5;
 constexpr int SC_ROWS_K = 32, SC_ROWS_MN = 8;
 constexpr int SC_BYTES = 4096;
 static_assert(SC_ROWS_K * BK * 4 == SC_BYTES && SC_ROWS_MN * BM * 4 == SC_BYTES, "a_scale slice per stage");
@@ -476,11 +478,12 @@ __global__ void __launch_bounds__(NUM_THREADS, (Cfg<MODE, B_MN>::CTAS_PER_SM))
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_x, const Params p) {
   constexpr bool SC_SMEM = EXT == EXT_SCALE_SMEM, SC_GMEM = EXT == EXT_SCALE_GMEM, SCALE = SC_SMEM || SC_GMEM;
-  constexpr bool PROD_BWD = EXT == EXT_PROD_BWD, CAR_BWD = EXT == EXT_CAR_BWD;
+  constexpr bool PROD_BWD = EXT == EXT_PROD_BWD, CAR_BWD = EXT == EXT_CAR_BWD, TRANS_D = EXT == EXT_TRANS_D;
   using C = Cfg<MODE, B_MN, SC_SMEM ? SC_BYTES : 0>;
   constexpr bool BF16 = MODE == 4;
-  static_assert(!BF16 || (!A_MN && !B_MN), "bf16x3: A K-major fp32, B the transposed (K-major) bf16 plane");
-  static_assert(!SCALE || BF16 || (MODE == 0 && A_MN && B_MN), "A scale: bf16x3, or single-pass TF32 weight gradient");
+  static_assert(!BF16 || !B_MN, "bf16x3: A fp32 of either major, B the transposed (K-major) bf16 plane");
+  static_assert(!SCALE || (BF16 && !A_MN) || (MODE == 0 && A_MN && B_MN), "A scale: bf16x3 (K-major A), or single-pass TF32 weight gradient");
+  static_assert(!TRANS_D || ((MODE == 0 || MODE == 1) && A_MN && !B_MN), "transposed D: TF32 / 3xTF32, A MN-major, B K-major");
   static_assert(!PROD_BWD || (MODE == 0 && !A_MN && !B_MN), "product backward: single-pass TF32, K-major operands");
   static_assert(!CAR_BWD || ((MODE == 0 || MODE == 1) && !A_MN && !B_MN), "CAR backward: TF32 / 3xTF32, K-major operands");
   static_assert(!CAR_BWD || C::STAGES * C::STAGE_BYTES >= (BM * EPI_LD + 2 * BM) * 4, "CAR backward: row slots behind the staged rows");
@@ -545,10 +548,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   uint32_t a[2][4][4], alo[2][4][4];      // tf32: hi (or the single-pass value) | lo (3xTF32)
   uint32_t ahi16[2][2][4], alo16[2][2][4];  // bf16x3: A_hi | A_lo pairs
   // tf32 A fragment q of k-step j is at a_off[q] + 1024 j (MN-major: 8 k-rows on) or a_off[q] ^ 32 j (K-major: the
-  // 16-byte chunk index (2 j + q / 2) ^ (row & 7) is chunk (q / 2) ^ (row & 7) with 2 j XORed in)
+  // 16-byte chunk index (2 j + q / 2) ^ (row & 7) is chunk (q / 2) ^ (row & 7) with 2 j XORed in).  bf16x3 with an
+  // MN-major A: a_off[2 h + e] is element (r0 + 8 h, 2 t + e), and k + 8 i has the same k & 7, so element
+  // (r0 + 8 h, 2 t + e + 8 i) is 1024 i bytes on
   uint32_t a_off[4];
 #pragma unroll
-  for (int q = 0; q < 4; ++q) a_off[q] = tile_off<A_MN>(r0 + (q & 1) * 8, t + (q >> 1) * 4);
+  for (int q = 0; q < 4; ++q)
+    a_off[q] = BF16 ? tile_off<true>(r0 + (q >> 1) * 8, 2 * t + (q & 1)) : tile_off<A_MN>(r0 + (q & 1) * 8, t + (q >> 1) * 4);
   const uint32_t sc0 = smem_u32(smem + C::SC_OFF);           // a_scale slice of stage 0 (shared address)
 
   // One k-tile; BUF = kt & 1 is a compile-time constant (the loop below is unrolled by two) so that the fragments stay
@@ -589,7 +595,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const int r = r0 + (q & 1) * 8, k = 16 * j + 2 * t + (q >> 1) * 8;
-          float2 x = *reinterpret_cast<const float2*>(sa + tile_off<false>(r, k));
+          // MN-major A: the pair (k, k + 1) is two 32-bit loads from adjacent k-rows.  Each load is free of bank
+          // conflicts: k * 128 B is whole bank rows, so the bank is 4 ((r >> 2) & 7 ^ k & 7) + (r & 3).  Over a warp
+          // (r = 16 w + g (+ 8), g = 0..7; k & 7 = 2 t (+ 1), t = 0..3) the chunk (r >> 2 & 7) ^ (k & 7) takes 8 distinct
+          // values - bit 0 from g >> 2, bits 1-2 from t - and r & 3 = g & 3 picks the word: 32 lanes, 32 banks.
+          float2 x;
+          if (A_MN) {
+            const uint32_t kk = (16 * j + (q >> 1) * 8) * 128;
+            x.x = *reinterpret_cast<const float*>(sa + a_off[(q & 1) * 2] + kk);
+            x.y = *reinterpret_cast<const float*>(sa + a_off[(q & 1) * 2 + 1] + kk);
+          } else {
+            x = *reinterpret_cast<const float2*>(sa + tile_off<false>(r, k));
+          }
           if (SC_SMEM) {        // __fmul_rn: the product is rounded on its own, never contracted into the split
             const float2 f = ld_shared_f2(sc_r[q & 1] + (16 * j + (q >> 1) * 8) * 4);
             x.x = __fmul_rn(x.x, f.x); x.y = __fmul_rn(x.y, f.y);
@@ -679,8 +696,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int c = 8 * j + 2 * t;
-    *reinterpret_cast<float2*>(stage + r0 * EPI_LD + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-    *reinterpret_cast<float2*>(stage + (r0 + 8) * EPI_LD + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    if (TRANS_D) {   // stage row = tile column: 4 (2 t + i) + g + const over a warp, 32 banks per scalar store
+      stage[c * EPI_LD + r0] = acc[4 * j]; stage[(c + 1) * EPI_LD + r0] = acc[4 * j + 1];
+      stage[c * EPI_LD + r0 + 8] = acc[4 * j + 2]; stage[(c + 1) * EPI_LD + r0 + 8] = acc[4 * j + 3];
+    } else {
+      *reinterpret_cast<float2*>(stage + r0 * EPI_LD + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(stage + (r0 + 8) * EPI_LD + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
   }
   __syncthreads();
   if (PROD_BWD) {
@@ -689,6 +711,27 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
   if (CAR_BWD) {
     car_bwd_epilogue(p, stage, s_l, s_u, m0, n_blk, tid);
+    return;
+  }
+  if (TRANS_D) {                      // D row = tile column n, D columns = tile rows m: 128 contiguous bytes per warp
+    const int64_t col = (int64_t)m0 + lane * 4;
+    if (col >= p.M) return;
+    for (int it = 0; it < BN / 8; ++it) {
+      const int nl = it * 8 + warp;
+      const int64_t row = (int64_t)n_blk * BN + nl;
+      if (row >= p.N) break;
+      const float4 v = *reinterpret_cast<const float4*>(stage + nl * EPI_LD + lane * 4);
+      float* d = p.D + row * p.ldd + col;
+      if (col + 4 <= p.M) {
+        if (p.accumulate) atomicAdd(reinterpret_cast<float4*>(d), v);      // red.global.add.v4.f32
+        else *reinterpret_cast<float4*>(d) = v;
+      } else {
+        const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+          if (col + j < p.M) { if (p.accumulate) atomicAdd(d + j, e[j]); else d[j] = e[j]; }
+      }
+    }
     return;
   }
   const int c4 = lane * 4;
@@ -831,10 +874,12 @@ extern "C" int nar_pack_bf16x3(const float* const* W, void* const* out, const in
   return NAR_OK;
 }
 
-extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda, int a_kmajor,
-                             const float* B, int64_t ldb, int b_kmajor, float* D, int64_t ldd,
-                             const nar_gemm_epilogue* epi, void* stream) {
-  using namespace nar::gemm;
+namespace nar {
+namespace gemm {
+
+// nar_gemm_tf32, and with trans_d D written transposed (nar_gemm_tf32_dt)
+static int gemm(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda, int a_kmajor, const float* B,
+                int64_t ldb, int b_kmajor, float* D, int64_t ldd, const nar_gemm_epilogue* epi, void* stream, bool trans_d) {
   if (!ctx || !ctx->encode_tiled) return NAR_ERR_NO_DEVICE;
   if (!A || !epi || (!B && epi->precision != 4)) return NAR_ERR_INVALID;
   const bool car_bwd = epi->car_pp != nullptr;       // writes the CAR layer-1 gradients instead of D
@@ -845,14 +890,17 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   if (epi->dact && !car_bwd && (!epi->aux || (epi->ld_aux & 3) != 0 || (reinterpret_cast<uintptr_t>(epi->aux) & 15u) != 0)) return NAR_ERR_INVALID;
   if (epi->precision != 1 && epi->precision != 3 && epi->precision != 4) return NAR_ERR_INVALID;
   const bool bf16 = epi->precision == 4;
-  if (bf16 && (!a_kmajor || !epi->b_bf16 || epi->accumulate || epi->split_k > 1)) return NAR_ERR_INVALID;
+  if (bf16 && (!epi->b_bf16 || epi->accumulate || epi->split_k > 1)) return NAR_ERR_INVALID;
   const bool blo = epi->precision == 3 && epi->b_lo != nullptr;
   const int mode = bf16 ? 4 : (epi->precision == 1 ? 0 : (blo ? 2 : 1));
   const bool scale = epi->a_scale != nullptr, prod_bwd = epi->pred != nullptr;
   const int64_t a_rows = a_kmajor ? M : K, a_cols = a_kmajor ? K : M;       // A's storage
+  // transposed D: TF32 / 3xTF32 splitting B in-kernel, A MN-major, B K-major, a plain (or accumulated) product
+  if (trans_d && ((mode != 0 && mode != 1) || a_kmajor || !b_kmajor || epi->bias || epi->act || epi->dact || epi->aux || scale ||
+                  prod_bwd || car_bwd)) return NAR_ERR_INVALID;
   if (scale) {
     // implemented: bf16x3 (K-major A), and single-pass TF32 with both operands MN-major (the weight gradient)
-    if (!(mode == 4 || (mode == 0 && !a_kmajor && !b_kmajor)) || prod_bwd) return NAR_ERR_INVALID;
+    if (!((mode == 4 && a_kmajor) || (mode == 0 && !a_kmajor && !b_kmajor)) || prod_bwd) return NAR_ERR_INVALID;
     if (epi->a_scale_group < 1 || a_rows > 0x7fffffffLL || a_cols > 0x7fffffffLL || epi->a_scale_group > a_rows ||
         epi->ld_a_scale < a_cols || (epi->ld_a_scale & 3) != 0 ||
         (reinterpret_cast<uintptr_t>(epi->a_scale) & 15u) != 0) return NAR_ERR_INVALID;
@@ -942,7 +990,11 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
     if (mode == 0) return launch<false, false, 0, EXT_CAR_BWD>(ta, tb, tbl, p, grid, st);
     return launch<false, false, 1, EXT_CAR_BWD>(ta, tb, tbl, p, grid, st);
   }
-  if (mode == 4) return launch<false, false, 4>(ta, tb, tbl, p, grid, st);
+  if (trans_d) {
+    if (mode == 0) return launch<true, false, 0, EXT_TRANS_D>(ta, tb, tbl, p, grid, st);
+    return launch<true, false, 1, EXT_TRANS_D>(ta, tb, tbl, p, grid, st);
+  }
+  if (mode == 4) return amn ? launch<true, false, 4>(ta, tb, tbl, p, grid, st) : launch<false, false, 4>(ta, tb, tbl, p, grid, st);
 #define NAR_GEMM_CASE(a, b) \
   if (amn == a && bmn == b) { \
     if (mode == 0) return launch<a, b, 0>(ta, tb, tbl, p, grid, st); \
@@ -952,4 +1004,19 @@ extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, cons
   NAR_GEMM_CASE(false, false) NAR_GEMM_CASE(false, true) NAR_GEMM_CASE(true, false) NAR_GEMM_CASE(true, true)
 #undef NAR_GEMM_CASE
   return NAR_ERR_INVALID;
+}
+
+}  // namespace gemm
+}  // namespace nar
+
+extern "C" int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda, int a_kmajor,
+                             const float* B, int64_t ldb, int b_kmajor, float* D, int64_t ldd,
+                             const nar_gemm_epilogue* epi, void* stream) {
+  return nar::gemm::gemm(ctx, M, N, K, A, lda, a_kmajor, B, ldb, b_kmajor, D, ldd, epi, stream, false);
+}
+
+extern "C" int nar_gemm_tf32_dt(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, int64_t lda, int a_kmajor,
+                                const float* B, int64_t ldb, int b_kmajor, float* D, int64_t ldd,
+                                const nar_gemm_epilogue* epi, void* stream) {
+  return nar::gemm::gemm(ctx, M, N, K, A, lda, a_kmajor, B, ldb, b_kmajor, D, ldd, epi, stream, true);
 }

@@ -550,7 +550,10 @@ class NarEngine:
         n_cand = K + 1
         b = lambda n: self.buffer(st, n)      # noqa: E731
         X = b('X')
+        H1 = b('H1')
         if self.dedup:
+            # the candidate rows of H1 are stored transposed (H1cT [C, ldr]) behind the clicked rows
+            H1 = torch.cat([H1[:L], b('H1cT')[:, :L * n_cand].t()], dim=0)
             c0 = self.plan.ctx_col0
             pos = st['t']['pos_idx'][:L].long()
             uidx = b('neg_uidx')[pos].long()                                  # [L, K]
@@ -560,7 +563,7 @@ class NarEngine:
         # with dropout the RNN OUTPUT the reference exposes is the dropped one (DropoutWrapper); the state is HO<i>
         ho = 'HOd%d' if (self.keep_prob < 1.0 and train) else 'HO%d'
         extra = {n: b(n) for n in ('Z1', 'Z2', 'Z3')} if self.ranking == 'mlp' else {}
-        return dict(X=X.clone(), H1=b('H1'), E=b('E'), **extra, HO=[b(ho % i) for i in range(self.layers)], F1=b('F1'), PR=b('PR'),
+        return dict(X=X.clone(), H1=H1, E=b('E'), **extra, HO=[b(ho % i) for i in range(self.layers)], F1=b('F1'), PR=b('PR'),
                     logits=b('logits'), row_pos=b('row_pos').view(-1), row_item=b('row_item').view(-1),
                     stats=b('stats').view(-1).clone(),
                     neg=b('neg').view(-1)[st['s0'] * T * K:(st['s0'] + st['B']) * T * K].view(st['B'], T, K))

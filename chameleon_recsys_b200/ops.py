@@ -64,12 +64,12 @@ def _chk_f32(*ts):
 def gemm(A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N: int, K: int, *, a_kmajor=True, b_kmajor=True,
          lda=None, ldb=None, ldd=None, bias=None, act=ACT_NONE, dact=ACT_NONE, aux=None, ld_aux=None,
          accumulate=False, split_k=1, precision=3, b_lo=None, b_bf16=None, ld_bf16=0, a_scale=None, a_scale_group=0,
-         pred=None, d_pred=None, pred_group=0, car=None):
+         pred=None, d_pred=None, pred_group=0, car=None, trans_d=False):
     global LAUNCHES
     LAUNCHES += 1
     """D[M,N] = epilogue(sum_k A(m,k) B(n,k)); see nar_gemm_tf32.  a_scale / pred / d_pred: row strides from the tensors.
     car: dict(pp, pc, pi, pos_idx, neg_uidx, dpp, dpc, dpi, k) for the CAR layer-1 backward epilogue (D = None; ld_car from
-    pp)."""
+    pp).  trans_d: D stored transposed, D[n*ldd + m] (nar_gemm_tf32_dt)."""
     _chk_f32(A, B, D, bias, aux, a_scale, pred, d_pred)
     lda = A.stride(0) if lda is None else lda
     ldb = (B.stride(0) if B is not None else 0) if ldb is None else ldb
@@ -85,8 +85,9 @@ def gemm(A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N: int, K: i
             setattr(epi, 'car_' + f, _p(car[f]))
         epi.ld_car, epi.car_k = car['pp'].stride(0), int(car['k'])
     ctx = context()
-    check(ctx.lib.nar_gemm_tf32(ctx.handle, M, N, K, _p(A), lda, 1 if a_kmajor else 0, _p(B), ldb, 1 if b_kmajor else 0,
-                                _p(D), ldd, C.byref(epi), _stream()), 'nar_gemm_tf32')
+    fn = 'nar_gemm_tf32_dt' if trans_d else 'nar_gemm_tf32'
+    check(getattr(ctx.lib, fn)(ctx.handle, M, N, K, _p(A), lda, 1 if a_kmajor else 0, _p(B), ldb, 1 if b_kmajor else 0,
+                               _p(D), ldd, C.byref(epi), _stream()), fn)
 
 
 _PACK_SCRATCH: dict = {}

@@ -171,8 +171,8 @@ typedef struct {
   int32_t precision;      /* 1 = TF32, 3 = 3xTF32 (error-compensated, ~fp32 accuracy) */
   const float* b_lo;      /* precision 3 only, optional: x - tf32_trunc(x) of operand B, same shape / ld as B (see
                              nar_tf32_lo; the weights' lo plane is maintained by nar_adam_tf).  NULL: split B in-kernel */
-  const void* b_bf16;     /* precision 4 (bf16x3: bf16 hi + lo pieces on the bf16 tensor path, fp32 accumulate; A must be K-major
-                             fp32): operand B as the pre-split transposed plane written by nar_pack_bf16x3 - [N, ld_bf16]
+  const void* b_bf16;     /* precision 4 (bf16x3: bf16 hi + lo pieces on the bf16 tensor path, fp32 accumulate; A fp32 of
+                             either major): operand B as the pre-split transposed plane written by nar_pack_bf16x3 - [N, ld_bf16]
                              bf16, row n = per block of 32 k the 32 hi values then the 32 lo values; B / ldb are ignored */
   int64_t ld_bf16;        /* elements per row of b_bf16 (>= ceil(K/32)*64, multiple of 8) */
   const float* a_scale;   /* optional A scale, defined on A's storage: the stored element A[i*lda + j] enters the MMA as
@@ -218,6 +218,14 @@ int nar_gemm_tf32(nar_ctx* ctx, int64_t M, int64_t N, int64_t K,
                   const float* A, int64_t lda, int a_kmajor,
                   const float* B, int64_t ldb, int b_kmajor,
                   float* D, int64_t ldd, const nar_gemm_epilogue* epi /*host*/, void* stream);
+/* the same product with D stored transposed: D[n*ldd + m].  For a weight gradient dW [in, out] += X^T dY computed as
+ * dW^T = dY^T X: A = dY MN-major, B = X^T K-major (e.g. nar_car_combine_t's H1cT), so that both operands reach the
+ * tensor cores without a transpose in shared memory.  precision 1, or 3 without b_lo; a_kmajor = 0, b_kmajor = 1; no bias /
+ * act / dact / a_scale / pred / car_ epilogue; accumulate and split_k as for nar_gemm_tf32.                              */
+int nar_gemm_tf32_dt(nar_ctx* ctx, int64_t M, int64_t N, int64_t K,
+                     const float* A, int64_t lda, int a_kmajor,
+                     const float* B, int64_t ldb, int b_kmajor,
+                     float* D, int64_t ldd, const nar_gemm_epilogue* epi /*host*/, void* stream);
 
 /* ---- session RNN (replaces tf.contrib.rnn.UGRNNCell in MultiRNNCell / dynamic_rnn,
  *      nar_model.py:1308-1342).  Rows are the valid positions only, grouped by session:
@@ -277,6 +285,10 @@ int nar_sample_negatives_uidx(nar_ctx* ctx, const int64_t* all_items_global, int
 int nar_car_combine(const float* PP /*[L,C]*/, const float* PC /*[L,C]*/, const float* PI /*[U,C]*/,
                     const int32_t* pos_idx, const int32_t* neg_uidx, int64_t L, int64_t K, int64_t C, int act,
                     float* H1c, void* stream);
+/* the same rows stored transposed: H1cT [C, ldr] with H1cT[c*ldr + r] = H1c[r*C + c], r < L*(1+K) <= ldr, ldr a multiple
+ * of 4 (columns r >= L*(1+K) are not written); bit-identical values                                                      */
+int nar_car_combine_t(const float* PP, const float* PC, const float* PI, const int32_t* pos_idx, const int32_t* neg_uidx,
+                      int64_t L, int64_t K, int64_t C, int act, float* H1cT, int64_t ldr, void* stream);
 /* (its backward is the layer-2 dgrad's epilogue: nar_gemm_epilogue.car_pp)                                          */
 
 /* ---- scorer + loss (replaces tf.multiply + matching_dense_layer_1..4 :478-500, softmax

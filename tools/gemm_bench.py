@@ -7,7 +7,9 @@ dgrad (single-pass TF32, leaky derivative from a separate aux, and with the CAR 
 instead of a stored dH1) and split-K wgrad (single-pass TF32, both operands
 MN-major, split chosen by the library), and the scorer's first layer
 (C -> 128) forward / dgrad / wgrad, also with the scorer product (51 candidates per position) as separate kernels
-(mul_pred + forward, dgrad + mul_pred_bwd) against folded into the GEMMs (A scaled by PR, product backward epilogue).  Each step case also reports the share of the data-sheet peak of the tensor path it
+(mul_pred + forward, dgrad + mul_pred_bwd) against folded into the GEMMs (A scaled by PR, product backward epilogue).
+CAR layer 2 also in the form the step runs with the candidate rows stored transposed (H1cT [C, ldr]): the forward with
+an MN-major A, and the weight gradient as dW^T = dE^T H1 (A = dE MN-major, B = H1cT K-major, D stored transposed).  Each step case also reports the share of the data-sheet peak of the tensor path it
 issues on (bf16 for bf16x3, counting its 3 MMAs per product; TF32 otherwise) and the rate at which TMA fills shared
 memory with operand tiles."""
 import json
@@ -79,6 +81,9 @@ def step_cases(dev):
     scorer on 132 SMs), red.add into dW."""
     R = STEP_R
     H1 = torch.randn(R, C, device=dev)
+    ldr = (R + 31) // 32 * 32
+    H1T = torch.zeros(C, ldr, device=dev)
+    H1T[:, :R] = H1.t()
     E = torch.empty(R, C, device=dev)
     dE = torch.randn(R, C, device=dev)
     dH1 = torch.empty(R, C, device=dev)
@@ -127,9 +132,11 @@ def step_cases(dev):
         ops.mul_pred_bwd(dPD, Ec, PR, L, n_cand, C, dEc, dPR, cand_act=ops.ACT_TANH)
     return [
         ('step L2 fwd   bf16x3 +bias tanh', lambda: ops.gemm(H1, None, E, R, C, C, ldb=0, bias=b2, act=ops.ACT_TANH, precision=4, b_bf16=W2plane, ld_bf16=W2plane.stride(0)), [R, C, C], E, 4),
+        ('step L2 fwd   bf16x3 A:MN (H1cT) +bias tanh', lambda: ops.gemm(H1T, None, E, R, C, C, a_kmajor=False, lda=ldr, ldb=0, bias=b2, act=ops.ACT_TANH, precision=4, b_bf16=W2plane, ld_bf16=W2plane.stride(0)), [R, C, C], E, 4),
         ('step L2 dgrad 1x +dact leaky aux sep', lambda: ops.gemm(dE, W2, dH1, R, C, C, precision=1, dact=ops.ACT_LEAKY, aux=H1), [R, C, C], dH1, 1),
         ('step L2 dgrad 1x CAR layer-1 backward epilogue (G1 462 x 51 rows)', car_dgrad, [Rg, C, C], DB, 1),
         ('step L2 wgrad 1x split-K', lambda: ops.gemm(H1, dE, dW2, C, C, R, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), [C, C, R], dW2, 1),
+        ('step L2 wgrad 1x split-K dW^T = dE^T H1cT^T, D transposed', lambda: ops.gemm(dE, H1T, dW2, C, C, R, a_kmajor=False, b_kmajor=True, ldb=ldr, accumulate=True, split_k=0, precision=1, trans_d=True), [C, C, R], dW2, 1),
         ('step M1 fwd   bf16x3 +bias leaky', lambda: ops.gemm(PD, None, Z1, R, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0)), [R, 128, C], Z1, 4),
         ('step M1 dgrad 1x', lambda: ops.gemm(dZ1, M0, dPD, R, C, 128, precision=1), [R, C, 128], dPD, 1),
         ('step M1 wgrad 1x split-K', lambda: ops.gemm(PD, dZ1, dM0, C, 128, R, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1), [C, 128, R], dM0, 1),
