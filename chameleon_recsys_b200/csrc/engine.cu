@@ -95,7 +95,9 @@ namespace {
 // forward and the weight gradient scale Ec by PR as they load it (nar_gemm_epilogue.a_scale, the same rounded product), the
 // dgrad's epilogue forms dEc and dPR from whole positions (nar_gemm_epilogue.pred).  PD and dPD are never stored.  Needs
 // the bf16x3 forward and single-pass TF32 backward, and positions that fit an M tile (1 + K <= 128); otherwise, or with
-// NAR_FUSED_SCORER_PRODUCT=0, nar_mul_pred / nar_mul_pred_bwd run around the plain GEMMs.
+// NAR_FUSED_SCORER_PRODUCT=0, nar_mul_pred / nar_mul_pred_bwd run around the plain GEMMs.  A recommend call folds the
+// product whenever the forward is bf16x3: the two other conditions belong to the training step's dgrad epilogue and
+// backward precision, and a recommend call runs neither.
 bool fused_product(const nar_engine* e) {
   const nar_model_cfg& c = e->cfg;
   return e->fused_product && c.ranking == 0 && c.K + 1 <= 128 && c.fwd_precision == 4 && c.bwd_precision == 1;
@@ -103,6 +105,15 @@ bool fused_product(const nar_engine* e) {
 
 // gate blocks per unit (the width of GX, Wx and the bias): UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o)
 int64_t gate_blocks(const nar_model_cfg& c) { return c.rnn_cell == NAR_CELL_LSTM ? 4 : c.rnn_cell == NAR_CELL_GRU ? 3 : 2; }
+
+// the feature plan of one call: the static part + the call's staged context and popularity inputs + its row statistics
+nar_feature_plan call_plan(const nar_model_cfg& c, const nar_step_io* io, const float* stats) {
+  nar_feature_plan plan = c.plan;
+  for (int i = 0; i < NAR_MAX_SRC; ++i) { plan.ctx_int[i] = io->ctx_int[i]; plan.ctx_float[i] = io->ctx_float[i]; }
+  plan.pop_norm = io->pop_norm;
+  plan.stats = stats;
+  return plan;
+}
 
 int64_t prep_carve(const nar_engine* e, int64_t Bg, int64_t B, int64_t T, int64_t L_cap, void* base, PrepBufs* pb) {
   const nar_model_cfg& c = e->cfg;
@@ -285,6 +296,29 @@ struct Seq {
     chk(nar_dropout_rows(src, dst, rows, cols, cols, row_pos, io->L, c.K + 1, c.K, tensor_id, c.keep_prob, c.dropout_seed,
                          (uint32_t)(io->global_step + 1), st));
   }
+  // the scorer (nar_model.py:444-517) of n_pos positions x n_cand candidate rows Ec against their positions' PR, on main:
+  // logits, and the softmax cross-entropy times inv_count added to loss[0] (:639-667; nov: the novelty regulariser).
+  // MLP: `fused` folds the product Ec * PR into the M1 GEMM (fused_product), else nar_mul_pred writes it to PD first;
+  // dZ3 given (training): also dZ3 and the last layer's gradients.  Cosine: dE / dPR given (training): their gradients.
+  void scorer(const float* Ec, const float* PR, int64_t n_pos, int64_t n_cand, bool fused, float* PD, float* Z1, float* Z2,
+              float* Z3, float* logits, float* loss, float inv_count, float* dZ3, float* dE, float* dPR,
+              const nar_novelty_reg* nov) {
+    const int64_t R = n_pos * n_cand, C = c.C;
+    if (c.ranking == 0) {
+      if (fused) {
+        fwd(Ec, C, c.off_M[0], c.ld_M[0], c.off_c[0], Z1, 128, R, 128, C, NAR_ACT_LEAKY_RELU, main, PR, C, n_cand);
+      } else {
+        chk(nar_mul_pred(Ec, PR, n_pos, n_cand, C, PD, main));
+        fwd(PD, C, c.off_M[0], c.ld_M[0], c.off_c[0], Z1, 128, R, 128, C, NAR_ACT_LEAKY_RELU, main);
+      }
+      fwd(Z1, 128, c.off_M[1], c.ld_M[1], c.off_c[1], Z2, 64, R, 64, 128, NAR_ACT_LEAKY_RELU, main);
+      fwd(Z2, 64, c.off_M[2], c.ld_M[2], c.off_c[2], Z3, 32, R, 32, 64, NAR_ACT_LEAKY_RELU, main);
+      chk(nar_score_softmax_ce(Z3, 32, 32, W(c.off_M[3]), c.ld_M[3], W(c.off_c[3]), n_pos, n_cand, c.inv_temperature, inv_count,
+                               logits, loss, dZ3, dZ3 ? G(c.off_M[3]) : nullptr, dZ3 ? G(c.off_c[3]) : nullptr, nov, main));
+    } else {
+      chk(nar_cosine_softmax_ce(Ec, PR, n_pos, n_cand, C, c.inv_temperature, inv_count, logits, loss, dE, dPR, nov, main));
+    }
+  }
 };
 
 // CAR (nar_model.py:374-405) of the L clicked rows sb.X[0:L] on the main stream, then the session branch - RNN (:408,
@@ -341,11 +375,7 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   const float inv_count = 1.0f / (float)(io->L_global > 0 ? io->L_global : 1);
   const int64_t U = pb.U, NB = 2 * L + U;
 
-  // ---- feature plan of this step: static part + the staged inputs
-  nar_feature_plan plan = c.plan;
-  for (int i = 0; i < NAR_MAX_SRC; ++i) { plan.ctx_int[i] = io->ctx_int[i]; plan.ctx_float[i] = io->ctx_float[i]; }
-  plan.pop_norm = io->pop_norm;
-  plan.stats = pb.stats;
+  const nar_feature_plan plan = call_plan(c, io, pb.stats);
   nar_row_layout rl;
   if (c.dedup) { rl.n_rows = NB; rl.n_input = L; rl.n_cand = 0; rl.n_positive = L; rl.n_full = 2 * L; rl.ctx_col0 = c0; }
   else { rl.n_rows = R; rl.n_input = L; rl.n_cand = n_cand; rl.n_positive = 0; rl.n_full = R; rl.ctx_col0 = c0; }
@@ -374,22 +404,8 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
   nov.cand_ids = pb.row_item + L; nov.loss_nov = io->loss + 2;
   const nar_novelty_reg* novp = c.novelty_reg_factor > 0.f ? &nov : nullptr;
   const bool fused = fused_product(e);
-  if (c.ranking == 0) {
-    if (fused) {
-      s.fwd(Ec, C, c.off_M[0], c.ld_M[0], c.off_c[0], sb.Z1, 128, Rc, 128, C, NAR_ACT_LEAKY_RELU, main, sb.PR, C, n_cand);
-    } else {
-      s.chk(nar_mul_pred(Ec, sb.PR, L, n_cand, C, sb.PD, main));
-      s.fwd(sb.PD, C, c.off_M[0], c.ld_M[0], c.off_c[0], sb.Z1, 128, Rc, 128, C, NAR_ACT_LEAKY_RELU, main);
-    }
-    s.fwd(sb.Z1, 128, c.off_M[1], c.ld_M[1], c.off_c[1], sb.Z2, 64, Rc, 64, 128, NAR_ACT_LEAKY_RELU, main);
-    s.fwd(sb.Z2, 64, c.off_M[2], c.ld_M[2], c.off_c[2], sb.Z3, 32, Rc, 32, 64, NAR_ACT_LEAKY_RELU, main);
-    s.chk(nar_score_softmax_ce(sb.Z3, 32, 32, s.W(c.off_M[3]), c.ld_M[3], s.W(c.off_c[3]), L, n_cand, c.inv_temperature, inv_count,
-                               sb.logits, io->loss, train ? sb.dZ3 : nullptr, train ? s.G(c.off_M[3]) : nullptr,
-                               train ? s.G(c.off_c[3]) : nullptr, novp, main));
-  } else {
-    s.chk(nar_cosine_softmax_ce(Ec, sb.PR, L, n_cand, C, c.inv_temperature, inv_count, sb.logits, io->loss,
-                                train ? sb.dE + L * C : nullptr, train ? sb.dPR : nullptr, novp, main));
-  }
+  s.scorer(Ec, sb.PR, L, n_cand, fused, sb.PD, sb.Z1, sb.Z2, sb.Z3, sb.logits, io->loss, inv_count, train ? sb.dZ3 : nullptr,
+           train ? sb.dE + L * C : nullptr, train ? sb.dPR : nullptr, novp);
   // every rank holds the same weights: the regulariser is added once (rank 0) so that a sum over ranks is exact
   // (off the critical path: it only feeds the reported loss)
   if (c.reg_l2 > 0.f && c.rank == 0) { cudaStream_t st = s.fork(); s.chk(nar_l2_loss_add(c.params, c.reg_end, c.reg_l2, io->loss + 1, st)); }
@@ -592,10 +608,7 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
   s.chk(nar_feature_stats(e->ctx, io->buffer, c.buf_len, c.n_norm, c.plan.created_at_ts, io->pop_norm, io->max_ts,
                           c.plan.log_base_recency, c.plan.log_base_novelty, rb.row_pos, rb.row_item, L + N, L, 0, io->event_ts,
                           rb.stats, main));
-  nar_feature_plan plan = c.plan;
-  for (int i = 0; i < NAR_MAX_SRC; ++i) { plan.ctx_int[i] = io->ctx_int[i]; plan.ctx_float[i] = io->ctx_float[i]; }
-  plan.pop_norm = io->pop_norm;
-  plan.stats = rb.stats;
+  const nar_feature_plan plan = call_plan(c, io, rb.stats);
   nar_row_layout rl;
   rl.n_rows = L + N; rl.n_input = L; rl.n_cand = 0; rl.n_positive = 0; rl.n_full = L; rl.ctx_col0 = c0;
   s.chk(nar_gather_features(e->ctx, &plan, rb.row_pos, rb.row_item, &rl, io->event_ts, io->max_ts, sb.X, main));
@@ -611,6 +624,7 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
   }
 
   // ---- per block of queries: every candidate chunk into logits [qb, N], then the top n of each query
+  const bool fused = e->fused_product && c.fwd_precision == 4;
   for (int64_t q0 = 0; q0 < Q && !s.rc; q0 += qb) {
     const int64_t Qb = Q - q0 < qb ? Q - q0 : qb;
     const float* pcq = rb.PCq + q0 * C; const float* prq = rb.PRq + q0 * C;
@@ -620,20 +634,7 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
       s.chk(nar_car_combine_grid(pcq, rb.PI, Qb, Nc, C, NAR_ACT_LEAKY_RELU, rb.H1g, main));
       s.fwd(rb.H1g, C, c.off_W2, C, c.off_b2, rb.Eg, C, P, C, C, NAR_ACT_TANH, main);
       float* lg = Nc == N ? rb.logits : rb.lg_chunk;
-      if (c.ranking == 0) {
-        if (e->fused_product && c.fwd_precision == 4) {     // the product folded into the GEMM as in run_step (any Nc)
-          s.fwd(rb.Eg, C, c.off_M[0], c.ld_M[0], c.off_c[0], rb.Z1, 128, P, 128, C, NAR_ACT_LEAKY_RELU, main, prq, C, Nc);
-        } else {
-          s.chk(nar_mul_pred(rb.Eg, prq, Qb, Nc, C, rb.H1g, main));
-          s.fwd(rb.H1g, C, c.off_M[0], c.ld_M[0], c.off_c[0], rb.Z1, 128, P, 128, C, NAR_ACT_LEAKY_RELU, main);
-        }
-        s.fwd(rb.Z1, 128, c.off_M[1], c.ld_M[1], c.off_c[1], rb.Z2, 64, P, 64, 128, NAR_ACT_LEAKY_RELU, main);
-        s.fwd(rb.Z2, 64, c.off_M[2], c.ld_M[2], c.off_c[2], rb.Z3, 32, P, 32, 64, NAR_ACT_LEAKY_RELU, main);
-        s.chk(nar_score_softmax_ce(rb.Z3, 32, 32, s.W(c.off_M[3]), c.ld_M[3], s.W(c.off_c[3]), Qb, Nc, c.inv_temperature, 0.f, lg,
-                                   rb.loss, nullptr, nullptr, nullptr, nullptr, main));
-      } else {
-        s.chk(nar_cosine_softmax_ce(rb.Eg, prq, Qb, Nc, C, c.inv_temperature, 0.f, lg, rb.loss, nullptr, nullptr, nullptr, main));
-      }
+      s.scorer(rb.Eg, prq, Qb, Nc, fused, rb.H1g, rb.Z1, rb.Z2, rb.Z3, lg, rb.loss, 0.f, nullptr, nullptr, nullptr, nullptr);
       if (Nc != N)
         s.chk((int)cudaMemcpy2DAsync(rb.logits + j0, (size_t)N * sizeof(float), lg, (size_t)Nc * sizeof(float),
                                      (size_t)Nc * sizeof(float), (size_t)Qb, cudaMemcpyDeviceToDevice, main));

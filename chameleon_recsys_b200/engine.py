@@ -51,14 +51,16 @@ def set_plan_columns(p: FeaturePlanC, pl: FeaturePlan):
 
 
 class NarEngine:
+    use_side_stream = True          # stage_ahead always stages on the side stream; kept for bench.py, which reads it
+
     def __init__(self, plan: FeaturePlan, layout: ParamLayout, content_article_embeddings_matrix: np.ndarray,
                  articles_metadata: Dict[str, np.ndarray], *, negative_samples: int, negative_sample_from_buffer: int,
                  softmax_temperature: float, reg_weight_decay: float, lr: float,
                  recent_clicks_buffer_max_size: int, recent_clicks_for_normalization: int,
                  elapsed_days_smooth_log_base: float = 1.3, popularity_smooth_log_base: float = 2.0,
                  ranking: str = 'mlp', rnn_cell: str = 'ugrnn', sampler_seed: int = 42, device: Optional[int] = None,
-                 fwd_precision: Optional[int] = None, bwd_precision: int = 1, process_group=None, max_batch: int = 0,
-                 dedup: Optional[bool] = None, keep_prob: float = 1.0, novelty_reg_factor: float = 0.0,
+                 fwd_precision: int = 4, bwd_precision: int = 1, process_group=None, max_batch: int = 0,
+                 dedup: bool = True, keep_prob: float = 1.0, novelty_reg_factor: float = 0.0,
                  dropout_seed: Optional[int] = None):
         if not torch.cuda.is_available():
             raise NarError('NarEngine needs a CUDA (sm_90a) device; there is no CPU fallback')
@@ -84,8 +86,6 @@ class NarEngine:
         self.seed = int(sampler_seed)
         # forward GEMMs: 3 = 3xTF32, 4 = bf16x3 (bf16 hi + lo pieces on the kind::f16 path: same error compensation at twice
         # the tensor rate and 2/3 of the operand bytes; logits within 3e-5 of fp32 instead of 3e-6 - the bar is 1e-3)
-        if fwd_precision is None:
-            fwd_precision = int(os.environ.get('NAR_FWD_PRECISION', '4'))
         self.fwd_prec, self.bwd_prec = int(fwd_precision), int(bwd_precision)
         self.pg = process_group
         self.world = torch.distributed.get_world_size(process_group) if process_group is not None else 1
@@ -94,8 +94,8 @@ class NarEngine:
         self.dp_balance = os.environ.get('NAR_DP_BALANCE', '1') == '1'
         self.C, self.H, self.Hp, self.layers = layout.C, layout.H, layout.Hp, layout.layers
         self.V = plan.num_items
-        # per-unique-id CAR layer 1 (exact; csrc/car.cu).  NAR_DEDUP=0 materialises every candidate row instead.
-        self.dedup = (os.environ.get('NAR_DEDUP', '1') == '1') if dedup is None else bool(dedup)
+        # per-unique-id CAR layer 1 (exact; csrc/car.cu).  dedup=False materialises every candidate row instead.
+        self.dedup = bool(dedup)
         # dropout (nar_model.py:338-340, :417-419, :1330-1333): masks are drawn per candidate row, so the rows cannot be
         # shared between candidates - training with keep_prob < 1 materialises every row
         self.keep_prob = float(keep_prob)
@@ -123,17 +123,16 @@ class NarEngine:
         self.params_lo = torch.zeros(n, device=d)      # w - tf32_trunc(w): B_lo plane of the 3xTF32 forward GEMMs
         self.global_step = 0
         self.loss_dev = self._grads_ext[n:]               # [xe, l2 regulariser, novelty regulariser, -]: total = [0] + [1] - [2]
-        self.loss_host = torch.zeros(4).pin_memory()
-        self._loss_hosts = [self.loss_host, torch.zeros(4).pin_memory()]    # two in flight: submit(n+1) before result(n)
+        self._loss_hosts = [torch.zeros(4).pin_memory() for _ in range(2)]   # two in flight: submit(n+1) before result(n)
         self._loss_slot = 0
+        self.loss_host = torch.zeros(4).pin_memory()      # eval_step's own: an evaluation never overwrites an unread step
         self._bufs: Dict[str, torch.Tensor] = {}
         self._pinned: Dict[str, torch.Tensor] = {}
         self._side = None
         self._prep_flip = 0
-        self.use_side_stream = os.environ.get('NAR_SIDE_STREAM', '1') == '1'
         self._slot_events: Dict[str, torch.cuda.Event] = {}       # prepare() slot -> end of the last step that read it
         self._pin_events: Dict[str, torch.cuda.Event] = {}        # staging slot -> its last H2D copy
-        self.use_aux_stream = os.environ.get('NAR_AUX_STREAM', '1') == '1'
+        self.use_aux_stream = True
         self._views: dict = {}
         self.last: Dict[str, torch.Tensor] = {}
         self.ops = ops
@@ -437,27 +436,21 @@ class NarEngine:
         """Per-step plan for callers that launch the gather kernel themselves (micro-benchmarks): the static part + this
         step's staged input pointers + the statistics written by prepare()."""
         p = FeaturePlanC.from_buffer_copy(bytes(self._cfg.plan))
-        t = st['t']
-        for i, n in enumerate(self.plan.ctx_int_names):
-            p.ctx_int[i] = t['ci/' + n].data_ptr()
-        for i, n in enumerate(self.plan.ctx_float_names):
-            p.ctx_float[i] = t['cf/' + n].data_ptr()
-        p.pop_norm = st['prep']['io'].pop_norm
+        io = st['prep']['io']
+        p.ctx_int, p.ctx_float, p.pop_norm = io.ctx_int, io.ctx_float, io.pop_norm
         p.stats = self.buffer(st, 'stats').data_ptr()
         return p
 
     # ------------------------------------------------------------------ the step
-    def _make_io(self, st: dict, slot: str, sampler_step: int) -> StepIO:
+    def _staged_io(self, st: dict) -> StepIO:
+        """A StepIO holding the inputs staged in ``st``: dims, ids, timestamps, labels, the recent-clicks state and the
+        context features.  Train, evaluate and predict all start from it."""
         t = st['t']
-        cap, prep_ws, ws = self._ensure_capacity(st['Bg'], st['B'], st['T'], st['L'], slot)
         io = StepIO()
-        io.B, io.Bg, io.T, io.sess0, io.L, io.L_global, io.L_cap = st['B'], st['Bg'], st['T'], st['s0'], st['L'], st['L_global'], cap
-        io.global_step = self.global_step
-        io.sampler_step = int(sampler_step) & 0xFFFFFFFF
-        io.train = 1                        # the carve of a training step is a superset: evaluation reuses the same offsets
+        io.B, io.Bg, io.T, io.sess0, io.L, io.L_global = st['B'], st['Bg'], st['T'], st['s0'], st['L'], st['L_global']
         io.all_items, io.event_ts = t['all_items'].data_ptr(), t['event_ts'].data_ptr()
         io.item_clicked, io.label_next = t['item_clicked'].data_ptr(), t['label_next'].data_ptr()
-        if st.get('dstate'):
+        if st['dstate']:
             # the state as of NOW: every update of an earlier batch has been queued (stream order does the rest)
             buf_t, pop_t = self.dstate.buffer_ids(), self.dstate.articles_recent_pop_norm()
             st['_hold_state'] = (buf_t, pop_t)
@@ -469,6 +462,15 @@ class NarEngine:
         for i, n in enumerate(self.plan.ctx_float_names):
             io.ctx_float[i] = t['cf/' + n].data_ptr()
         io.pos_idx, io.sess_off = t['pos_idx'].data_ptr(), t['sess_off'].data_ptr()
+        return io
+
+    def _make_io(self, st: dict, slot: str, sampler_step: int) -> StepIO:
+        cap, prep_ws, ws = self._ensure_capacity(st['Bg'], st['B'], st['T'], st['L'], slot)
+        io = self._staged_io(st)
+        io.L_cap = cap
+        io.global_step = self.global_step
+        io.sampler_step = int(sampler_step) & 0xFFFFFFFF
+        io.train = 1                        # the carve of a training step is a superset: evaluation reuses the same offsets
         io.prep_ws, io.prep_ws_bytes = prep_ws.data_ptr(), prep_ws.numel()
         io.ws, io.ws_bytes = ws.data_ptr(), ws.numel()
         io.loss = self.loss_dev.data_ptr()
@@ -592,38 +594,24 @@ class NarEngine:
             self._side = torch.cuda.Stream(device=self.dev)
         return self._side
 
-    def stage_ahead(self, features, labels, buffer, pop_norm, slot: str, after: Optional[torch.cuda.Event] = None) -> dict:
+    def stage_ahead(self, features, labels, buffer, pop_norm, slot: str, after: Optional[torch.cuda.Event] = None,
+                    prev: Optional[dict] = None) -> dict:
         """Stage the NEXT step while the current one runs: the host packs the batch into the slot's pinned buffer; the
-        H2D copy and the weight-independent front (sampler, row lists, statistics) run on a side stream next to the
-        current step's GEMMs.  NAR_SIDE_STREAM=0 queues the copy behind the running step on the main stream instead
-        and leaves the front inline."""
-        if self.use_side_stream:
-            side = self.side_stream()
-            if after is not None:
-                side.wait_event(after)        # the step that last read this slot's buffers (two slots alternate) is done
-            st = self.stage(features, labels, buffer, pop_norm, slot=slot, stream=side)
-            return self.prepare(st, self.global_step + 1, stream=side)
-        return self.stage(features, labels, buffer, pop_norm, slot=slot)
-
-    def stage_ahead_device_state(self, features, labels, slot: str, prev: Optional[dict],
-                                 after: Optional[torch.cuda.Event] = None) -> dict:
-        """``stage_ahead`` with the device-resident state: on the side stream, first the state absorbs the PREVIOUS batch
-        (``prev`` = its staged dict; what the hook's after_run does on the host in the reference), then the new batch is
-        copied and its weight-independent front runs against the updated state."""
-        side = self.side_stream() if self.use_side_stream else torch.cuda.current_stream()
-        if self.use_side_stream and getattr(self, '_dstate_ready', None) is not None:
+        H2D copy and the weight-independent front (sampler, row lists, statistics) run on the side stream next to the
+        current step's GEMMs.  ``buffer`` / ``pop_norm`` None: the device-resident state is read, and on the side stream
+        it first absorbs the PREVIOUS batch (``prev`` = its staged dict; what the hook's after_run does on the host in
+        the reference)."""
+        side = self.side_stream()
+        if getattr(self, '_dstate_ready', None) is not None:
             side.wait_event(self._dstate_ready)
             self._dstate_ready = None
-        if after is not None and self.use_side_stream:
-            side.wait_event(after)
+        if after is not None:
+            side.wait_event(after)            # the step that last read this slot's buffers (two slots alternate) is done
         if prev is not None:
-            if self.use_side_stream and prev.get('copied') is not None:
-                side.wait_event(prev['copied'])
+            side.wait_event(prev['copied'])
             self.advance_device_state(prev, stream=side)
-        st = self.stage(features, labels, None, None, slot=slot, stream=side if self.use_side_stream else None)
-        if self.use_side_stream:
-            return self.prepare(st, self.global_step + 1, stream=side)
-        return st
+        st = self.stage(features, labels, buffer, pop_norm, slot=slot, stream=side)
+        return self.prepare(st, self.global_step + 1, stream=side)
 
     def submit(self, st: dict, keep: bool = False) -> dict:
         """Queue one training step; nothing here waits for the GPU.  ``result(out)`` later waits for THIS step only
@@ -641,10 +629,7 @@ class NarEngine:
 
     def result(self, out: dict) -> dict:
         out['done'].synchronize()
-        host = out['loss_host']
-        out['xe_loss'] = float(host[0]); out['reg_loss'] = float(host[1]); out['nov_reg_loss'] = float(host[2])
-        out['total_loss'] = out['xe_loss'] + out['reg_loss'] - out['nov_reg_loss']
-        return out
+        return _read_loss(out, out['loss_host'])
 
     # ---- evaluation (ModeKeys.EVAL): forward + ranking of the 1+K candidates + HR@n / MRR@n accumulators
     def share_params(self, other: 'NarEngine'):
@@ -686,10 +671,8 @@ class NarEngine:
         if before_sync is not None:
             before_sync()
         torch.cuda.current_stream().synchronize()
-        out['xe_loss'] = float(self.loss_host[0]); out['reg_loss'] = float(self.loss_host[1]); out['nov_reg_loss'] = float(self.loss_host[2])
-        out['total_loss'] = out['xe_loss'] + out['reg_loss'] - out['nov_reg_loss']
         out['stage'] = st
-        return out
+        return _read_loss(out, self.loss_host)
 
     # ---- recommendation (ModeKeys.PREDICT): score a candidate set for query positions, keep the top n
     MAX_TOP_N = 4096
@@ -771,18 +754,8 @@ class NarEngine:
         ids = torch.empty(Q, top_n, dtype=torch.int64, device=d)
         scores = torch.empty(Q, top_n, dtype=torch.float32, device=d)
         probs = torch.empty(Q, top_n, dtype=torch.float32, device=d)
-        t = st['t']
-        io = StepIO()
-        io.B, io.Bg, io.T, io.sess0, io.L, io.L_global, io.L_cap = st['B'], Bg, T, st['s0'], L, st['L_global'], L
-        io.global_step, io.train = self.global_step, 0
-        io.all_items, io.event_ts = t['all_items'].data_ptr(), t['event_ts'].data_ptr()
-        io.item_clicked, io.label_next = t['item_clicked'].data_ptr(), t['label_next'].data_ptr()
-        io.buffer, io.max_ts, io.pop_norm = t['buffer'].data_ptr(), t['max_ts'].data_ptr(), t['pop_norm'].data_ptr()
-        for i, n in enumerate(self.plan.ctx_int_names):
-            io.ctx_int[i] = t['ci/' + n].data_ptr()
-        for i, n in enumerate(self.plan.ctx_float_names):
-            io.ctx_float[i] = t['cf/' + n].data_ptr()
-        io.pos_idx, io.sess_off = t['pos_idx'].data_ptr(), t['sess_off'].data_ptr()
+        io = self._staged_io(st)
+        io.L_cap, io.global_step, io.train = L, self.global_step, 0
         io.ws, io.ws_bytes = ws.data_ptr(), ws.numel()
         cur = torch.cuda.current_stream()
         check(self._lib.nar_engine_recommend(self._handle, C.byref(io), C.c_void_p(0 if q_rows_t is None else q_rows_t.data_ptr()),
@@ -797,14 +770,13 @@ class NarEngine:
         return out
 
     def train_step(self, features, labels, buffer, pop_norm, keep: bool = False, sync: bool = True) -> dict:
-        st = self.stage(features, labels, buffer, pop_norm)
-        out = self.step(st, train=True, keep=keep)
-        if st['L'] > 0 or self.world > 1:
-            self.apply_gradients(st)                  # (the loss accumulators ride along with the gradients)
-        self.loss_host.copy_(self.loss_dev, non_blocking=True)
-        out['stage'] = st
-        if sync:
-            torch.cuda.current_stream().synchronize()
-            out['xe_loss'] = float(self.loss_host[0]); out['reg_loss'] = float(self.loss_host[1]); out['nov_reg_loss'] = float(self.loss_host[2])
-            out['total_loss'] = out['xe_loss'] + out['reg_loss'] - out['nov_reg_loss']
-        return out
+        """Stage, run and apply one training step; ``sync``: wait for it and read its loss (else ``result(out)`` does)."""
+        out = self.submit(self.stage(features, labels, buffer, pop_norm), keep=keep)
+        return self.result(out) if sync else out
+
+
+def _read_loss(out: dict, host: torch.Tensor) -> dict:
+    """The four loss keys of ``out`` from a host copy of the loss accumulators [xe, l2, novelty, -]."""
+    out['xe_loss'], out['reg_loss'], out['nov_reg_loss'] = host[:3].tolist()
+    out['total_loss'] = out['xe_loss'] + out['reg_loss'] - out['nov_reg_loss']
+    return out

@@ -172,22 +172,9 @@ class Estimator:
         nar_model.py:1635-1650), fetches batch n+1 (tf.data prefetch(1), datasets.py:142) and stages it - H2D copy,
         negative sampling, row lists, normalisation statistics - on a side stream; the loss of step n is read only after
         step n+1 has been queued (two pinned loss slots, one event per step), so the GPU never waits for the host."""
-        it = input_fn()
-
-        def fetch():
-            try:
-                return it.get_next() if hasattr(it, 'get_next') else next(it)
-            except (OutOfRangeError, StopIteration):
-                return None
-
-        def feed_of(spec):
-            feed = {}
-            for h in spec.training_chief_hooks:
-                feed.update(h.before_run(None))
-            return feed
-
+        batches = _batches(input_fn(), steps)
         n = 0
-        nxt = fetch() if (steps is None or steps > 0) else None
+        nxt = next(batches, None)
         if nxt is None:
             return self
         spec = self._ensure_spec(*nxt)
@@ -200,12 +187,19 @@ class Estimator:
         # brought up to date when train() returns.
         use_ds = os.environ.get('NAR_DEVICE_STATE', '1') == '1' and self._state() is not None
         prev_st = None
+
+        def stage_next(batch, slot, after=None):
+            if use_ds:                                              # the device state absorbs prev_st first
+                return eng.stage_ahead(batch[0], batch[1], None, None, slot, after=after, prev=prev_st)
+            feed = {}
+            for h in spec.training_chief_hooks:
+                feed.update(h.before_run(None))
+            return eng.stage_ahead(batch[0], batch[1], feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'],
+                                   slot, after=after)
+
         if use_ds:
             eng.attach_device_state(self._state())
-            st_next = eng.stage_ahead_device_state(nxt[0], nxt[1], 'pipe0', None)
-        else:
-            feed = feed_of(spec)
-            st_next = eng.stage_ahead(nxt[0], nxt[1], feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], 'pipe0')
+        st_next = stage_next(nxt, 'pipe0')
         pending = None                                              # (features, labels, out) of the step whose loss is unread
         # baseline recommenders (nar_model.py:1641-1646): every batch is folded into their tables (and the session kNN
         # rings, with the batch's session ids) on the side stream, behind the batch's copy; the main stream's work is
@@ -216,9 +210,7 @@ class Estimator:
 
         def fold(st):
             if tables is not None and st['has_clicks']:
-                import torch
-                side = eng.side_stream() if eng.use_side_stream else torch.cuda.current_stream()
-                tables.update(st['t']['all_items'], lens=st['fold_lens'], stream=side, after=st.get('copied'),
+                tables.update(st['t']['all_items'], lens=st['fold_lens'], stream=eng.side_stream(), after=st.get('copied'),
                               session_ids=st['fold_sids'])
 
         def finish(p):
@@ -244,17 +236,13 @@ class Estimator:
                 for h in spec.training_chief_hooks:
                     h.after_run(None, run_values)                    # host state now describes "before step n+1"
             n += 1
-            nxt = fetch() if (steps is None or n < steps) else None
+            nxt = next(batches, None)
             if nxt is not None:
                 # slot (n & 1) was last read by step n-1 (= pending): its event gates the side-stream copy
                 after = pending[2]['done'] if pending is not None else None
+                st_next = stage_next(nxt, 'pipe%d' % (n & 1), after)
                 if use_ds:
-                    st_next = eng.stage_ahead_device_state(nxt[0], nxt[1], 'pipe%d' % (n & 1), prev_st, after=after)
                     fold(prev_st)                                    # after the device state absorbed it
-                else:
-                    feed = feed_of(spec)
-                    st_next = eng.stage_ahead(nxt[0], nxt[1], feed['pop_recent_items_buffer'],
-                                              feed['articles_recent_pop_norm'], 'pipe%d' % (n & 1), after=after)
             elif use_ds:
                 eng.advance_device_state(prev_st)                    # the last batch of this train() call
                 fold(prev_st)
@@ -310,18 +298,7 @@ class Estimator:
         import torch
         if positions not in ('last', 'all'):
             raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
-        it = input_fn()
-
-        def fetch():
-            try:
-                return it.get_next() if hasattr(it, 'get_next') else next(it)
-            except (OutOfRangeError, StopIteration):
-                return None
-
-        n = 0
-        nxt = fetch() if (steps is None or steps > 0) else None
-        while nxt is not None:
-            features, labels = nxt
+        for n, (features, labels) in enumerate(_batches(input_fn(), steps)):
             if getattr(self, '_predict_spec', None) is None:
                 self._predict_spec = self.model_fn(features, labels, ModeKeys.PREDICT, self.params)
             spec = self._predict_spec
@@ -344,8 +321,6 @@ class Estimator:
                        'predicted_item_ids': out['predicted_item_ids'][sel],
                        'predicted_item_scores': out['predicted_item_scores'][sel],
                        'predicted_item_probs': out['predicted_item_probs'][sel]}
-            n += 1
-            nxt = fetch() if (steps is None or n < steps) else None
         torch.cuda.synchronize()
 
     def evaluate(self, input_fn, steps: Optional[int] = None, hooks=None, name=None) -> dict:
@@ -359,15 +334,8 @@ class Estimator:
         ``avg_norm_pop_by_pos_PP`` of the model and ``hitrate_at_n_by_pos_<suffix>_PP`` of every baseline, for each
         session position PP ('%02d', from 01) that had a query (none without input)."""
         import torch
-        it = input_fn()
-
-        def fetch():
-            try:
-                return it.get_next() if hasattr(it, 'get_next') else next(it)
-            except (OutOfRangeError, StopIteration):
-                return None
-
-        nxt = fetch() if (steps is None or steps > 0) else None
+        batches = _batches(input_fn(), steps)
+        nxt = next(batches, None)
         if nxt is None:
             empty = {'loss': float('nan'), 'hitrate_at_n': float('nan'), 'mrr_at_n': float('nan'),
                      'global_step': 0 if self._spec is None else self._spec.model.global_step()}
@@ -404,7 +372,7 @@ class Estimator:
                 h.after_run(None, run_values)
             loss_sum += out['total_loss']
             n += 1
-            nxt = fetch() if (steps is None or n < steps) else None
+            nxt = next(batches, None)
         bench = {}
         for h in spec.evaluation_hooks:
             bench.update(h.benchmark_results())
@@ -422,6 +390,18 @@ class Estimator:
     @property
     def model(self) -> Optional[NARModuleModel]:
         return None if self._spec is None else self._spec.model
+
+
+def _batches(it, steps: Optional[int]):
+    """(features, labels) from the input_fn iterator ``it`` until it runs out or ``steps`` batches were taken (None: all)."""
+    n = 0
+    while steps is None or n < steps:
+        try:
+            batch = it.get_next() if hasattr(it, 'get_next') else next(it)
+        except (OutOfRangeError, StopIteration):
+            return
+        yield batch
+        n += 1
 
 
 def _session_clicks(features, labels) -> np.ndarray:

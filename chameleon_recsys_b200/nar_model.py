@@ -50,7 +50,7 @@ class NARModuleModel:
                  eval_cold_start=False,
                  # --- extensions (not in the reference signature) ---
                  rnn_cell='ugrnn', ranking='mlp', sampler_seed=42, init_seed=42, device=None,
-                 process_group=None, fwd_precision=None, bwd_precision=1):
+                 process_group=None, fwd_precision=4, bwd_precision=1):
         from .engine import NarEngine          # imports torch + the CUDA library; fails loudly without them
         self.mode = mode
         self.lr = lr

@@ -50,7 +50,7 @@ def run_steps(eng, staged):
     for i, st in enumerate(staged):
         eng.step(st, train=True)
         eng.apply_gradients(st)
-        if eng.use_side_stream and i + 1 < len(staged):
+        if i + 1 < len(staged):
             eng.prepare(staged[i + 1], eng.global_step + 1, stream=side)
 
 

@@ -66,7 +66,7 @@ def main():
             done.pop(i - 2).synchronize()
         eng.step(staged[i], train=True)
         eng.apply_gradients(staged[i])
-        if eng.use_side_stream and i + 1 < len(staged):
+        if i + 1 < len(staged):
             eng.prepare(staged[i + 1], eng.global_step + 1, stream=side)
         ev = torch.cuda.Event()
         ev.record()
