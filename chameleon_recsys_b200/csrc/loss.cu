@@ -133,6 +133,9 @@ score_softmax_ce_kernel(const float* __restrict__ z3, int64_t ld_z, int width, c
 // cosine mode: one CTA (128 threads = 4 warps) per position; pred row staged in shared memory,
 // each warp walks candidates, warp-shuffle dot products, then the same softmax-CE.
 constexpr int COS_THREADS = 128;
+// l2-normalisation floor on the norm, x / max(|x|, eps) (the oracle's F.normalize).  A norm held at the floor is a
+// constant: the gradient of its row has no normalisation term.
+constexpr float COS_EPS = 1e-12f;
 
 __global__ void __launch_bounds__(COS_THREADS)
 cosine_softmax_ce_kernel(const float* __restrict__ cand, const float* __restrict__ pred, int64_t n_cand, int C,
@@ -141,7 +144,7 @@ cosine_softmax_ce_kernel(const float* __restrict__ cand, const float* __restrict
   extern __shared__ float sh[];
   float* sp = sh;                       // [C] pred row
   float* s_dot = sh + C;                // [n_cand] <cand_j, pred>
-  float* s_nrm = s_dot + n_cand;        // [n_cand] |cand_j|
+  float* s_nrm = s_dot + n_cand;        // [n_cand] |cand_j| (before the floor)
   float* s_ds = s_nrm + n_cand;         // [n_cand] d loss / d cos_j
   __shared__ float s_red[8];
   const int64_t l = blockIdx.x;
@@ -151,19 +154,23 @@ cosine_softmax_ce_kernel(const float* __restrict__ cand, const float* __restrict
   pp = warp_sum(pp);
   if (lane == 0) s_red[w] = pp;
   __syncthreads();
-  const float pn = fmaxf(sqrtf(s_red[0] + s_red[1] + s_red[2] + s_red[3]), 1e-12f);   // tf.nn.l2_normalize epsilon
+  const float pn_raw = sqrtf(s_red[0] + s_red[1] + s_red[2] + s_red[3]), pn = fmaxf(pn_raw, COS_EPS);
+  const bool pn_live = pn_raw >= COS_EPS;
   for (int64_t j = w; j < n_cand; j += COS_THREADS / 32) {
     const float* e = cand + (l * n_cand + j) * C;
     float d = 0.f, n = 0.f;
     for (int c = lane; c < C; c += 32) { const float v = e[c]; d = fmaf(v, sp[c], d); n = fmaf(v, v, n); }
     d = warp_sum(d); n = warp_sum(n);
-    if (lane == 0) { s_dot[j] = d; s_nrm[j] = fmaxf(sqrtf(n), 1e-12f); }
+    if (lane == 0) { s_dot[j] = d; s_nrm[j] = sqrtf(n); }
   }
   __syncthreads();
   float* lg = logits + l * n_cand;
   if (w == 0) {
     float mx = -INFINITY;
-    for (int64_t j = lane; j < n_cand; j += 32) { const float s = s_dot[j] / (s_nrm[j] * pn) * inv_temp; lg[j] = s; mx = fmaxf(mx, s); }
+    for (int64_t j = lane; j < n_cand; j += 32) {
+      const float s = s_dot[j] / (fmaxf(s_nrm[j], COS_EPS) * pn) * inv_temp;
+      lg[j] = s; mx = fmaxf(mx, s);
+    }
     mx = warp_max(mx);
     __syncwarp();
     float se = 0.f;
@@ -186,15 +193,17 @@ cosine_softmax_ce_kernel(const float* __restrict__ cand, const float* __restrict
   }
   __syncthreads();
   if (d_cand == nullptr) return;
-  // cos = <e,p>/(|e||p|) : d/de = p/(|e||p|) - cos * e/|e|^2 ; d/dp = e/(|e||p|) - cos * p/|p|^2
+  // cos = <e,p>/(|e||p|) : d/de = p/(|e||p|) - cos * e/|e|^2 ; d/dp = e/(|e||p|) - cos * p/|p|^2 (no second term for a
+  // floored norm)
   for (int c = threadIdx.x; c < C; c += COS_THREADS) {
     const float pc = sp[c];
     float dp = 0.f;
     for (int64_t j = 0; j < n_cand; ++j) {
-      const float en = s_nrm[j], cs = s_dot[j] / (en * pn), ds = s_ds[j];
+      const float en = fmaxf(s_nrm[j], COS_EPS), cs = s_dot[j] / (en * pn), ds = s_ds[j];
+      const float ce = s_nrm[j] >= COS_EPS ? cs : 0.f, cp = pn_live ? cs : 0.f;
       const float ec = cand[(l * n_cand + j) * C + c];
-      d_cand[(l * n_cand + j) * C + c] = ds * (pc / (en * pn) - cs * ec / (en * en));
-      dp = fmaf(ds, ec / (en * pn) - cs * pc / (pn * pn), dp);
+      d_cand[(l * n_cand + j) * C + c] = ds * (pc / (en * pn) - ce * ec / (en * en));
+      dp = fmaf(ds, ec / (en * pn) - cp * pc / (pn * pn), dp);
     }
     d_pred[l * C + c] = dp;
   }
@@ -299,6 +308,10 @@ extern "C" int nar_cosine_softmax_ce(const float* cand, const float* pred, int64
   if (n_pos <= 0) return NAR_OK;
   const size_t smem = (size_t)(C + 3 * n_cand) * sizeof(float);
   if (smem > 48 * 1024) return NAR_ERR_UNSUPPORTED;
+  // with the kernel's static s_red, the top 32 bytes of that range (which the engine's cosine_chunk_cap reaches) exceed
+  // the 48 KB a launch gets without opting in
+  if (smem > 48 * 1024 - 8 * sizeof(float))
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(nar::loss::cosine_softmax_ce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   nar::loss::cosine_softmax_ce_kernel<<<(unsigned)n_pos, nar::loss::COS_THREADS, smem, as_stream(stream)>>>(
       cand, pred, n_cand, (int)C, inv_temperature, inv_count, logits, loss_sum, d_cand, d_pred, nv);
   NAR_LAUNCH_CHECK();
