@@ -889,6 +889,10 @@ static int gemm(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, i
   if (epi->bias && (reinterpret_cast<uintptr_t>(epi->bias) & 15u) != 0) return NAR_ERR_INVALID;
   if (epi->dact && !car_bwd && (!epi->aux || (epi->ld_aux & 3) != 0 || (reinterpret_cast<uintptr_t>(epi->aux) & 15u) != 0)) return NAR_ERR_INVALID;
   if (epi->precision != 1 && epi->precision != 3 && epi->precision != 4) return NAR_ERR_INVALID;
+  auto is_act = [](int32_t a) { return a == NAR_ACT_NONE || a == NAR_ACT_LEAKY_RELU || a == NAR_ACT_TANH; };
+  if (!is_act(epi->act) || !is_act(epi->dact)) return NAR_ERR_INVALID;
+  // every split-K CTA runs the epilogue on its own partial sum: a bias or an activation would apply once per split
+  if (epi->split_k > 1 && (epi->bias || epi->act)) return NAR_ERR_INVALID;
   const bool bf16 = epi->precision == 4;
   if (bf16 && (!epi->b_bf16 || epi->accumulate || epi->split_k > 1)) return NAR_ERR_INVALID;
   const bool blo = epi->precision == 3 && epi->b_lo != nullptr;
@@ -936,8 +940,8 @@ static int gemm(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, i
   const bool amn = !a_kmajor, bmn = !b_kmajor;
   int split = epi->split_k;
   if (split <= 0) {          // auto, for accumulate: as many CTAs as fit in one wave of the SMs' resident slots
-    split = 1;               // (a CTA past a whole wave would run alone in a second one), at least 8 k-tiles per split
-    if (epi->accumulate) {
+    split = 1;               // (a CTA past a whole wave would run alone in a second one), at least 8 k-tiles per split;
+    if (epi->accumulate && !epi->bias && !epi->act) {    // one split when the epilogue adds a bias or applies act
       const int per_sm = mode == 0 ? ctas_per_sm<0>(bmn) : (mode == 1 ? ctas_per_sm<1>(bmn) : ctas_per_sm<2>(bmn));
       const int64_t fit = (int64_t)per_sm * ctx->sm_count / (n_tiles * m_tiles);
       const int64_t cap = k_tiles / 8 > 1 ? k_tiles / 8 : 1;

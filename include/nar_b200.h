@@ -162,12 +162,13 @@ typedef enum { NAR_CELL_UGRNN = 0, NAR_CELL_GRU = 1, NAR_CELL_LSTM = 2 } nar_rnn
 
 typedef struct {
   const float* bias;      /* [N] added before the activation, or NULL */
-  int32_t act;            /* nar_act applied to acc+bias */
+  int32_t act;            /* nar_act applied to acc+bias (any other value is rejected) */
   int32_t dact;           /* nar_act whose DERIVATIVE (evaluated from the forward OUTPUT aux) multiplies the result */
   const float* aux;       /* [M,N] forward output of the layer being differentiated (dact != NONE) */
   int64_t ld_aux;
   int32_t accumulate;     /* 1: D += result with atomics (required when split_k > 1) */
-  int32_t split_k;        /* >=1 */
+  int32_t split_k;        /* >=1; <= 0 with accumulate: chosen by the library.  Each split runs the epilogue on its own
+                             partial sum, so split_k > 1 with bias or act is rejected, and the library's choice is 1 then */
   int32_t precision;      /* 1 = TF32, 3 = 3xTF32 (error-compensated, ~fp32 accuracy) */
   const float* b_lo;      /* precision 3 only, optional: x - tf32_trunc(x) of operand B, same shape / ld as B (see
                              nar_tf32_lo; the weights' lo plane is maintained by nar_adam_tf).  NULL: split B in-kernel */
