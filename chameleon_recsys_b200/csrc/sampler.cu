@@ -336,7 +336,7 @@ static int carve(void* base, int64_t bytes, int64_t NB, int64_t buf_len, int64_t
 }  // namespace nar
 
 extern "C" int nar_sample_negatives_workspace(int64_t Bg, int64_t T1, int64_t buf_len, int64_t K, int64_t* bytes) {
-  if (!bytes) return NAR_ERR_INVALID;
+  if (!bytes || buf_len < 0) return NAR_ERR_INVALID;
   nar::sampler::PoolWs ws;
   return nar::sampler::carve(nullptr, 0, Bg * T1, buf_len, K * 20, &ws, bytes);
 }
@@ -357,6 +357,9 @@ extern "C" int nar_sample_negatives_uidx(nar_ctx* ctx, const int64_t* all_items_
   using namespace nar::sampler;
   if (!ctx || !all_items_global || !buffer || !out || !workspace) return NAR_ERR_INVALID;
   if (T1 < 2 || K <= 0 || B < 0 || sess0 < 0 || sess0 + B > Bg) return NAR_ERR_INVALID;
+  // a negative buffer length would shrink the pool's stream and carve the workspace from negative sizes; a negative
+  // sample count has no meaning (the oracle's slice would drop entries from the end)
+  if (buf_len < 0 || n_from_buffer < 0) return NAR_ERR_INVALID;
   const int64_t cap = K * 20;
   if (cap > MAX_POOL) return NAR_ERR_UNSUPPORTED;
   if (Bg * T1 + buf_len >= (1ll << 32)) return NAR_ERR_UNSUPPORTED;

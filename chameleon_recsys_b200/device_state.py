@@ -1,11 +1,12 @@
-"""Device-resident ``ClickedItemsState`` (SURVEY.md section 8f #1) - STAGED.
+"""Device-resident ``ClickedItemsState`` (SURVEY.md section 8f #1).
 
 The recent-clicks buffer and the recent-popularity vector live in HBM (two ping-pong slots: the step in flight reads
 one while the update for the next step writes the other) and are advanced by one single-CTA kernel per step
 (``nar_state_update``, csrc/state.cu) from the batch arrays that are already staged for the step.  Same arithmetic as
-the host class (clicked_items_state.py, itself pinned against the reference's).  Not yet wired into the default
-training loop: the host update costs 0.19 ms per step and is overlapped with the GPU step; wiring it in removes the
-0.34 MB per-step upload of buffer + popularity.  Covered by tests/test_device_state.py (runs on a GPU box).
+the host class (clicked_items_state.py, itself pinned against the reference's).  ``Estimator.train`` keeps the state
+here by default (``NarEngine.attach_device_state``; ``NAR_DEVICE_STATE=0`` keeps the hook's host update and its 0.34 MB
+per-step upload of buffer + popularity) and writes it back to the host object when training returns.  Covered by
+tests/test_device_state.py (runs on a GPU box), bit for bit against oracle/clicked_items_state_ref.py.
 """
 from __future__ import annotations
 

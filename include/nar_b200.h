@@ -265,7 +265,8 @@ int nar_lstm_bwd(nar_ctx* ctx, const float* d_hout, const float* h_out, const fl
 /* ---- negative sampler (replaces nar_model.py:1220-1304: tf.random_shuffle x(2+clicks),
  *      tf.unique, unsorted_segment_min, tf.setdiff1d inside nested tf.map_fn).  RNG spec:
  *      oracle/sampler_ref.py.  all_items_global [Bg,T1] builds the pool; negatives are
- *      produced for local sessions [sess0, sess0+B).  out [B,T1-1,K] int64, zero padded.   */
+ *      produced for local sessions [sess0, sess0+B).  out [B,T1-1,K] int64, zero padded.
+ *      buf_len < 0 or n_from_buffer < 0: NAR_ERR_INVALID; K*20 > 16384: NAR_ERR_UNSUPPORTED. */
 int nar_sample_negatives_workspace(int64_t Bg, int64_t T1, int64_t buf_len, int64_t K, int64_t* bytes /*host*/);
 int nar_sample_negatives(nar_ctx* ctx, const int64_t* all_items_global, int64_t Bg, int64_t T1,
                          int64_t sess0, int64_t B, const int64_t* buffer, int64_t buf_len,
@@ -364,7 +365,7 @@ int nar_host_state_update_batch(int64_t* buffer, int64_t cap, const int64_t* ite
                                 int64_t* batch_scratch, int64_t* scratch, int64_t* recent_pop, double* pop_norm,
                                 int64_t* articles_pop, int64_t num_items, double min_norm_pop);
 
-/* ---- device-resident ClickedItemsState (same update as above, in HBM; STAGED: not yet on the default training loop).
+/* ---- device-resident ClickedItemsState (same update as above, in HBM; what Estimator.train advances every step).
  *      old_items / old_ts [cap] -> new_items / new_ts [cap] (distinct buffers: ping-pong); all_items [Bg,T+1] =
  *      [item_clicked | label_last_item], event_ts [Bg,T]; recent_pop [V] int64 scratch / output; pop_norm [V] float32
  *      (what the graph reads), pop_norm64 [V] float64 or NULL; articles_pop [V] in/out; err[0] = 1 on an id outside
