@@ -4,10 +4,13 @@
 // State: a ring of S slots holding the last S sessions in insertion order (logical index 0 = oldest; head and count are
 // tracked by the caller, which knows them from the batch sizes).  Slot: session id (int64), length, and up to W item ids
 // (int32, sorted ascending, deduplicated).  An item is stored as +x while (x, id) is in the reference's item -> sessions
-// map ("live") and as -x once an eviction has discarded that pair; the similarity always uses |x| (the full set).
-// Update, per batch: stage the new entries (sorted sets), evict the oldest max(0, count + B - S) entries (clearing the
-// live bits of their items in every surviving slot, staged ones included, with the same session id: the reference's
-// discard also drops the pair of a newer entry with that id), then copy the staged entries into their slots.
+// map ("live") and as -x once an eviction has discarded that pair; the similarity always uses |x| (the full set).  Every
+// entry with the same session id holding x carries the same sign: it is one map lookup.
+// Update, per batch: stage the new entries (sorted sets); set +x again in every old slot with the id of a staged entry
+// whose set holds x (the reference adds the new pairs to the map before it evicts, so a returning id revives them);
+// evict the oldest max(0, count + B - S) entries (clearing the live bits of their items in every surviving slot, staged
+// ones included, with the same session id: the reference's discard also drops the pair of a newer entry with that id);
+// then copy the staged entries into their slots.
 // Score, one CTA per query: candidates with multiplicity from the live sets and the reference's binary search over the
 // ring in insertion order, the 'recent' cut, fp64 similarities in the reference's association, the neighbour cut, item
 // scores of the query's own candidates summed copy by copy, exact ranking and an integer rank histogram.
@@ -58,6 +61,27 @@ __device__ __forceinline__ bool contains(const int* set, int n, int x) {
   int lo = 0, hi = n;
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (set[mid] < x) lo = mid + 1; else hi = mid; }
   return lo < n && set[lo] == x;
+}
+
+// one CTA per staged entry b: +x in every surviving old entry (logical E..count-1) with its id whose set holds x
+__global__ void relive_kernel(const int64_t* ids, const int* lens, int* items, int64_t S, int W, int64_t head,
+                              int64_t count, int64_t E, const int64_t* st_ids, const int* st_lens, const int* st_items) {
+  __shared__ int s_set[MAX_W];
+  const int64_t b = blockIdx.x;
+  const int n = st_lens[b];
+  const int64_t sid = st_ids[b];
+  for (int k = threadIdx.x; k < n; k += blockDim.x) s_set[k] = st_items[b * W + k];
+  __syncthreads();
+  for (int64_t i = E + threadIdx.x; i < count; i += blockDim.x) {
+    const int64_t p = (head + i) % S;
+    if (ids[p] != sid) continue;
+    int* row = items + p * W;
+    const int L = lens[p];
+    for (int k = 0; k < L; ++k) {
+      const int x = row[k];
+      if (x < 0 && contains(s_set, n, -x)) row[k] = -x;      // every writer stores the same value
+    }
+  }
 }
 
 // one CTA per evicted entry e (logical e < E): survivors are the old entries E..count-1 and the staged ones
@@ -407,6 +431,10 @@ extern "C" int nar_sknn_update(int64_t* ids, int32_t* lens, int32_t* items, int6
   stage_kernel<<<(unsigned)B, MAX_W, 0, s>>>(all_items, T1, session_ids, num_items, st_ids, st_lens, st_items, (int)W, err);
   NAR_LAUNCH_CHECK();
   const int64_t E = count + B - S > 0 ? count + B - S : 0;
+  if (count > E) {
+    relive_kernel<<<(unsigned)B, 256, 0, s>>>(ids, lens, items, S, (int)W, head, count, E, st_ids, st_lens, st_items);
+    NAR_LAUNCH_CHECK();
+  }
   if (E > 0) {
     evict_kernel<<<(unsigned)E, 256, 0, s>>>(ids, lens, items, S, (int)W, head, count, E, st_ids, st_lens, st_items, B);
     NAR_LAUNCH_CHECK();
