@@ -15,6 +15,7 @@ constexpr int LIST_THREADS = 128;
 constexpr int REDUCE_THREADS = 256;
 constexpr int MAX_M = 64;                  // list positions scored per query (top_n)
 constexpr int N_VALUES = 6;                // per query: ndcg, esi-r, esi-rr, eild-r, eild-rr, 1 (the query count)
+constexpr size_t MAX_LIST_SMEM = 200 * 1024;   // list_kernel's dynamic shared memory: [m, m] fp64 + [m, acr_dim] fp32
 
 __device__ __forceinline__ double disc(int k) { return 1.0 / log2((double)(k + 2)); }
 
@@ -322,10 +323,15 @@ extern "C" int nar_eval_metrics_lists(const int64_t* ids, int64_t row_stride, in
   if (m < 2) return NAR_ERR_INVALID;                      // the reference divides by an empty sum below two items
   if (m > MAX_M || nq > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
   const size_t smem = sizeof(double) * m * m + sizeof(float) * m * acr_dim;
-  if (smem > 200 * 1024) return NAR_ERR_UNSUPPORTED;
+  if (smem > MAX_LIST_SMEM) return NAR_ERR_UNSUPPORTED;
   if (nq == 0 || (row_mask & ((1LL << rows) - 1)) == 0) return NAR_OK;
-  if (smem > 48 * 1024)
-    NAR_CHECK_CUDA(cudaFuncSetAttribute(list_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // the kernel's static arrays count against the 48 KB a launch gets without opting in, so a dynamic size just below
+  // 48 KB needs the attribute too: raise it once to the cap
+  static bool attr = false;
+  if (!attr) {
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(list_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MAX_LIST_SMEM));
+    attr = true;
+  }
   ListArgs a;
   a.ids = ids; a.row_stride = row_stride; a.q_stride = q_stride; a.nq = nq; a.len = len; a.m = (int)m;
   a.labels = labels; a.label_stride = label_stride;

@@ -23,6 +23,7 @@ from ._lib import check
 KEYS = ('ndcg_at_n', 'esi-r_at_n', 'esi-rr_at_n', 'content_eild-r_at_n', 'content_eild-rr_at_n')
 COVERAGE_KEY = 'item_coverage_at_n'
 MAX_TOP_N = 64             # list positions the kernel scores per query
+MAX_LIST_SMEM = 200 * 1024 # the list kernel's shared memory per query: top_n^2 fp64 distances, top_n fp32 ACR rows
 _N_VALUES = 6              # accumulator columns: the five sums of KEYS, then the query count
 
 
@@ -52,6 +53,10 @@ class EvalMetrics:
     def __init__(self, rows: int, num_items: int, acr: torch.Tensor, acr_dim: int, top_n: int, neg_relevance: float,
                  acr_norm: Optional[torch.Tensor] = None, err: Optional[torch.Tensor] = None):
         check_params(top_n, neg_relevance)
+        smem = 8 * int(top_n) ** 2 + 4 * int(top_n) * int(acr_dim)
+        if smem > MAX_LIST_SMEM:
+            raise ValueError('eval_extended_metrics holds top_n ACR rows per query in %d bytes of shared memory; top_n %d '
+                             'with acr_dim %d needs %d' % (MAX_LIST_SMEM, int(top_n), int(acr_dim), smem))
         self.rows, self.num_items, self.top_n = int(rows), int(num_items), int(top_n)
         self.neg_relevance = float(neg_relevance)
         self.acr, self.acr_dim = acr, int(acr_dim)
