@@ -15,7 +15,8 @@ Two jobs:
    variable name, logical shape, initialiser, L2 flag, and its slot in ONE flat fp32
    buffer (params / grads / adam_m / adam_v share offsets).  L2-regularised tensors come
    first so the optimiser kernel can apply ``reg_l2 * w`` by index range.  Padded
-   rows/cols (H=255 -> 256, F -> multiple of 4) hold zeros and provably stay zero.
+   rows/cols (H -> the next of 32, 64, ..., 1024, e.g. 255 -> 256 and 300 -> 512; F -> multiple of 4) hold zeros and
+   provably stay zero.
 """
 from __future__ import annotations
 
@@ -183,6 +184,9 @@ INIT_LECUN_UNIFORM = 'lecun_uniform'   # tf.initializers.lecun_uniform: U(+-sqrt
 INIT_ZEROS = 'zeros'
 INIT_ONES = 'ones'
 
+# padded hidden sizes Hp the session-cell recurrence kernels accept (csrc/rnn.cu shape_ok)
+HP_SIZES = (32, 64, 128, 256, 512, 1024)
+
 
 @dataclass
 class ParamTensor:
@@ -216,7 +220,10 @@ class ParamLayout:
         H = int(rnn_units)
         self.C, self.H, self.layers = C, H, int(rnn_num_layers)
         self.Cp = round_up(C, 4)
-        self.Hp = round_up(H, 4)
+        # the recurrence kernels (csrc/rnn.cu) run Hp = 32, 64, ..., 1024: the state is padded to the smallest of those
+        if not 1 <= H <= HP_SIZES[-1]:
+            raise ValueError('rnn_units=%d: must be in [1, %d]' % (H, HP_SIZES[-1]))
+        self.Hp = min(s for s in HP_SIZES if s >= H)
         if self.Cp != C:
             raise ValueError('CAR_embedding_size must be a multiple of 4')
         Hp = self.Hp

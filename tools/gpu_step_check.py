@@ -54,8 +54,34 @@ def rel(a, b):
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)) if a.size else 0.0
 
 
+def engine_kinks(lasts, session_size, T, n_cand):
+    """The engine's leaky_relu slope choices for NarOracle's kink alignment, from the ``last`` intermediates of one step
+    (or of the data-parallel shards of one step, in rank order: their positions follow each other session-major)."""
+    valid = np.arange(T)[None, :] < np.clip(np.asarray(session_size) - 1, 0, T)[:, None]
+    ins, cands, f1, zs = [], [], [], {}
+    for last in lasts:
+        L = last['F1'].shape[0]
+        H1 = last['H1'].cpu().numpy() > 0
+        ins.append(H1[:L]); cands.append(H1[L:].reshape(L, n_cand, -1)); f1.append(last['F1'].cpu().numpy() > 0)
+        for zn in ('Z1', 'Z2', 'Z3'):
+            if zn in last:
+                zs.setdefault(zn, []).append((last[zn].cpu().numpy() > 0).reshape(L, n_cand, -1))
+    Hc = np.concatenate(cands)
+    kinks = {'valid': torch.as_tensor(valid), 'h1_in': np.concatenate(ins), 'h1_pos': Hc[:, 0], 'h1_neg': Hc[:, 1:],
+             'f1': np.concatenate(f1)}
+    for zn, parts in zs.items():
+        Z = np.concatenate(parts)
+        kinks[zn.lower() + '_pos'] = Z[:, 0]
+        kinks[zn.lower() + '_neg'] = Z[:, 1:]
+    return kinks
+
+
 def run_case(name, profile, warm, n_steps, hp_over=None, oracle_dtype=torch.float64, sync_state=True, engine_kw=None,
-             align_kinks=True, **mk):
+             align_kinks=True, raw=False, batch_map=None, **mk):
+    """``raw``: every step also starts the engine's outputs (gradients, loss accumulators, step workspace) from NaN and
+    hands back, under r['raw'], the flat buffers around the step (params / adam_m / adam_v before and after the optimiser,
+    the gradient), the logical gradients of both sides and the loss parts.  ``batch_map(feats, labels)`` -> (feats,
+    labels) rewrites every batch before either side sees it."""
     pb = make_problem(name, profile=profile, **(hp_over or {}), **mk)
     hp = pb.hp
     if warm:
@@ -70,13 +96,23 @@ def run_case(name, profile, warm, n_steps, hp_over=None, oracle_dtype=torch.floa
     res = {'case': name, 'profile': profile, 'warm': warm, 'ranking': hp.ranking, 'layers': hp.rnn_num_layers, 'steps': []}
     for step in range(1, n_steps + 1):
         feats, labels = it.get_next()
+        if batch_map is not None:
+            feats, labels = batch_map(feats, labels)
         if sync_state and step > 1:
             # per-step parity: start every step from the oracle's exact state (weights + Adam slots)
             eng.load_logical_state(orc.get_params(), {k: v.numpy() for k, v in orc.adam_m.items()},
                                    {k: v.numpy() for k, v in orc.adam_v.items()}, orc.step)
         buf = pb.clicked_items_state.get_recent_clicks_buffer().copy()
         pop = pb.clicked_items_state.get_articles_recent_pop_norm().copy()
-        out = eng.train_step(feats, labels, buf, pop, keep=True)
+        st = eng.stage(feats, labels, buf, pop)
+        if raw:
+            before = [t.detach().cpu().numpy().copy() for t in (eng.params, eng.adam_m, eng.adam_v)]
+            t_adam = eng.global_step + 1
+            eng.prepare(st, t_adam)                              # sizes the step workspace (submit then runs the step on it)
+            eng.grads.fill_(float('nan')); eng.loss_dev.fill_(float('nan'))
+            eng._ws.fill_(0xFF)                                   # every float of the step workspace a NaN
+            w_ref = {k: v.detach().clone() for k, v in orc.params.items()}
+        out = eng.result(eng.submit(st, keep=True))
         st = out['stage']
         B, T, L = st['B'], st['T'], st['L']
         neg_gpu = out['negatives'].cpu().numpy()
@@ -86,18 +122,7 @@ def run_case(name, profile, warm, n_steps, hp_over=None, oracle_dtype=torch.floa
         last = eng.last
         n_cand = K + 1
         # kink alignment (see NarOracle._dense): the oracle differentiates leaky_relu with the ENGINE's slope choices
-        kinks = None
-        if align_kinks and L > 0:
-            valid = np.arange(T)[None, :] < np.clip(np.asarray(feats['session_size']) - 1, 0, T)[:, None]
-            H1 = last['H1'].cpu().numpy() > 0
-            Hc = H1[L:].reshape(L, n_cand, -1)
-            kinks = {'valid': torch.as_tensor(valid), 'h1_in': H1[:L], 'h1_pos': Hc[:, 0], 'h1_neg': Hc[:, 1:],
-                     'f1': last['F1'].cpu().numpy() > 0}
-            for zn in ('Z1', 'Z2', 'Z3'):
-                if zn in last:
-                    Z = (last[zn].cpu().numpy() > 0).reshape(L, n_cand, -1)
-                    kinks[zn.lower() + '_pos'] = Z[:, 0]
-                    kinks[zn.lower() + '_neg'] = Z[:, 1:]
+        kinks = engine_kinks([last], feats['session_size'], T, n_cand) if align_kinks and L > 0 else None
         o, grads = orc.train_step(feats, labels, neg_ref, buf, pop, kinks=kinks)
         mask = o['mask'].numpy()
         r = {'step': step, 'B': B, 'T': T, 'L': L, 'neg_equal': bool(np.array_equal(neg_gpu, neg_ref))}
@@ -157,6 +182,20 @@ def run_case(name, profile, warm, n_steps, hp_over=None, oracle_dtype=torch.floa
                 du = (p_gpu[k] - params_before[k])[big]; dr = (p_ref[k] - params_before[k])[big]
                 upd.append(float(np.abs(du - dr).max() / hp.learning_rate))
         r['update_err_over_lr'] = max(upd) if upd else 0.0
+        if raw:
+            g_ref = {}
+            for k, g in grads.items():
+                g = g.detach()
+                if orc.reg > 0 and orc.regularised(k):
+                    g = g - orc.reg * w_ref[k]            # the same fp64 product autograd formed: exact where only L2 acts
+                g_ref[k] = g.numpy().astype(np.float64)
+            after = [t.detach().cpu().numpy().copy() for t in (eng.params, eng.adam_m, eng.adam_v)]
+            r['raw'] = {'grads': g_gpu, 'grads_ref': g_ref, 'flat_grads': eng.grads.detach().cpu().numpy().copy(),
+                        'before': before, 'after': after, 't': t_adam, 'applied': eng.global_step == t_adam,
+                        'loss': [out['xe_loss'], out['reg_loss'], out['nov_reg_loss']],
+                        'loss_ref': [float(o['xe_loss']), float(o['reg_loss']), float(o['nov_reg_loss'])],
+                        'logits': lg, 'logits_ref': lg_ref}
+            res['layout'], res['hp'], res['regularised'] = pb.layout, hp, orc.regularised
         res['steps'].append(r)
         # host state update (hook.after_run)
         pb.clicked_items_state.update_from_batch(feats['item_clicked'], feats['event_timestamp'], labels['label_last_item'])
