@@ -89,7 +89,7 @@ class GemmEpilogue(C.Structure):
                 ('precision', C.c_int32), ('b_lo', C.c_void_p), ('b_bf16', C.c_void_p), ('ld_bf16', C.c_int64),
                 ('a_scale', C.c_void_p), ('ld_a_scale', C.c_int64), ('a_scale_group', C.c_int64),
                 ('pred', C.c_void_p), ('d_pred', C.c_void_p), ('ld_pred', C.c_int64), ('pred_group', C.c_int64),
-                ('car_pp', C.c_void_p), ('car_pc', C.c_void_p), ('car_pi', C.c_void_p), ('car_pos_idx', C.c_void_p),
+                ('d_bias', C.c_void_p), ('car_pp', C.c_void_p), ('car_pc', C.c_void_p), ('car_pi', C.c_void_p), ('car_pos_idx', C.c_void_p),
                 ('car_neg_uidx', C.c_void_p), ('car_dpp', C.c_void_p), ('car_dpc', C.c_void_p), ('car_dpi', C.c_void_p),
                 ('ld_car', C.c_int64), ('car_k', C.c_int64)]
 

@@ -269,12 +269,13 @@ struct Seq {
     chk(nar_gemm_tf32_dt(e->ctx, n_out, n_in, rows, dY, lddy, 0, XT, ldxt, 1, G(off_W), ldw, &ep, st));
   }
   // through the scorer product and the CAR tanh: v = dY W^T; dX[r] = v[r] * pred[r / group] * tanh'(cand[r]) and
-  // dpred[l] = sum over position l's rows of v * cand (nar_mul_pred_bwd's arithmetic)
+  // dpred[l] = sum over position l's rows of v * cand (nar_mul_pred_bwd's arithmetic); the column sums of dX are added
+  // to the gradient of the bias at off_b (the bias of the layer that produced cand)
   void dgrad_prod(const float* dY, int64_t lddy, int64_t off_W, int64_t ldw, const float* cand, const float* pred, int64_t group,
-                  float* dX, float* dpred, int64_t M, int64_t n_in, int64_t n_out, cudaStream_t st) {
+                  float* dX, float* dpred, int64_t off_b, int64_t M, int64_t n_in, int64_t n_out, cudaStream_t st) {
     nar_gemm_epilogue ep; memset(&ep, 0, sizeof(ep));
     ep.dact = NAR_ACT_TANH; ep.aux = cand; ep.ld_aux = n_in; ep.split_k = 1; ep.precision = c.bwd_precision;
-    ep.pred = pred; ep.d_pred = dpred; ep.ld_pred = n_in; ep.pred_group = group;
+    ep.pred = pred; ep.d_pred = dpred; ep.ld_pred = n_in; ep.pred_group = group; ep.d_bias = G(off_b);
     chk(nar_gemm_tf32(e->ctx, M, n_in, n_out, dY, lddy, 1, W(off_W), ldw, 1, dX, n_in, &ep, st));
   }
   // through CAR layer 1 of the candidate rows (dedup): v = dY W^T is the gradient of H1c = leaky(pre) (nar_car_combine);
@@ -424,9 +425,11 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
       else s.wgrad(sb.PD, C, sb.dZ1, 128, c.off_M[0], c.ld_M[0], C, 128, Rc, st);
       s.bgrad(sb.dZ1, 128, Rc, 128, c.off_c[0], st);
     }
-    // candidate rows: through the product and the CAR tanh in one pass; d(pred) reduced over the candidates
+    // candidate rows: through the product and the CAR tanh in one pass; d(pred) reduced over the candidates, and the
+    // candidate rows' share of the layer-2 bias gradient summed from the dEc the epilogue writes (red.add into the
+    // gradient buffer, which the memset at the top of the step zeroed earlier on this stream)
     if (fused) {
-      s.dgrad_prod(sb.dZ1, 128, c.off_M[0], c.ld_M[0], Ec, sb.PR, n_cand, dEc, sb.dPR, Rc, C, 128, main);
+      s.dgrad_prod(sb.dZ1, 128, c.off_M[0], c.ld_M[0], Ec, sb.PR, n_cand, dEc, sb.dPR, c.off_b2, Rc, C, 128, main);
     } else {
       s.dgrad(sb.dZ1, 128, c.off_M[0], c.ld_M[0], sb.dPD, C, Rc, C, 128, NAR_ACT_NONE, nullptr, 0, 0, main);
       s.chk(nar_mul_pred_bwd(sb.dPD, Ec, sb.PR, L, n_cand, C, NAR_ACT_TANH, dEc, sb.dPR, main));
@@ -443,7 +446,7 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
     cudaStream_t st = s.fork();
     if (c.dedup) s.wgrad_xt(sb.H1cT, sb.ldr, dEc, C, c.off_W2, C, C, C, Rc, st);
     else s.wgrad(H1c, C, dEc, C, c.off_W2, C, C, C, Rc, st);
-    s.bgrad(dEc, C, Rc, C, c.off_b2, st);
+    if (!fused) s.bgrad(dEc, C, Rc, C, c.off_b2, st);            // fused: summed in dgrad_prod's epilogue
   }
   // ---- S
   {
@@ -833,7 +836,7 @@ extern "C" int nar_engine_buffer(const nar_engine* e, const nar_step_io* io, con
       {"row_pos", pb.row_pos, R, 1}, {"row_item", pb.row_item, R, 1}, {"base_pos", pb.base_pos, NB, 1},
       {"base_item", pb.base_item, NB, 1},
       {"X", sb.X, c.dedup ? NB : R, c.Fp}, {"dX", sb.dX, c.dedup ? NB : R, c.Fp}, {"H1", sb.H1, R, c.C}, {"H1cT", sb.H1cT, c.C, sb.ldr}, {"E", sb.E, R, c.C},
-      {"dE", sb.dE, R, c.C}, {"dH1", sb.dH1, R, c.C}, {"F1", sb.F1, L, 512}, {"PR", sb.PR, L, c.C},
+      {"dE", sb.dE, R, c.C}, {"dPR", sb.dPR, L, c.C}, {"dH1", sb.dH1, R, c.C}, {"F1", sb.F1, L, 512}, {"PR", sb.PR, L, c.C},
       {"logits", sb.logits, L, n_cand}, {"PD", sb.PD, Rc, c.C}, {"Z1", sb.Z1, Rc, 128}, {"Z2", sb.Z2, Rc, 64}, {"Z3", sb.Z3, Rc, 32}, {"PP", sb.PP, L, c.C},
       {"PI", sb.PI, pb.U, c.C}, {"PC", sb.PC, L, c.C}, {"DB", sb.DB, 3 * L + pb.U, c.C},
       {"HO0", sb.HO[0], L, c.Hp}, {"HO1", sb.HO[1], L, c.Hp}, {"HO2", sb.HO[2], L, c.Hp}, {"HO3", sb.HO[3], L, c.Hp},

@@ -32,7 +32,8 @@
 //           128-byte swizzle row, so ONE K-major TMA box brings both halves and no transpose pass is needed.
 // The scorer's product PD = Ec * PR[position] (nar_model.py:478, :493) never reaches HBM: its Dense layer's forward and
 // weight gradient scale A by PR where the fragment is built (EXT_SCALE_*), and its dgrad derives dEc and dPR in an
-// epilogue over position-aligned M tiles (EXT_PROD_BWD).
+// epilogue over position-aligned M tiles (EXT_PROD_BWD), optionally with the column sums of dEc (the gradient of the
+// bias of the layer that produced Ec).
 #include "common.cuh"
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -54,7 +55,7 @@ constexpr int EPI_LD = BN + 4;               // floats per staged accumulator ro
 //                   A needs the scale rows of the tile's row groups (at most SC_ROWS_K) x 32 k, an MN-major A those of
 //                   the k-tile's k groups (at most SC_ROWS_MN) x 128 m; SC_BYTES per stage either way
 //   EXT_SCALE_GMEM  A scale read from global memory at the fragment: any group size (those whose slices do not fit)
-//   EXT_PROD_BWD    scorer-product backward epilogue (nar_gemm_epilogue.pred): position-aligned M tiles
+//   EXT_PROD_BWD    scorer-product backward epilogue (nar_gemm_epilogue.pred, .d_bias): position-aligned M tiles
 //   EXT_CAR_BWD     CAR layer-1 backward epilogue (nar_gemm_epilogue.car_*): the gradients of PP / PC / PI, no D
 //                   (TF32 or 3xTF32 with B split in-kernel, K-major operands)
 //   EXT_TRANS_D     D written transposed, D[n * ldd + m] (nar_gemm_tf32_dt): a weight gradient computed as
@@ -95,8 +96,9 @@ struct Params {
   int n_tiles;                 // blockIdx.x = m_blk * n_tiles + n_blk (N fastest: CTAs sharing an A tile run together)
   // A scale (EXT_SCALE_*): A's storage is [a_rows, a_cols]; storage row i uses scale row i / group
   const float* a_scale; int64_t ld_a_scale, a_rows, a_cols; uint32_t group;
-  // EXT_PROD_BWD: M tile m_blk = positions [m_blk * pos_per_tile, ...), `group` rows each, n_pos positions in all
-  const float* pred; float* d_pred; int64_t ld_pred, n_pos; int pos_per_tile;
+  // EXT_PROD_BWD: M tile m_blk = positions [m_blk * pos_per_tile, ...), `group` rows each, n_pos positions in all;
+  // d_bias (optional): += the column sums of D
+  const float* pred; float* d_pred; float* d_bias; int64_t ld_pred, n_pos; int pos_per_tile;
   // EXT_CAR_BWD: row r = slot r % (car_k + 1) of position r / (car_k + 1); [L | L | U, ld_car] pre-activation parts and
   // their gradients
   const float *car_pp, *car_pc, *car_pi; const int32_t *car_pos_idx, *car_neg_uidx;
@@ -346,37 +348,104 @@ __device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
   return v;
 }
 
-// EXT_PROD_BWD epilogue: `stage` holds v = dL/d(prod) of the tile's rows; thread = (position, column), walking the
-// position's rows in order so that d_pred is the same fmaf chain as nar_mul_pred_bwd's
-__device__ __forceinline__ void prod_bwd_epilogue(const Params& p, const float* stage, int m_blk, int n_blk, int tid) {
-  const int P = p.pos_per_tile, g = (int)p.group;
-  for (int idx = tid; idx < P * BN; idx += NUM_THREADS) {
-    const int pl = idx / BN, c = idx % BN;
-    const int64_t pos = (int64_t)m_blk * P + pl, col = (int64_t)n_blk * BN + c;
-    if (pos >= p.n_pos || col >= p.N) continue;
-    const float pr = __ldg(p.pred + pos * p.ld_pred + col);
-    const float* v = stage + pl * g * EPI_LD + c;
-    const float* e = p.aux + pos * g * p.ld_aux + col;
-    float* d = p.D + pos * g * p.ldd + col;
-    float acc = 0.f;
-    int j = 0;
-    for (; j + 8 <= g; j += 8) {      // eight rows of aux in flight, then the dependent chain in row order
-      float ev[8];
+// four consecutive floats of a row, `nc` of them valid (zeros past them): one 16-byte load when the row is aligned
+__device__ __forceinline__ float4 load4(const float* q, int nc, bool v4) {
+  if (v4 && nc == 4) return *reinterpret_cast<const float4*>(q);
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (nc > 0) v.x = q[0];
+  if (nc > 1) v.y = q[1];
+  if (nc > 2) v.z = q[2];
+  if (nc > 3) v.w = q[3];
+  return v;
+}
+// (a float4 store next to the scalar stores of a partial group is split into four by the compiler)
+__device__ __forceinline__ void st_global_v4(float* q, const float4& v) {
+  asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(q), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
+// EXT_PROD_BWD epilogue: `stage` holds v = dL/d(prod) of the tile's rows.  EC_ROWS rows of Ec fit behind it in the
+// operand ring, so the tile is processed in chunks of whole positions (or, for a position longer than EC_ROWS, in
+// chunks of one position's rows), each in two phases:
+//   elementwise  thread = (row, 4 columns), all rows of the chunk in flight at once: dEc = v * pr * act'(Ec) with
+//                16-byte loads and stores, Ec copied into shared memory, and dEc added to the thread's column sums;
+//   chain        thread = (position, column): d_pred = fmaf(v, Ec, d_pred) over the position's rows in row order from
+//                shared memory - the same chain as nar_mul_pred_bwd's (carried across chunks in `chain`).
+// d_bias: the eight warps' column sums (each over its rows in order) added in a fixed tree, one red.add per column.
+template <int EC_ROWS>
+__device__ __forceinline__ void prod_bwd_epilogue(const Params& p, float* stage, int m_blk, int n_blk, int tid) {
+  constexpr int RQ = (EC_ROWS + 7) / 8;                       // rows per thread and chunk
+  static_assert(EC_ROWS >= 8, "the eight warps' column sums reuse the Ec rows");
+  const int g = (int)p.group;
+  const int64_t pos0 = (int64_t)m_blk * p.pos_per_tile, row0 = pos0 * g;
+  const int n_pos = (int)min((int64_t)p.pos_per_tile, p.n_pos - pos0);
+  const int warp = tid >> 5, c4 = (tid & 31) * 4;
+  const int64_t col = (int64_t)n_blk * BN + c4;
+  const int nc = (int)min((int64_t)4, p.N - col);             // valid columns of the thread's group (<= 0: none)
+  const bool aux_v4 = ((reinterpret_cast<uintptr_t>(p.aux) | (uintptr_t)p.ld_aux * 4) & 15) == 0;
+  const bool pred_v4 = ((reinterpret_cast<uintptr_t>(p.pred) | (uintptr_t)p.ld_pred * 4) & 15) == 0;
+  float* ec = stage + BM * EPI_LD;                            // [EC_ROWS, BN]: Ec of the chunk's rows
+  const int pc = g <= EC_ROWS ? EC_ROWS / g : 1;              // positions per chunk
+  float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
+  float chain = 0.f;
+  for (int pb = 0; pb < n_pos; pb += pc) {
+    const int np = min(pc, n_pos - pb), pr_end = (pb + np) * g;
+    for (int r0 = pb * g; r0 < pr_end; r0 += EC_ROWS) {       // chunk: tile rows [r0, r1)
+      const int r1 = min(r0 + EC_ROWS, pr_end);
+      if (nc > 0) {
+        float4 ev[RQ], pv[RQ];
 #pragma unroll
-      for (int u = 0; u < 8; ++u) ev[u] = e[(j + u) * p.ld_aux];
+        for (int q = 0; q < RQ; ++q) {
+          const int r = r0 + warp + 8 * q;
+          if (r < r1) {
+            ev[q] = load4(p.aux + (row0 + r) * p.ld_aux + col, nc, aux_v4);
+            pv[q] = load4(p.pred + (pos0 + r / g) * p.ld_pred + col, nc, pred_v4);
+          }
+        }
 #pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const float x = v[(j + u) * EPI_LD];
-        d[(j + u) * p.ldd] = x * pr * act_grad_from_output(ev[u], p.dact);
-        acc = fmaf(x, ev[u], acc);
+        for (int q = 0; q < RQ; ++q) {
+          const int r = r0 + warp + 8 * q;
+          if (r < r1) {
+            const float4 x = *reinterpret_cast<const float4*>(stage + r * EPI_LD + c4);
+            const float4 e = ev[q], pr = pv[q];
+            const float4 d = make_float4(x.x * pr.x * act_grad_from_output(e.x, p.dact), x.y * pr.y * act_grad_from_output(e.y, p.dact),
+                                         x.z * pr.z * act_grad_from_output(e.z, p.dact), x.w * pr.w * act_grad_from_output(e.w, p.dact));
+            float* dst = p.D + (row0 + r) * p.ldd + col;
+            if (nc == 4) {
+              st_global_v4(dst, d);
+            } else {
+              dst[0] = d.x;
+              if (nc > 1) dst[1] = d.y;
+              if (nc > 2) dst[2] = d.z;
+            }
+            *reinterpret_cast<float4*>(ec + (r - r0) * BN + c4) = e;
+            bsum.x += d.x; bsum.y += d.y; bsum.z += d.z; bsum.w += d.w;
+          }
+        }
       }
+      __syncthreads();                // the chain reads other threads' rows of Ec
+      for (int idx = tid; idx < np * BN; idx += NUM_THREADS) {
+        const int pl = pb + idx / BN, c = idx % BN;
+        const int64_t colc = (int64_t)n_blk * BN + c;
+        if (colc >= p.N) continue;
+        const int beg = max(pl * g, r0), end = min((pl + 1) * g, r1);
+        float acc = beg == pl * g ? 0.f : chain;
+#pragma unroll 8
+        for (int r = beg; r < end; ++r) acc = fmaf(stage[r * EPI_LD + c], ec[(r - r0) * BN + c], acc);
+        if (end == (pl + 1) * g) p.d_pred[(pos0 + pl) * p.ld_pred + colc] = acc;
+        else chain = acc;             // only when g > EC_ROWS: one position per chunk, thread = column
+      }
+      __syncthreads();                // the next chunk overwrites Ec
     }
-    for (; j < g; ++j) {
-      const float x = v[j * EPI_LD], ej = e[j * p.ld_aux];
-      d[j * p.ldd] = x * pr * act_grad_from_output(ej, p.dact);
-      acc = fmaf(x, ej, acc);
+  }
+  if (p.d_bias) {
+    float* part = ec;                 // [8 warps, BN]
+    *reinterpret_cast<float4*>(part + warp * BN + c4) = bsum;
+    __syncthreads();
+    if (tid < BN && (int64_t)n_blk * BN + tid < p.N) {
+      const float* s = part + tid;
+      const float t = ((s[0] + s[BN]) + (s[2 * BN] + s[3 * BN])) + ((s[4 * BN] + s[5 * BN]) + (s[6 * BN] + s[7 * BN]));
+      atomicAdd(p.d_bias + (int64_t)n_blk * BN + tid, t);      // red.global.add.f32
     }
-    p.d_pred[pos * p.ld_pred + col] = acc;
   }
 }
 
@@ -705,8 +774,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
   }
   __syncthreads();
-  if (PROD_BWD) {
-    prod_bwd_epilogue(p, stage, m_blk, n_blk, tid);
+  if (PROD_BWD) {                     // Ec rows of a chunk in the rest of the operand ring (60 at 3 stages of 32 KB)
+    prod_bwd_epilogue<(C::STAGES * C::STAGE_BYTES - BM * EPI_LD * 4) / (BN * 4)>(p, stage, m_blk, n_blk, tid);
     return;
   }
   if (CAR_BWD) {
@@ -915,7 +984,7 @@ static int gemm(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, i
     const int64_t g = epi->pred_group;
     if (mode != 0 || !a_kmajor || !b_kmajor || epi->accumulate || epi->split_k > 1 || epi->bias || epi->act) return NAR_ERR_INVALID;
     if (g < 1 || g > BM || M % g != 0 || !epi->d_pred || !epi->aux || epi->ld_aux < N || epi->ld_pred < N) return NAR_ERR_INVALID;
-  } else if (epi->d_pred || epi->pred_group != 0 || epi->ld_pred != 0) {
+  } else if (epi->d_pred || epi->pred_group != 0 || epi->ld_pred != 0 || epi->d_bias) {
     return NAR_ERR_INVALID;
   }
   if (car_bwd) {
@@ -970,7 +1039,7 @@ static int gemm(nar_ctx* ctx, int64_t M, int64_t N, int64_t K, const float* A, i
   p.n_tiles = (int)n_tiles;
   p.a_scale = epi->a_scale; p.ld_a_scale = epi->ld_a_scale; p.a_rows = a_rows; p.a_cols = a_cols;
   p.group = (uint32_t)(scale ? epi->a_scale_group : (prod_bwd ? epi->pred_group : 1));
-  p.pred = epi->pred; p.d_pred = epi->d_pred; p.ld_pred = epi->ld_pred; p.n_pos = n_pos; p.pos_per_tile = (int)pos_per_tile;
+  p.pred = epi->pred; p.d_pred = epi->d_pred; p.d_bias = epi->d_bias; p.ld_pred = epi->ld_pred; p.n_pos = n_pos; p.pos_per_tile = (int)pos_per_tile;
   p.car_pp = epi->car_pp; p.car_pc = epi->car_pc; p.car_pi = epi->car_pi; p.car_pos_idx = epi->car_pos_idx;
   p.car_neg_uidx = epi->car_neg_uidx; p.car_dpp = epi->car_dpp; p.car_dpc = epi->car_dpc; p.car_dpi = epi->car_dpi;
   p.ld_car = epi->ld_car; p.car_k = (int)epi->car_k;

@@ -64,20 +64,21 @@ def _chk_f32(*ts):
 def gemm(A: torch.Tensor, B: torch.Tensor, D: torch.Tensor, M: int, N: int, K: int, *, a_kmajor=True, b_kmajor=True,
          lda=None, ldb=None, ldd=None, bias=None, act=ACT_NONE, dact=ACT_NONE, aux=None, ld_aux=None,
          accumulate=False, split_k=1, precision=3, b_lo=None, b_bf16=None, ld_bf16=0, a_scale=None, a_scale_group=0,
-         pred=None, d_pred=None, pred_group=0, car=None, trans_d=False):
+         pred=None, d_pred=None, pred_group=0, d_bias=None, car=None, trans_d=False):
     global LAUNCHES
     LAUNCHES += 1
     """D[M,N] = epilogue(sum_k A(m,k) B(n,k)); see nar_gemm_tf32.  a_scale / pred / d_pred: row strides from the tensors.
+    d_bias: += the column sums of D (with pred only).
     car: dict(pp, pc, pi, pos_idx, neg_uidx, dpp, dpc, dpi, k) for the CAR layer-1 backward epilogue (D = None; ld_car from
     pp).  trans_d: D stored transposed, D[n*ldd + m] (nar_gemm_tf32_dt)."""
-    _chk_f32(A, B, D, bias, aux, a_scale, pred, d_pred)
+    _chk_f32(A, B, D, bias, aux, a_scale, pred, d_pred, d_bias)
     lda = A.stride(0) if lda is None else lda
     ldb = (B.stride(0) if B is not None else 0) if ldb is None else ldb
     ldd = (D.stride(0) if D is not None else 0) if ldd is None else ldd
     epi = GemmEpilogue(_p(bias), act, dact, _p(aux), (aux.stride(0) if (aux is not None and ld_aux is None) else (ld_aux or 0)),
                        1 if accumulate else 0, int(split_k), int(precision), _p(b_lo), _p(b_bf16), int(ld_bf16),
                        _p(a_scale), a_scale.stride(0) if a_scale is not None else 0, int(a_scale_group),
-                       _p(pred), _p(d_pred), pred.stride(0) if pred is not None else 0, int(pred_group))
+                       _p(pred), _p(d_pred), pred.stride(0) if pred is not None else 0, int(pred_group), _p(d_bias))
     if car is not None:
         _chk_f32(car['pp'], car['pc'], car['pi'], car['dpp'], car['dpc'], car['dpi'])
         assert car['pos_idx'].dtype == torch.int32 and car['neg_uidx'].dtype == torch.int32

@@ -190,6 +190,8 @@ typedef struct {
   float* d_pred;
   int64_t ld_pred;        /* row stride of pred and d_pred (>= N) */
   int64_t pred_group;
+  float* d_bias;          /* optional with pred: d_bias[c] += sum over the M rows of D[r, c] (the gradient of a bias added
+                             before dact), float atomics into a buffer the caller owns; rejected without pred.  NULL: none */
   const float* car_pp;    /* optional CAR layer-1 backward epilogue (precision 1, or 3 without b_lo; K-major A and B, no split-K / bias / act /
                              accumulate / aux / a_scale / pred; D must be NULL; N a multiple of 4): row r of the result v is
                              the gradient of H1c[r] = dact(pre) for candidate j = r % (car_k+1) of position l = r / (car_k+1),

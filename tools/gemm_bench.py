@@ -7,7 +7,9 @@ dgrad (single-pass TF32, leaky derivative from a separate aux, and with the CAR 
 instead of a stored dH1) and split-K wgrad (single-pass TF32, both operands
 MN-major, split chosen by the library), and the scorer's first layer
 (C -> 128) forward / dgrad / wgrad, also with the scorer product (51 candidates per position) as separate kernels
-(mul_pred + forward, dgrad + mul_pred_bwd) against folded into the GEMMs (A scaled by PR, product backward epilogue).
+(mul_pred + forward, dgrad + mul_pred_bwd) against folded into the GEMMs (A scaled by PR, product backward epilogue),
+and that epilogue with and without the layer-2 bias column sums next to the nar_colsum_add pass they replace (with the
+rate of its least HBM traffic, one read of Ec and one write of dEc).
 CAR layer 2 also in the form the step runs with the candidate rows stored transposed (H1cT [C, ldr]): the forward with
 an MN-major A, and the weight gradient as dW^T = dE^T H1 (A = dE MN-major, B = H1cT K-major, D stored transposed).  Each step case also reports the share of the data-sheet peak of the tensor path it
 issues on (bf16 for bf16x3, counting its 3 MMAs per product; TF32 otherwise) and the rate at which TMA fills shared
@@ -107,6 +109,7 @@ def step_cases(dev):
     PR = torch.tanh(torch.randn(L, C, device=dev))
     dEc = torch.empty(Rp, C, device=dev)
     dPR = torch.empty(L, C, device=dev)
+    db2 = torch.zeros(C, device=dev)
 
     def mul_pred_fwd():
         ops.mul_pred(Ec, PR, L, n_cand, C, PD)
@@ -144,6 +147,8 @@ def step_cases(dev):
         ('step M1 fwd bf16x3 A scaled by PR', lambda: ops.gemm(Ec, None, Z1, Rp, 128, C, ldb=0, bias=c0, act=ops.ACT_LEAKY, precision=4, b_bf16=M0plane, ld_bf16=M0plane.stride(0), a_scale=PR, a_scale_group=n_cand), [Rp, 128, C], Z1, 4),
         ('step M1 dgrad 1x + mul_pred_bwd', dgrad_mul_pred_bwd, [Rp, C, 128], dEc, 1),
         ('step M1 dgrad 1x product backward epilogue', lambda: ops.gemm(dZ1, M0, dEc, Rp, C, 128, precision=1, dact=ops.ACT_TANH, aux=Ec, pred=PR, d_pred=dPR, pred_group=n_cand), [Rp, C, 128], dEc, 1),
+        ('step M1 dgrad 1x product backward epilogue + layer-2 bias column sums', lambda: ops.gemm(dZ1, M0, dEc, Rp, C, 128, precision=1, dact=ops.ACT_TANH, aux=Ec, pred=PR, d_pred=dPR, pred_group=n_cand, d_bias=db2), [Rp, C, 128], dEc, 1),
+        ('step colsum_add of dEc (layer-2 bias, candidate rows)', lambda: ops.colsum_add(dEc, Rp, C, C, db2), [Rp, C, 0], db2, 0),
         ('step M1 wgrad 1x split-K A scaled by PR', lambda: ops.gemm(Ec, dZ1, dM0, C, 128, Rp, a_kmajor=False, b_kmajor=False, accumulate=True, split_k=0, precision=1, a_scale=PR, a_scale_group=n_cand), [C, 128, Rp], dM0, 1),
     ]
 
@@ -177,7 +182,14 @@ def main():
         if only and only not in name:
             continue
         ms = bench(fn, iters, flush)
-        print(json.dumps({'case': name, 'shape': shape, 'us': ms * 1e3, **step_rates(shape, prec, ms * 1e3)}), flush=True)
+        M, N, K = shape
+        if K == 0:                    # not a GEMM: one read of [M, N] fp32
+            out = {'case': name, 'shape': [M, N], 'us': ms * 1e3, 'hbm_GBps': M * N * 4 / (ms * 1e-3) / 1e9}
+        else:
+            out = {'case': name, 'shape': shape, 'us': ms * 1e3, **step_rates(shape, prec, ms * 1e3)}
+        if 'product backward' in name:            # the least HBM traffic: Ec read once, dEc written once
+            out['ec_dec_GBps'] = 2 * M * N * 4 / (ms * 1e-3) / 1e9
+        print(json.dumps(out), flush=True)
 
 
 if __name__ == '__main__':
