@@ -149,6 +149,8 @@ _SIGNATURES = {
     'nar_engine_recommend_workspace_bytes': (C.c_int, [vp, i64, i64, i64, i32, i64, C.POINTER(i64), C.POINTER(i64),
                                                        C.POINTER(i64)]),
     'nar_engine_recommend': (C.c_int, [vp, C.POINTER(StepIO), vp, vp, i64, vp, i64, i32, i32, i64, i64, vp, vp, vp, vp]),
+    'nar_rank_labels': (C.c_int, [vp, vp, i64, i64, vp, vp, vp, i64, i32, vp, vp, vp]),
+    'nar_engine_rank_labels': (C.c_int, [vp, C.POINTER(StepIO), vp, i64, i32, i64, i64, vp, vp, vp]),
     'nar_host_state_update': (C.c_int, [vp, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, C.c_double]),
     'nar_host_state_update_batch': (C.c_int, [vp, i64, vp, vp, vp, i64, i64, i64, vp, vp, vp, vp, vp, i64, C.c_double]),
     'nar_state_update': (C.c_int, [vp, vp, i64, vp, vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, i64, C.c_double, vp, vp]),

@@ -591,13 +591,14 @@ int64_t rec_plan(const nar_engine* e, int64_t L, int64_t Q, int64_t N, int gathe
   }
 }
 
-int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, const int32_t* q_pos, int64_t Q,
-                  const int64_t* cand_ids, int64_t N, int32_t top_n, int32_t exclude, int64_t qb, int64_t nb, int64_t* out_ids,
-                  float* out_scores, float* out_probs, cudaStream_t main) {
+// Scores every (query, candidate) pair of a recommend call block by block: each finished [Qb, N] logits block of the
+// queries q0 .. q0+Qb-1 goes to finish(logits, q0, Qb) (the top n, or the label ranks of an unsampled evaluation).
+template <class Finish>
+int run_candidate_blocks(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, int64_t Q, const int64_t* cand_ids,
+                         int64_t N, int64_t qb, int64_t nb, cudaStream_t main, Finish finish) {
   const nar_model_cfg& c = e->cfg;
-  const int64_t L = io->L, T = io->T, C = c.C, Fp = c.Fp, c0 = c.ctx_col0;
+  const int64_t L = io->L, C = c.C, Fp = c.Fp, c0 = c.ctx_col0;
   if (L <= 0 || Q <= 0 || Q > L || N <= 0 || qb < 1 || nb < 1 || (c.ranking == 1 && nb > cosine_chunk_cap(c))) return NAR_ERR_INVALID;
-  if (top_n < 1 || top_n > N || top_n > 4096) return NAR_ERR_INVALID;
   if (qb > Q) qb = Q;
   if (nb > N) nb = N;
   const int gather_q = q_rows != nullptr;
@@ -642,11 +643,32 @@ int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, c
         s.chk((int)cudaMemcpy2DAsync(rb.logits + j0, (size_t)N * sizeof(float), lg, (size_t)Nc * sizeof(float),
                                      (size_t)Nc * sizeof(float), (size_t)Qb, cudaMemcpyDeviceToDevice, main));
     }
-    s.chk(nar_topn_candidates(rb.logits, cand_ids, Qb, N, top_n, exclude ? io->item_clicked : nullptr, q_pos + q0, T,
-                              out_ids + q0 * top_n, out_scores ? out_scores + q0 * top_n : nullptr,
-                              out_probs ? out_probs + q0 * top_n : nullptr, main));
+    s.chk(finish(rb.logits, q0, Qb));
   }
   return s.rc;
+}
+
+int run_recommend(nar_engine* e, const nar_step_io* io, const int64_t* q_rows, const int32_t* q_pos, int64_t Q,
+                  const int64_t* cand_ids, int64_t N, int32_t top_n, int32_t exclude, int64_t qb, int64_t nb, int64_t* out_ids,
+                  float* out_scores, float* out_probs, cudaStream_t main) {
+  if (top_n < 1 || top_n > N || top_n > 4096) return NAR_ERR_INVALID;
+  const int64_t T = io->T;
+  return run_candidate_blocks(e, io, q_rows, Q, cand_ids, N, qb, nb, main, [&](const float* logits, int64_t q0, int64_t Qb) {
+    return nar_topn_candidates(logits, cand_ids, Qb, N, top_n, exclude ? io->item_clicked : nullptr, q_pos + q0, T,
+                               out_ids + q0 * top_n, out_scores ? out_scores + q0 * top_n : nullptr,
+                               out_probs ? out_probs + q0 * top_n : nullptr, main);
+  });
+}
+
+// every valid position of the batch is a query (Q = L, q_pos = pos_idx); see nar_engine_rank_labels
+int run_rank_labels(nar_engine* e, const nar_step_io* io, const int64_t* cand_ids, int64_t N, int32_t top_n, int64_t qb,
+                    int64_t nb, int32_t* rank, int64_t* hist, cudaStream_t main) {
+  if (top_n < 1) return NAR_ERR_INVALID;
+  const int64_t T = io->T;
+  const int32_t* q_pos = io->pos_idx;
+  return run_candidate_blocks(e, io, nullptr, io->L, cand_ids, N, qb, nb, main, [&](const float* logits, int64_t q0, int64_t Qb) {
+    return nar_rank_labels(logits, cand_ids, Qb, N, io->label_next, io->all_items, q_pos + q0, T, top_n, rank + q0, hist, main);
+  });
 }
 
 }  // namespace
@@ -818,6 +840,16 @@ extern "C" int nar_engine_recommend(nar_engine* e, const nar_step_io* io, const 
   if (io->train) return NAR_ERR_INVALID;
   return run_recommend(e, io, q_rows, q_pos, Q, cand_ids, N, top_n, exclude_session_clicks, q_block, n_block, out_ids, out_scores,
                        out_probs, as_stream(stream));
+}
+
+extern "C" int nar_engine_rank_labels(nar_engine* e, const nar_step_io* io, const int64_t* cand_ids, int64_t N, int32_t top_n,
+                                      int64_t q_block, int64_t n_block, int32_t* rank, int64_t* hist, void* stream) {
+  if (!e || !io || !io->ws || !io->pos_idx || !cand_ids || !rank || !hist || !io->buffer || !io->pop_norm || !io->item_clicked ||
+      !io->label_next || !io->all_items)
+    return NAR_ERR_INVALID;
+  if (io->train) return NAR_ERR_INVALID;
+  if (io->T + 1 > 1024) return NAR_ERR_UNSUPPORTED;          // the exclusion row of nar_rank_labels
+  return run_rank_labels(e, io, cand_ids, N, top_n, q_block, n_block, rank, hist, as_stream(stream));
 }
 
 extern "C" int64_t nar_engine_launch_count(const nar_engine* e) { return e ? e->launches : 0; }

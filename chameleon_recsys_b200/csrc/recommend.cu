@@ -7,6 +7,8 @@
 //   car_combine_grid_kernel  H1[q*Nc + j] = act(PC[q] + PI[j])  for a block of queries x a chunk of candidates
 //   topn_kernel              per query row of logits [Q, N]: softmax statistics over the non-excluded candidates and an
 //                            exact top n (radix select on order-preserving keys, compaction, bitonic sort of <= 4096)
+//   rank_labels_kernel       per query row of logits [Q, N]: the label's rank among its non-excluded competitors and an
+//                            integer histogram of the ranks below n (unsampled evaluation, DESIGN.md section 13)
 #include "common.cuh"
 
 namespace nar {
@@ -236,6 +238,79 @@ topn_kernel(const float* __restrict__ logits, const int64_t* __restrict__ cand_i
   }
 }
 
+// ------------------------------------------------------------------------------------------------ label rank
+// Unsampled evaluation (NarEngine.rank_labels): per query row of logits [Q, N], the number of competitors whose key is
+// above the label's.  Competitors are the candidates other than the label that are not in the session's row
+// all_items[b, 0..T] (its clicks and its last label); ties go to the label.
+constexpr int RANK_NT = 256;
+constexpr int RANK_WARPS = RANK_NT / 32;
+
+__global__ void __launch_bounds__(RANK_NT)
+rank_labels_kernel(const float* __restrict__ logits, const int64_t* __restrict__ cand_ids, int64_t N,
+                   const int64_t* __restrict__ label_next, const int64_t* __restrict__ all_items,
+                   const int32_t* __restrict__ q_pos, int64_t T, int top_n, int32_t* __restrict__ rank,
+                   unsigned long long* __restrict__ hist) {
+  __shared__ int64_t excl[MAX_EXCL];
+  __shared__ uint32_t bloom[BLOOM_WORDS];
+  __shared__ int red_above[RANK_WARPS], red_comp[RANK_WARPS];
+  __shared__ int64_t s_lab;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int64_t q = blockIdx.x;
+  const int64_t pos = q_pos[q], b = pos / T;
+  const int n_excl = (int)(T + 1);
+  for (int i = tid; i < BLOOM_WORDS; i += RANK_NT) bloom[i] = 0u;
+  if (tid == 0) {                                  // the label's index in the ascending candidate ids, -1 when absent
+    const int64_t id = label_next[pos];
+    int64_t lo = 0, hi = N;
+    while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (cand_ids[mid] < id) lo = mid + 1; else hi = mid; }
+    s_lab = (id != 0 && lo < N && cand_ids[lo] == id) ? lo : -1;
+  }
+  __syncthreads();
+  const int64_t* row = all_items + b * (T + 1);
+  for (int i = tid; i < n_excl; i += RANK_NT) {
+    const int64_t id = row[i];
+    excl[i] = id;
+    const uint32_t h = bloom_slot(id);
+    atomicOr(&bloom[h >> 5], 1u << (h & 31));
+  }
+  __syncthreads();
+  const int64_t lab = s_lab;
+  if (lab < 0) {                                   // a label outside the candidates is not ranked
+    if (tid == 0) rank[q] = -1;
+    return;
+  }
+  const float* lg = logits + q * N;
+  const uint32_t key_lab = order_key(lg[lab]);
+  int above = 0, comp = 0;
+  for (int64_t j = tid; j < N; j += RANK_NT) {
+    if (j == lab) continue;
+    const int64_t id = cand_ids[j];
+    const uint32_t h = bloom_slot(id);
+    if (bloom[h >> 5] & (1u << (h & 31))) {
+      bool hit = false;
+      for (int i = 0; i < n_excl && !hit; ++i) hit = excl[i] == id;
+      if (hit) continue;
+    }
+    ++comp;
+    above += order_key(lg[j]) > key_lab;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    above += __shfl_xor_sync(0xffffffffu, above, o);
+    comp += __shfl_xor_sync(0xffffffffu, comp, o);
+  }
+  if (lane == 0) { red_above[w] = above; red_comp[w] = comp; }
+  __syncthreads();
+  if (tid == 0) {
+    above = 0; comp = 0;
+    for (int i = 0; i < RANK_WARPS; ++i) { above += red_above[i]; comp += red_comp[i]; }
+    rank[q] = above;
+    if (above < top_n) atomicAdd(&hist[above], 1ull);
+    atomicAdd(&hist[top_n], 1ull);
+    atomicAdd(&hist[top_n + 1], (unsigned long long)comp);
+  }
+}
+
 }  // namespace rec
 }  // namespace nar
 
@@ -290,6 +365,19 @@ extern "C" int nar_topn_candidates(const float* logits, const int64_t* cand_ids,
   static_assert(sizeof(nar::rec::TopnShared) <= 48 * 1024, "top-n scratch must fit the default shared-memory window");
   nar::rec::topn_kernel<<<(unsigned)Q, nar::rec::TOPN_NT, smem, as_stream(stream)>>>(
       logits, cand_ids, N, top_n, item_clicked, q_pos, T, out_ids, out_scores, out_probs);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_rank_labels(const float* logits, const int64_t* cand_ids, int64_t Q, int64_t N, const int64_t* label_next,
+                               const int64_t* all_items, const int32_t* q_pos, int64_t T, int32_t top_n, int32_t* rank,
+                               int64_t* hist, void* stream) {
+  if (!logits || !cand_ids || !label_next || !all_items || !q_pos || !rank || !hist) return NAR_ERR_INVALID;
+  if (Q <= 0) return NAR_OK;
+  if (N <= 0 || N > 0x7fffffffLL || T <= 0 || top_n < 1) return NAR_ERR_INVALID;
+  if (T + 1 > nar::rec::MAX_EXCL || Q > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
+  nar::rec::rank_labels_kernel<<<(unsigned)Q, nar::rec::RANK_NT, 0, as_stream(stream)>>>(
+      logits, cand_ids, N, label_next, all_items, q_pos, T, top_n, rank, reinterpret_cast<unsigned long long*>(hist));
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

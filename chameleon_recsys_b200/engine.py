@@ -769,6 +769,63 @@ class NarEngine:
         out['q_block'], out['n_block'] = int(qb.value), int(nb.value)
         return out
 
+    # ---- unsampled evaluation (DESIGN.md section 13): rank each label against every candidate the sampler could draw
+    MAX_RANK_SESSION = 1023           # positions T of a batch: the session row of T + 1 ids is the kernel's exclusion list
+
+    @staticmethod
+    def unsampled_pool(item_clicked, label_last_item, buffer) -> np.ndarray:
+        """The sorted distinct nonzero ids of the batch's clicks, its last labels and the recent-clicks buffer: every id
+        the negative sampler of an EVAL step may draw from (nar_model.py:1220-1304, before the per-session exclusion)."""
+        ids = np.concatenate([np.asarray(a, dtype=np.int64).reshape(-1) for a in (item_clicked, label_last_item, buffer)])
+        return np.unique(ids[ids != 0])
+
+    def rank_labels(self, st: dict, candidates, top_n: int, hist: Optional[torch.Tensor] = None,
+                    ws_budget: Optional[int] = None) -> dict:
+        """Rank the label of every valid position of the EVAL batch staged in ``st`` (eval_step's ``out['stage']``) against
+        ``candidates`` (distinct ids in [1, V), any order; see unsampled_pool), each scored as recommend scores it.  The
+        competitors of a query are the candidates other than its label outside its session's row [item_clicked[b] |
+        label_last_item[b]]; rank = how many of them score above the label (ties go to the label).  ``hist`` [top_n + 2]
+        int64 device accumulator (default: a new zero one): the count of each rank below top_n, the ranked queries and
+        their competitors.  Reads the staged batch, the weights and the state it was staged with; writes nothing else.
+        -> dict(rank [L] int32 device tensor, -1 for a label outside the candidates; hist; candidates (ascending);
+        q_block, n_block)."""
+        if self.world > 1:
+            raise NotImplementedError('the unsampled evaluation runs on one process; data-parallel evaluation is not '
+                                      'implemented')
+        if isinstance(top_n, (bool, np.bool_)) or not isinstance(top_n, (int, np.integer)) or top_n < 1:
+            raise ValueError('top_n must be a positive integer, not %r' % (top_n,))
+        top_n = int(top_n)
+        if st['T'] > self.MAX_RANK_SESSION:
+            raise ValueError('the unsampled evaluation ranks sessions of at most %d positions, not %d'
+                             % (self.MAX_RANK_SESSION, st['T']))
+        L, d = st['L'], self.dev
+        cand = np.sort(self.resolve_candidates(np.asarray(candidates), None)) if L > 0 else np.sort(np.asarray(candidates))
+        N = int(cand.size)
+        if hist is None:
+            hist = torch.zeros(top_n + 2, dtype=torch.int64, device=d)
+        if hist.dtype != torch.int64 or hist.numel() != top_n + 2 or hist.device != d:
+            raise ValueError('hist must be an int64 tensor of top_n + 2 = %d entries on %s' % (top_n + 2, d))
+        rank = torch.empty(max(L, 1), dtype=torch.int32, device=d)[:L]
+        out = {'rank': rank, 'hist': hist, 'candidates': cand, 'q_block': 0, 'n_block': 0}
+        if L == 0:
+            return out
+        budget = int(self._ws_budget if ws_budget is None else ws_budget)
+        wb, qb, nb = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        check(self._lib.nar_engine_recommend_workspace_bytes(self._handle, L, L, N, 0, budget, C.byref(wb), C.byref(qb),
+                                                             C.byref(nb)), 'nar_engine_recommend_workspace_bytes')
+        self._sync_cfg()
+        ws = self._buf('rec_ws', int(wb.value), 1, torch.uint8).view(-1)
+        cand_t = torch.from_numpy(cand).to(d)
+        io = self._staged_io(st)
+        io.L_cap, io.global_step, io.train = L, self.global_step, 0
+        io.ws, io.ws_bytes = ws.data_ptr(), ws.numel()
+        check(self._lib.nar_engine_rank_labels(self._handle, C.byref(io), C.c_void_p(cand_t.data_ptr()), N, top_n,
+                                               int(qb.value), int(nb.value), C.c_void_p(rank.data_ptr()),
+                                               C.c_void_p(hist.data_ptr()), C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+              'nar_engine_rank_labels')
+        out['q_block'], out['n_block'] = int(qb.value), int(nb.value)
+        return out
+
     def train_step(self, features, labels, buffer, pop_norm, keep: bool = False, sync: bool = True) -> dict:
         """Stage, run and apply one training step; ``sync``: wait for it and read its loss (else ``result(out)`` does)."""
         out = self.submit(self.stage(features, labels, buffer, pop_norm), keep=keep)

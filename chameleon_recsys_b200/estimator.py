@@ -104,7 +104,8 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
                                    eval_benchmark_classifiers=params.get('eval_benchmarks') or (),
                                    eval_extended_metrics=bool(params.get('eval_extended_metrics', False)),
                                    eval_metrics_by_session_position=bool(
-                                       params.get('eval_metrics_by_session_position', False)))]
+                                       params.get('eval_metrics_by_session_position', False)),
+                                   eval_unsampled_metrics=bool(params.get('eval_unsampled_metrics', False)))]
     if mode == ModeKeys.TRAIN:
         def train_op(feats, labs, feed, sync=True):
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
@@ -332,7 +333,10 @@ class Estimator:
         ``content_eild-r_at_n`` and ``content_eild-rr_at_n``, and each as ``<key>_<suffix>`` for every baseline.  With
         ``eval_metrics_by_session_position`` also ``hitrate_at_n_by_pos_PP``, ``clicks_at_pos_PP`` and
         ``avg_norm_pop_by_pos_PP`` of the model and ``hitrate_at_n_by_pos_<suffix>_PP`` of every baseline, for each
-        session position PP ('%02d', from 01) that had a query (none without input)."""
+        session position PP ('%02d', from 01) that had a query (none without input).  With ``eval_unsampled_metrics``
+        also ``unsampled_hitrate_at_n``, ``unsampled_mrr_at_n``, ``unsampled_ndcg_at_n`` and
+        ``unsampled_candidates_per_query``: each label ranked against every article the negative sampler could have drawn
+        for it (DESIGN.md section 13; NaN without input)."""
         import torch
         batches = _batches(input_fn(), steps)
         nxt = next(batches, None)
@@ -344,6 +348,9 @@ class Estimator:
                 from .eval_metrics import metric_names
                 for s in [''] + list(parse_classifiers(self.params.get('eval_benchmarks') or ())):
                     empty.update({k: float('nan') for k in metric_names(s)})
+            if self.params.get('eval_unsampled_metrics'):
+                from .eval_metrics import UNSAMPLED_KEYS
+                empty.update({k: float('nan') for k in UNSAMPLED_KEYS})
             return empty
         if self._eval_spec is None:
             self._eval_spec = self.model_fn(nxt[0], nxt[1], ModeKeys.EVAL, self.params)
@@ -378,6 +385,7 @@ class Estimator:
             bench.update(h.benchmark_results())
             bench.update(h.extended_results())
             bench.update(h.by_position_results())
+            bench.update(h.unsampled_results())
             h.end()
         eng = spec.model.engine
         if eng.world > 1:                                           # data parallel: every rank ranked its own sessions

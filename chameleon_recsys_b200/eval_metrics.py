@@ -8,6 +8,9 @@ with ``add_lists`` straight from the device buffers that hold them (the model's 
 
 ``ByPosition`` does the same for the hit rate by session position (the reference's ``HitRateBySessionPosition``, switch
 ``eval_metrics_by_session_position``; DESIGN.md section 11, spec oracle/by_position_ref.py).
+
+``unsampled_results`` turns the integer rank histogram of ``NarEngine.rank_labels`` into the unsampled hit rate, MRR and
+NDCG (switch ``eval_unsampled_metrics``; DESIGN.md section 13, spec oracle/unsampled_ref.py).
 """
 from __future__ import annotations
 
@@ -211,3 +214,24 @@ class ByPosition:
                     out['clicks_at_pos_%02d' % p] = q
                     out['avg_norm_pop_by_pos_%02d' % p] = float(np.float32(norm_pop[t]) / np.float32(q))
         return out
+
+
+# ------------------------------------------------------------------ unsampled hit rate, MRR and NDCG (DESIGN.md section 13)
+UNSAMPLED_KEYS = ('unsampled_hitrate_at_n', 'unsampled_mrr_at_n', 'unsampled_ndcg_at_n', 'unsampled_candidates_per_query')
+
+
+def unsampled_results(hist, top_n: int) -> Dict[str, float]:
+    """The unsampled metrics from the integer accumulator of NarEngine.rank_labels (hist [top_n + 2]: the count of each
+    rank r < top_n, the ranked queries, their competitors), summed in float64 in rank order: the same bits for any blocking
+    and from run to run.  NaN for every key without a query."""
+    h = [int(v) for v in np.asarray(hist, dtype=np.int64).reshape(-1)]
+    n = int(top_n)
+    q = h[n]
+    if q == 0:
+        return {k: float('nan') for k in UNSAMPLED_KEYS}
+    hits = mrr = ndcg = 0.0
+    for r in range(n):
+        hits += float(h[r])
+        mrr += h[r] / (r + 1.0)
+        ndcg += h[r] / float(np.log2(r + 2.0))
+    return dict(zip(UNSAMPLED_KEYS, (hits / q, mrr / q, ndcg / q, h[n + 1] / q)))

@@ -152,6 +152,9 @@ class NARHParams:
     # and mean label popularity per position, in Estimator.evaluate (the reference trainer's flag of the same name,
     # nar_trainer_gcom.py:56; eval_metrics.ByPosition)
     eval_metrics_by_session_position: bool = False
+    # hit rate, MRR and NDCG of each label ranked against every article the negative sampler could have drawn for it, in
+    # Estimator.evaluate (DESIGN.md section 13; NarEngine.rank_labels)
+    eval_unsampled_metrics: bool = False
 
     def to_params(self, session_features_config, articles_features_config, articles_metadata,
                   content_article_embeddings_matrix) -> dict:
@@ -197,6 +200,8 @@ class NARHParams:
             params['eval_benchmarks'] = list(self.eval_benchmarks)
         if self.eval_extended_metrics:           # likewise only when requested
             params['eval_extended_metrics'] = True
+        if self.eval_unsampled_metrics:
+            params['eval_unsampled_metrics'] = True
         return params
 
     def copy(self, **kw) -> 'NARHParams':

@@ -153,7 +153,8 @@ class ItemsStateUpdaterHook:
                  eval_sessions_metrics_log=None, sessions_negative_items_log=None,
                  sessions_chameleon_recommendations_log=None, content_article_embeddings_matrix=None,
                  articles_metadata=None, eval_negative_sample_relevance=None, eval_benchmark_classifiers=(),
-                 eval_metrics_by_session_position=False, eval_cold_start=False, eval_extended_metrics=False):
+                 eval_metrics_by_session_position=False, eval_cold_start=False, eval_extended_metrics=False,
+                 eval_unsampled_metrics=False):
         self.mode = mode
         self.model = model
         self.eval_metrics_top_n = eval_metrics_top_n
@@ -190,6 +191,13 @@ class ItemsStateUpdaterHook:
                 raise NotImplementedError('the hit rate by session position runs on one process; data-parallel '
                                           'evaluation of it is not implemented')
             check_by_position_params(eval_metrics_top_n)
+        # hit rate, MRR and NDCG of each label against every article the negative sampler could have drawn for it
+        # (NarEngine.rank_labels): an int64 rank histogram [top_n + 2] on the device, read once at the end
+        self.unsampled_on = eval_unsampled_metrics and mode == ModeKeys.EVAL
+        self.unsampled_hist = None
+        if self.unsampled_on and model.engine.world > 1:
+            raise NotImplementedError('the unsampled evaluation metrics run on one process; data-parallel evaluation of '
+                                      'them is not implemented')
         # baseline recommenders (nar_model.py:1399-1407): [{'recommender': <suffix>, 'params': {...}}]; their state is the
         # BaselineTables object on the ClickedItemsState, shared by the TRAIN and EVAL hooks
         self.bench_metrics = None
@@ -213,6 +221,10 @@ class ItemsStateUpdaterHook:
     def begin(self):
         if self.mode == ModeKeys.EVAL:
             self.clicked_items_state.save_state_checkpoint()        # nar_model.py:1415
+            if self.unsampled_on:
+                import torch
+                self.unsampled_hist = torch.zeros(self.eval_metrics_top_n + 2, dtype=torch.int64,
+                                                  device=self.model.engine.dev)
             if self.baselines is not None:
                 import torch
                 self.bench_metrics = torch.zeros(self.baselines.n_rows, 3, dtype=torch.float64, device=self.model.engine.dev)
@@ -253,8 +265,15 @@ class ItemsStateUpdaterHook:
         model's ranked candidates [L, 1+K] on the device, None without queries): the model's and the baselines' top-n
         lists are measured with the popularity the batch was fed with, before the state learns from the batch
         (:1591-1603).  The hit rate by session position takes the same lists.  With a per-session log on also
-        'predicted_item_probs' [L, 1+K] and 'session_ids'."""
+        'predicted_item_probs' [L, 1+K] and 'session_ids'.  With the unsampled metrics on, every label of the staged
+        batch is ranked against the sampler's whole pool: the batch's clicks and labels and the recent-clicks buffer the
+        step was fed with, before the state learns from the batch."""
         ext, bp = self.extended, self.by_position           # set in EVAL only
+        if self.unsampled_hist is not None:
+            eng = self.model.engine
+            pool = eng.unsampled_pool(run_values['clicked_items'], run_values['last_item_label'],
+                                      self.clicked_items_state.get_recent_clicks_buffer())
+            eng.rank_labels(run_values['stage'], pool, self.eval_metrics_top_n, hist=self.unsampled_hist)
         if self.session_logs is not None:
             st = run_values['stage']
             t, pred = st['t'], run_values.get('predicted_item_ids')
@@ -326,6 +345,13 @@ class ItemsStateUpdaterHook:
         names = [(0, '')] + ([(1 + self.baselines.row(s), s) for s in self.baselines.enabled]
                              if self.baselines is not None else [])
         return self.by_position.results(names)
+
+    def unsampled_results(self) -> dict:
+        """The unsampled metrics of this evaluation (eval_metrics.unsampled_results; {} with them off)."""
+        if self.unsampled_hist is None:
+            return {}
+        from .eval_metrics import unsampled_results
+        return unsampled_results(self.unsampled_hist.cpu().numpy(), self.eval_metrics_top_n)
 
     def end(self, session=None):
         if self.mode == ModeKeys.EVAL:

@@ -299,6 +299,17 @@ def topn_candidates(logits, cand_ids, Q, N, top_n, out_ids, out_scores=None, out
                                           _p(out_ids), _p(out_scores), _p(out_probs), _stream()), 'nar_topn_candidates')
 
 
+def rank_labels(logits, cand_ids, Q, N, label_next, all_items, q_pos, T, top_n, rank, hist):
+    """Per query row of logits [Q, N]: rank [Q] int32 = competitors ordered above the label label_next[q_pos[q]] among the
+    ascending ``cand_ids``, excluding the session's row all_items [*, T+1]; ``hist`` [top_n + 2] int64 accumulates the
+    ranks below top_n, the ranked queries and their competitors (nar_rank_labels)."""
+    global LAUNCHES
+    LAUNCHES += 1
+    _chk_f32(logits)
+    check(_lib.load().nar_rank_labels(_p(logits), _p(cand_ids), Q, N, _p(label_next), _p(all_items), _p(q_pos), int(T),
+                                      int(top_n), _p(rank), _p(hist), _stream()), 'nar_rank_labels')
+
+
 def dropout_rows(src, dst, rows, cols, ld, row_pos, n_input, n_cand, K, tensor_id, keep_prob, seed, step):
     """dst = src * mask / keep_prob with the counter-based masks of oracle/dropout_ref.py (tensor_id 0: feature rows)."""
     global LAUNCHES

@@ -351,6 +351,16 @@ int nar_car_combine_grid(const float* PC, const float* PI, int64_t Q, int64_t Nc
 int nar_topn_candidates(const float* logits, const int64_t* cand_ids, int64_t Q, int64_t N, int32_t top_n,
                         const int64_t* item_clicked, const int32_t* q_pos, int64_t T, int64_t* out_ids, float* out_scores,
                         float* out_probs, void* stream);
+/* per query row of logits [Q,N] (unsampled evaluation, DESIGN.md section 13): query q at flat position q_pos[q] = b*T+t
+ * has the label label_next[b*T+t]; cand_ids [N] strictly ascending (N < 2^31).  Its competitors are the candidates other
+ * than the label that are not in the session's row all_items[b*(T+1) + 0..T] (T + 1 <= 1024, else NAR_ERR_UNSUPPORTED).
+ * rank[q] = number of competitors whose score orders above the label's (the order of nar_topn_candidates: -0 == +0, NaN
+ * above +inf; ties go to the label), or -1 when the label is 0 or not a candidate (such a query is not counted).
+ * hist [top_n + 2] int64 (accumulated): [r] += 1 for rank r < top_n, [top_n] += 1 per ranked query, [top_n + 1] += its
+ * number of competitors.                                                                                               */
+int nar_rank_labels(const float* logits, const int64_t* cand_ids, int64_t Q, int64_t N, const int64_t* label_next,
+                    const int64_t* all_items, const int32_t* q_pos, int64_t T, int32_t top_n, int32_t* rank, int64_t* hist,
+                    void* stream);
 
 /* ---- host state (CPU, no CUDA): ClickedItemsState.update_items_state (clicked_items_state.py:187-250) in one pass.
  *      buffer [cap,2] int64 {item, timestamp} newest first, zero padded (in/out); batch_items / batch_ts: the step's
@@ -502,6 +512,12 @@ int nar_engine_recommend_workspace_bytes(const nar_engine* eng, int64_t L, int64
 int nar_engine_recommend(nar_engine* eng, const nar_step_io* io /*host*/, const int64_t* q_rows, const int32_t* q_pos, int64_t Q,
                          const int64_t* cand_ids, int64_t N, int32_t top_n, int32_t exclude_session_clicks, int64_t q_block,
                          int64_t n_block, int64_t* out_ids, float* out_scores, float* out_probs, void* stream);
+/* Unsampled evaluation of a staged EVAL batch (same io and workspace as nar_engine_recommend with Q = L, q_rows = NULL):
+ * every valid position is a query, scored against cand_ids [N] (strictly ascending ids in [1, V)) block by block as
+ * nar_engine_recommend scores it, each logits block finished by nar_rank_labels with the batch's label_next, all_items
+ * and pos_idx.  rank [L] int32, hist [top_n + 2] int64 as there.  NAR_ERR_UNSUPPORTED for T + 1 > 1024.              */
+int nar_engine_rank_labels(nar_engine* eng, const nar_step_io* io /*host*/, const int64_t* cand_ids, int64_t N, int32_t top_n,
+                           int64_t q_block, int64_t n_block, int32_t* rank, int64_t* hist, void* stream);
 /* kernels launched by this engine so far */
 int64_t nar_engine_launch_count(const nar_engine* eng);
 
