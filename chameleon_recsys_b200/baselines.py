@@ -254,6 +254,58 @@ class BaselineTables:
             self.alpha, self.mask, int(top_n), _p(hist), _p(metrics), _p(out_ids), _p(self.err), stream),
             'nar_baselines_score')
 
+    def rank_unsampled(self, item_clicked: torch.Tensor, label_next: torch.Tensor, all_items: torch.Tensor, pool,
+                       articles_pop, top_n: int, hist: torch.Tensor, rank: Optional[torch.Tensor] = None,
+                       max_blocks: int = 0):
+        """Unsampled ranking (DESIGN.md section 14): the label of every query (label != 0) of the batch ``score`` has just
+        scored, against ``pool`` (sorted distinct ids, e.g. NarEngine.unsampled_pool) minus the label and its session's
+        row ``all_items`` [B, T+1], for every enabled baseline, each id scored as ``score`` scores a candidate (it reuses
+        the buffer histogram ``score`` built, so call it after ``score`` and before ``update``).  ``hist`` [n_rows,
+        top_n + 2] int64 device accumulator (rows as ``metrics``): the count of each rank below top_n, the queries, their
+        competitors.  ``rank`` [n_rows, B*T] int32 (optional): each query's rank, 0x7fffffff for a label the baseline does
+        not admit, -1 where no query.  ``max_blocks`` > 0 caps each kernel's grid.  Queues work on the current stream."""
+        s = torch.cuda.current_stream(self.dev)
+        self._wait(s)
+        d = self.dev
+        B, T = item_clicked.shape
+        assert hist.dtype == torch.int64 and hist.shape == (self.n_rows, top_n + 2) and hist.is_contiguous()
+        if rank is not None:
+            assert rank.dtype == torch.int32 and rank.shape == (self.n_rows, B * T) and rank.is_contiguous()
+            rank.fill_(-1)
+        ic = item_clicked.to(d, torch.int64).contiguous()
+        ln = label_next.to(d, torch.int64).contiguous()
+        ai = all_items.to(d, torch.int64).contiguous()
+
+        def up(x):                    # host arrays go up through a pinned copy on the stream: no host synchronisation
+            if torch.is_tensor(x) and x.is_cuda:
+                return x.to(d, torch.int64).contiguous().view(-1)
+            host = torch.as_tensor(np.ascontiguousarray(np.asarray(x, dtype=np.int64).reshape(-1)))
+            with torch.cuda.stream(s):
+                return host.pin_memory().to(d, non_blocking=True)
+        pl = up(pool)
+        stream = C.c_void_p(s.cuda_stream)
+        for sfx, ring in self.knn.items():
+            row = self.row(sfx)
+            ring.rank_unsampled(ic, ln, ai, pl, B, T, top_n, hist[row], None if rank is None else rank[row], s,
+                                max_blocks)
+        if not self.mask:
+            return
+        pop = up(articles_pop) if 'item_knn' in self.enabled else None
+        check(self.lib.nar_baselines_rank_unsampled(
+            *[_p(x) for x in self._tables()], self.cap, _p(ic), _p(ln), _p(ai), B, T, _p(pl), pl.numel(),
+            _p(getattr(self, 'hist_count', None)), _p(getattr(self, 'hist_first', None)), _p(pop), _p(self.acr),
+            self.acr_dim, 0 if self.acr is None else self.acr.shape[1], _p(self.acr_norm), self.num_items, self.reg_lambda,
+            self.alpha, self.mask, int(top_n), int(max_blocks), _p(None if rank is None else rank[:len(SUFFIXES)]),
+            _p(hist), _p(self.err), stream), 'nar_baselines_rank_unsampled')
+
+    def unsampled_results(self, hist) -> Dict[str, float]:
+        """{'unsampled_hitrate_at_n_<suffix>', 'unsampled_mrr_at_n_<suffix>', 'unsampled_ndcg_at_n_<suffix>'} of the
+        enabled baselines and 'unsampled_candidates_per_query' from an [n_rows, top_n + 2] accumulator
+        (eval_metrics.unsampled_results per row)."""
+        from .eval_metrics import unsampled_bench_results
+        return unsampled_bench_results(np.asarray(hist.cpu().numpy() if torch.is_tensor(hist) else hist),
+                                       [(s, self.row(s)) for s in self.enabled])
+
     @staticmethod
     def row(sfx: str) -> int:
         """Row of baseline ``sfx`` in the metrics accumulator and in ``out_ids``."""

@@ -165,14 +165,58 @@ struct ScoreArgs {
   const int* buf_count; const int* buf_first; const int64_t* articles_pop;
   const float* acr; int64_t acr_dim, acr_ld; const double* acr_norm; int64_t num_items;
   double knn_lambda, knn_alpha; int enabled; int top_n;
-  unsigned long long* rank_hist;   // [N_BASELINES, top_n + 1]: queries whose label ranked r (< top_n), and all queries
+  unsigned long long* rank_hist;   // sampled: [N_BASELINES, top_n + 1]: queries whose label ranked r (< top_n), all queries
+                                   // unsampled: [N_BASELINES, top_n + 2]: the same, then the competitor sum
   int64_t* out_ids;                // [N_BASELINES, B*T, top_n] or null
   int* err;
+  // unsampled ranking only
+  const int64_t* all_items;        // [B, T + 1] = item_clicked | label_last_item: the rows whose ids are not competitors
+  const int64_t* pool; int64_t n_pool;
+  int* rank;                       // [N_BASELINES, B*T] or null
 };
 
 // candidate x ranks before y: higher score, then lower tie key
 __device__ __forceinline__ bool before(double sx, long long tx, double sy, long long ty) {
   return sx > sy || (sx == sy && tx < ty);
+}
+
+// Score, tie key and admissibility of candidate c (-1: an invalid id) of a query whose current click is `item`, for the
+// pop_recent, coocurrent, item_knn and sr baselines (bl = 0, 1, 2, 4).  The sampled and the unsampled ranking both score
+// through here, so a (query, id) pair gets the same score in both.
+__device__ __forceinline__ void pair_score(const ScoreArgs& a, int bl, int64_t item, int64_t c, double& sc, long long& tie,
+                                           int& ok) {
+  sc = 0.0; tie = 0; ok = 0;
+  if (c < 0) return;
+  if (bl == 0) {                                                // pop_recent
+    const int cnt = a.buf_count[c];
+    sc = (double)cnt; tie = a.buf_first[c]; ok = cnt > 0;
+    return;
+  }
+  const int64_t s = find(a.keys, a.cap, ((unsigned long long)item << 32) | (unsigned long long)c);
+  if (s < 0) return;
+  const long long co = a.cooc[s];
+  if (bl == 1) { sc = (double)co; tie = -(long long)c; ok = co > 0; }
+  else if (bl == 2) {                                           // item_knn (fp64, the reference's association)
+    const double pc = pow((double)a.articles_pop[c] + a.knn_lambda, a.knn_alpha);
+    const double pa = pow((double)a.articles_pop[item] + a.knn_lambda, 1.0 - a.knn_alpha);
+    sc = __ddiv_rn((double)co, __dmul_rn(pc, pa)); tie = -(long long)c; ok = co > 0;
+  } else {                                                      // sr
+    const long long w = a.sr_w[s];
+    sc = (double)w; tie = a.sr_first[s]; ok = w > 0;
+  }
+}
+
+// cb: fp64 cosine of the ACR rows of `item` and c (-1: an invalid id, scores 0), one warp: lane-strided fma, then the
+// xor-shuffle tree (every lane ends with the same sum).  A zero row scores 0.
+__device__ __forceinline__ double cb_score(const ScoreArgs& a, int64_t item, int64_t c, int lane) {
+  double dot = 0.0;
+  if (c >= 0)
+    for (int64_t k = lane; k < a.acr_dim; k += 32)
+      dot = fma((double)a.acr[item * a.acr_ld + k], (double)a.acr[c * a.acr_ld + k], dot);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+  const double nn = c >= 0 ? a.acr_norm[item] * a.acr_norm[c] : 0.0;
+  return nn > 0.0 ? dot / nn : 0.0;
 }
 
 // one warp per query (b, t) with a nonzero label; candidates = label + the position's K negatives, first occurrence
@@ -205,18 +249,11 @@ __global__ void score_kernel(ScoreArgs a) {
     for (int bl = 0; bl < N_BASELINES; ++bl) {
       if (!((a.enabled >> bl) & 1)) continue;
       if (bl == 3) {                                            // cb: cosine of the ACR rows, warp-cooperative dots
-        const double na = a.acr_norm[item];
         for (int j = 0; j < nc; ++j) {
           const int64_t c = s_id[j];
-          double dot = 0.0;
-          if (c >= 0)
-            for (int64_t k = lane; k < a.acr_dim; k += 32)
-              dot = fma((double)a.acr[item * a.acr_ld + k], (double)a.acr[c * a.acr_ld + k], dot);
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+          const double sc = cb_score(a, item, c, lane);
           if (lane == 0) {
-            const double nn = c >= 0 ? na * a.acr_norm[c] : 0.0;
-            s_score[j] = nn > 0.0 ? dot / nn : 0.0;
+            s_score[j] = sc;
             s_tie[j] = -(long long)c;
             s_ok[j] = c >= 0;
           }
@@ -224,28 +261,8 @@ __global__ void score_kernel(ScoreArgs a) {
         __syncwarp();
       } else {
         for (int j = lane; j < nc; j += 32) {
-          const int64_t c = s_id[j];
-          double sc = 0.0; long long tie = 0; int ok = 0;
-          if (c >= 0) {
-            if (bl == 0) {                                      // pop_recent
-              const int cnt = a.buf_count[c];
-              sc = (double)cnt; tie = a.buf_first[c]; ok = cnt > 0;
-            } else {
-              const int64_t s = find(a.keys, a.cap, ((unsigned long long)item << 32) | (unsigned long long)c);
-              if (s >= 0) {
-                const long long co = a.cooc[s];
-                if (bl == 1) { sc = (double)co; tie = -(long long)c; ok = co > 0; }
-                else if (bl == 2) {                             // item_knn (fp64, the reference's association)
-                  const double pc = pow((double)a.articles_pop[c] + a.knn_lambda, a.knn_alpha);
-                  const double pa = pow((double)a.articles_pop[item] + a.knn_lambda, 1.0 - a.knn_alpha);
-                  sc = __ddiv_rn((double)co, __dmul_rn(pc, pa)); tie = -(long long)c; ok = co > 0;
-                } else {                                        // sr
-                  const long long w = a.sr_w[s];
-                  sc = (double)w; tie = a.sr_first[s]; ok = w > 0;
-                }
-              }
-            }
-          }
+          double sc; long long tie; int ok;
+          pair_score(a, bl, item, s_id[j], sc, tie, ok);
           s_score[j] = sc; s_tie[j] = tie; s_ok[j] = ok;
         }
         __syncwarp();
@@ -285,6 +302,112 @@ __global__ void finalize_kernel(const unsigned long long* rank_hist, int top_n, 
   metrics[bl * 3 + 0] += (double)hits;
   metrics[bl * 3 + 1] += rr;
   metrics[bl * 3 + 2] += (double)h[top_n];
+}
+
+// ---- unsampled ranking (DESIGN.md section 14): each label against the pool minus its session's row
+constexpr int RANK_NT = 256;
+constexpr int RANK_WARPS = RANK_NT / 32;
+constexpr int BLOOM_WORDS = 128;
+constexpr int MISS = 0x7fffffff;           // rank of a label the baseline does not admit: a miss at every n
+
+// One CTA per query (b, t) with label != 0 (grid-stride over the queries when the grid is capped).  The label is scored
+// first; then every pool id outside the session row all_items[b] (behind a Bloom filter) other than the label is a
+// competitor, scored as pair_score / cb_score score it (cb: one warp per id), and rank = the admissible competitors
+// before the label in the baseline's strict order.  Integer histograms only.
+__global__ void __launch_bounds__(RANK_NT) rank_unsampled_kernel(ScoreArgs a) {
+  __shared__ int64_t s_excl[MAX_SESSION];
+  __shared__ uint32_t s_bloom[BLOOM_WORDS];
+  __shared__ double s_lsc[N_BASELINES];
+  __shared__ long long s_ltie[N_BASELINES];
+  __shared__ int s_lok[N_BASELINES];
+  __shared__ int s_red[RANK_WARPS][N_BASELINES + 1];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int64_t nq = a.B * a.T, T1 = a.T + 1;
+  const int n_excl = (int)T1;
+  for (int64_t q = blockIdx.x; q < nq; q += gridDim.x) {
+    const int64_t label = a.label_next[q];
+    const int64_t item = a.item_clicked[q];
+    const bool bad = label != 0 && (item <= 0 || item >= a.num_items || label < 0 || label >= a.num_items);
+    if (label == 0 || bad) {                                    // block-uniform
+      if (tid == 0) {
+        if (bad) atomicExch(a.err, 1);
+        if (a.rank)
+          for (int bl = 0; bl < N_BASELINES; ++bl) a.rank[bl * nq + q] = -1;
+      }
+      continue;
+    }
+    const int64_t b = q / a.T;
+    __syncthreads();                                            // the previous query is done with the shared arrays
+    for (int i = tid; i < BLOOM_WORDS; i += RANK_NT) s_bloom[i] = 0u;
+    __syncthreads();
+    for (int i = tid; i < n_excl; i += RANK_NT) {
+      const int64_t id = a.all_items[b * T1 + i];
+      s_excl[i] = id;
+      const uint32_t h = bloom_slot(id);
+      atomicOr(&s_bloom[h >> 5], 1u << (h & 31));
+    }
+    if (w == 0) {
+      for (int bl = 0; bl < N_BASELINES; ++bl) {
+        if (!((a.enabled >> bl) & 1)) continue;
+        double sc; long long tie; int ok;
+        if (bl == 3) { sc = cb_score(a, item, label, lane); tie = -(long long)label; ok = 1; }
+        else pair_score(a, bl, item, label, sc, tie, ok);
+        if (lane == 0) { s_lsc[bl] = sc; s_ltie[bl] = tie; s_lok[bl] = ok; }
+      }
+    }
+    __syncthreads();
+    auto competitor = [&](int64_t c) -> bool {
+      if (c == label) return false;
+      const uint32_t h = bloom_slot(c);
+      if (s_bloom[h >> 5] & (1u << (h & 31)))
+        for (int i = 0; i < n_excl; ++i)
+          if (s_excl[i] == c) return false;
+      return true;
+    };
+    int above[N_BASELINES], comp = 0;
+#pragma unroll
+    for (int bl = 0; bl < N_BASELINES; ++bl) above[bl] = 0;
+    for (int64_t j = tid; j < a.n_pool; j += RANK_NT) {
+      const int64_t c = a.pool[j];
+      if (c <= 0 || c >= a.num_items) { atomicExch(a.err, 1); continue; }
+      if (!competitor(c)) continue;
+      ++comp;
+#pragma unroll
+      for (int bl = 0; bl < N_BASELINES; ++bl) {
+        if (bl == 3 || !((a.enabled >> bl) & 1)) continue;
+        double sc; long long tie; int ok;
+        pair_score(a, bl, item, c, sc, tie, ok);
+        above[bl] += ok && before(sc, tie, s_lsc[bl], s_ltie[bl]);
+      }
+    }
+    if ((a.enabled >> 3) & 1) {
+      for (int64_t j = w; j < a.n_pool; j += RANK_WARPS) {    // warp-uniform
+        const int64_t c = a.pool[j];
+        if (c <= 0 || c >= a.num_items || !competitor(c)) continue;
+        const double sc = cb_score(a, item, c, lane);
+        if (lane == 0) above[3] += before(sc, -(long long)c, s_lsc[3], s_ltie[3]);
+      }
+    }
+#pragma unroll
+    for (int bl = 0; bl <= N_BASELINES; ++bl) {
+      int v = bl < N_BASELINES ? above[bl] : comp;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) s_red[w][bl] = v;
+    }
+    __syncthreads();
+    if (tid < N_BASELINES && ((a.enabled >> tid) & 1)) {
+      const int bl = tid;
+      int ab = 0, cm = 0;
+      for (int i = 0; i < RANK_WARPS; ++i) { ab += s_red[i][bl]; cm += s_red[i][N_BASELINES]; }
+      const int r = s_lok[bl] ? ab : MISS;
+      if (a.rank) a.rank[bl * nq + q] = r;
+      unsigned long long* h = a.rank_hist + bl * (a.top_n + 2);
+      if (r < a.top_n) atomicAdd(h + r, 1ull);
+      atomicAdd(h + a.top_n, 1ull);
+      atomicAdd(h + a.top_n + 1, (unsigned long long)cm);
+    }
+  }
 }
 
 static inline bool pow2(int64_t x) { return x > 0 && (x & (x - 1)) == 0; }
@@ -401,6 +524,41 @@ extern "C" int nar_baselines_score(const int64_t* keys, const int64_t* cooc, con
     NAR_LAUNCH_CHECK();
   }
   finalize_kernel<<<1, 32, 0, s>>>(a.rank_hist, top_n, enabled, metrics);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_baselines_rank_unsampled(const int64_t* keys, const int64_t* cooc, const int64_t* sr_w,
+                                            const int64_t* sr_first, int64_t cap, const int64_t* item_clicked,
+                                            const int64_t* label_next, const int64_t* all_items, int64_t B, int64_t T,
+                                            const int64_t* pool, int64_t N, const int32_t* buf_count,
+                                            const int32_t* buf_first, const int64_t* articles_pop, const float* acr,
+                                            int64_t acr_dim, int64_t acr_ld, const double* acr_norm, int64_t num_items,
+                                            double knn_lambda, double knn_alpha, int32_t enabled, int32_t top_n,
+                                            int64_t max_blocks, int32_t* rank, int64_t* hist, int* err, void* stream) {
+  if (!item_clicked || !label_next || !all_items || (!pool && N > 0) || !hist || !err || B < 0 || T <= 0 || N < 0 ||
+      top_n < 1 || num_items <= 0 || num_items > 0x7fffffffLL || (enabled & ~31))
+    return NAR_ERR_INVALID;
+  if ((enabled & 1) && (!buf_count || !buf_first)) return NAR_ERR_INVALID;
+  if ((enabled & (2 | 4 | 16)) && (!keys || !cooc || !sr_w || !sr_first || !pow2(cap))) return NAR_ERR_INVALID;
+  if ((enabled & 4) && !articles_pop) return NAR_ERR_INVALID;
+  if ((enabled & 8) && (!acr || !acr_norm || acr_dim <= 0 || acr_ld < acr_dim)) return NAR_ERR_INVALID;
+  if (T + 1 > MAX_SESSION || N > 0x7fffffffLL || B * T > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
+  cudaStream_t s = as_stream(stream);
+  const int64_t nq = B * T;
+  if (rank && nq > 0) NAR_CHECK_CUDA(cudaMemsetAsync(rank, 0xff, sizeof(int32_t) * N_BASELINES * nq, s));
+  if (enabled == 0 || nq == 0) return NAR_OK;
+  ScoreArgs a = {};
+  a.keys = reinterpret_cast<const unsigned long long*>(keys); a.cooc = (const long long*)cooc;
+  a.sr_w = (const long long*)sr_w; a.sr_first = (const long long*)sr_first; a.cap = cap;
+  a.item_clicked = item_clicked; a.label_next = label_next; a.B = B; a.T = T;
+  a.buf_count = buf_count; a.buf_first = buf_first; a.articles_pop = articles_pop;
+  a.acr = acr; a.acr_dim = acr_dim; a.acr_ld = acr_ld; a.acr_norm = acr_norm; a.num_items = num_items;
+  a.knn_lambda = knn_lambda; a.knn_alpha = knn_alpha; a.enabled = enabled; a.top_n = top_n;
+  a.rank_hist = reinterpret_cast<unsigned long long*>(hist); a.err = err;
+  a.all_items = all_items; a.pool = pool; a.n_pool = N; a.rank = rank;
+  const int64_t grid = max_blocks > 0 && max_blocks < nq ? max_blocks : nq;
+  rank_unsampled_kernel<<<(unsigned)grid, RANK_NT, 0, s>>>(a);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

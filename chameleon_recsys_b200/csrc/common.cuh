@@ -102,4 +102,7 @@ __device__ __forceinline__ uint64_t shuffle_key(uint64_t seed, uint32_t step, ui
   return ((uint64_t)philox_word(p, idx & 3u) << 32) | (uint64_t)idx;
 }
 
+// bit of an id in the 4096-bit Bloom filters in front of the session-row exclusion lists (top n, label ranks)
+__device__ __forceinline__ uint32_t bloom_slot(int64_t id) { return ((uint32_t)id * 2654435761u) >> 20; }
+
 }  // namespace nar

@@ -48,7 +48,6 @@ __device__ __forceinline__ uint32_t order_key(float f) {
 
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
-__device__ __forceinline__ uint32_t bloom_slot(int64_t id) { return ((uint32_t)id * 2654435761u) >> 20; }
 
 struct TopnShared {
   unsigned long long sel[TOPN_MAX];         // (key << 32) | (0xffffffff - index): descending order = score desc, index asc

@@ -128,9 +128,14 @@ struct ScoreArgs {
   const int64_t* ids; const int* lens; const int* items; int64_t S; int W; int64_t head, count;
   const int64_t *item_clicked, *label_next, *negatives; int64_t B, T, K, num_items;
   int64_t sample_size, nn; int decay_div, jaccard, top_n;
-  unsigned long long* rank_hist;   // [top_n + 1]: queries whose label ranked r (< top_n), and all queries
+  unsigned long long* rank_hist;   // sampled: [top_n + 1]: queries whose label ranked r (< top_n), and all queries
+                                   // unsampled: [top_n + 2]: the same, then the competitor sum
   int64_t* out_ids;                // [B*T, top_n] or null
   int* err;
+  // unsampled ranking only
+  const int64_t* all_items;        // [B, T + 1] = item_clicked | label_last_item: the rows whose ids are not competitors
+  const int64_t* pool; int64_t n_pool;
+  int* rank;                       // [B*T] or null
 };
 
 template <typename V>
@@ -202,49 +207,44 @@ static inline size_t score_smem(int64_t count) {
   return (size_t)(28 * sc + 2 * n2);
 }
 
-// one CTA per query (b, t) with label != 0
-__global__ void __launch_bounds__(ST) score_kernel(ScoreArgs a) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  const int n = (int)a.count;
-  const int sc = n > 0 ? n : 1;
-  unsigned long long* s_acc = reinterpret_cast<unsigned long long*>(smem);  // position masks; later neighbour masks
-  int64_t* s_cid = reinterpret_cast<int64_t*>(smem + 8 * (size_t)sc);       // candidate session ids
-  double* s_sim = reinterpret_cast<double*>(smem + 16 * (size_t)sc);        // similarities; ring ids during the scan
-  uint16_t* s_slot = reinterpret_cast<uint16_t*>(smem + 24 * (size_t)sc);   // candidate -> logical slot
-  uint16_t* s_cnt = s_slot + sc;                                             // candidate -> copies
-  uint16_t* s_perm = s_cnt + sc;
+// The score kernels' dynamic shared memory (score_smem): per ring entry its neighbour mask, candidate session id,
+// similarity, slot, copies and sort permutation
+struct RingShared {
+  unsigned long long* acc;         // position masks; later neighbour masks
+  int64_t* cid;                    // candidate session ids
+  double* sim;                     // similarities; ring ids during the scan
+  uint16_t *slot, *cnt, *perm;     // candidate -> logical slot, candidate -> copies, sort permutation
+  __device__ RingShared(unsigned char* smem, int n) {
+    const int sc = n > 0 ? n : 1;
+    acc = reinterpret_cast<unsigned long long*>(smem);
+    cid = reinterpret_cast<int64_t*>(smem + 8 * (size_t)sc);
+    sim = reinterpret_cast<double*>(smem + 16 * (size_t)sc);
+    slot = reinterpret_cast<uint16_t*>(smem + 24 * (size_t)sc);
+    cnt = slot + sc;
+    perm = cnt + sc;
+  }
+};
+
+// Steps (1)-(4) of the scoring (DESIGN.md section 9) for the active session P = item_clicked[b, :np], called by every
+// thread of the CTA: the ring scan, the 'recent' cut, the similarities and the neighbour cut.  -> nb: the kept neighbours
+// are r.perm[0..nb) in neighbour order, neighbour k with similarity r.sim[k], r.cnt[k] copies and logical slot r.slot[k].
+__device__ int select_neighbours(const ScoreArgs& a, int64_t b, int np, const RingShared& r) {
   __shared__ int64_t s_P[MAX_T], s_pd[MAX_T];
   __shared__ unsigned long long s_pdm[MAX_T];      // distinct item of P -> positions holding it
   __shared__ int s_pfirst[MAX_T];
-  __shared__ int s_q[MAX_CAND], s_qf[MAX_CAND], s_qfirst[MAX_CAND];
-  __shared__ double s_qs[MAX_CAND];
   __shared__ int s_warp[NW];
   __shared__ int s_n, s_total, s_kept, s_nb;
   const int tid = threadIdx.x;
-  const int64_t q = blockIdx.x;
-  const int64_t label = a.label_next[q];
-  if (label == 0) return;                                            // block-uniform
-  const int64_t b = q / a.T, t = q % a.T;
-  const int np = (int)t + 1;
-  {
-    const int64_t item = a.item_clicked[q];
-    if (item <= 0 || item >= a.num_items || label < 0 || label >= a.num_items) {
-      if (tid == 0) atomicExch(a.err, 1);
-      return;
-    }
-  }
+  const int n = (int)a.count;
+  unsigned long long* s_acc = r.acc;
+  int64_t* s_cid = r.cid;
+  double* s_sim = r.sim;
+  uint16_t *s_slot = r.slot, *s_cnt = r.cnt, *s_perm = r.perm;
   // ---- the active session P = item_clicked[b, :t+1]: distinct items (sorted) with their position masks
   if (tid < np) {
     int64_t x = a.item_clicked[b * a.T + tid];
     if (x < 0 || x >= a.num_items) { atomicExch(a.err, 1); x = 0; }
     s_P[tid] = x;
-  }
-  // ---- the query's candidates: label + K negatives, distinct nonzero ids, sorted
-  const int nc = (int)a.K + 1;
-  for (int j = tid; j < nc; j += ST) {
-    int64_t id = j == 0 ? label : a.negatives[q * a.K + (j - 1)];
-    if (id < 0 || id >= a.num_items) { atomicExch(a.err, 1); id = 0; }
-    s_qf[j] = (int)id;
   }
   if (tid == 0) { s_n = 0; s_total = 0; s_kept = 0; s_nb = 0; }
   __syncthreads();
@@ -252,12 +252,6 @@ __global__ void __launch_bounds__(ST) score_kernel(ScoreArgs a) {
     int first = 1;
     for (int p = 0; p < tid; ++p) first &= s_P[p] != s_P[tid];
     s_pfirst[tid] = first;
-  }
-  for (int j = tid; j < nc; j += ST) {
-    const int x = s_qf[j];
-    int first = x != 0;
-    for (int k = 0; k < j && first; ++k) first = s_qf[k] != x;
-    s_qfirst[j] = first;
   }
   __syncthreads();
   if (tid < np && s_pfirst[tid]) {
@@ -270,16 +264,8 @@ __global__ void __launch_bounds__(ST) score_kernel(ScoreArgs a) {
     }
     s_pd[rank] = x; s_pdm[rank] = m;
   }
-  for (int j = tid; j < nc; j += ST) {
-    if (!s_qfirst[j]) continue;
-    const int x = s_qf[j];
-    int rank = 0;
-    for (int k = 0; k < nc; ++k) rank += s_qfirst[k] && s_qf[k] < x;
-    s_q[rank] = x;
-  }
-  int nP = 0, nq = 0;
+  int nP = 0;
   for (int p = 0; p < np; ++p) nP += s_pfirst[p];
-  for (int j = 0; j < nc; ++j) nq += s_qfirst[j];
   // ---- scan the ring: positions of P whose item is live in the slot, OR-ed into the slot the binary search finds
   int64_t* s_idc = reinterpret_cast<int64_t*>(s_sim);
   for (int i = tid; i < n; i += ST) { s_idc[i] = a.ids[(a.head + i) % a.S]; s_acc[i] = 0; }
@@ -351,32 +337,90 @@ __global__ void __launch_bounds__(ST) score_kernel(ScoreArgs a) {
   for (int r = tid; r < kept; r += ST)
     if (s_cnt[s_perm[r]] > 0) atomicAdd(&s_nb, 1);
   __syncthreads();
-  const int nb = s_nb;                                               // the kept neighbours: a prefix of perm
+  return s_nb;                                                       // the kept neighbours: a prefix of perm
+}
+
+// r.acc[k] = the mask of the ids ids[0..cn) (ascending, cn <= 64) that kept neighbour k (< nb) holds; ends with a barrier
+__device__ __forceinline__ void neighbour_masks(const ScoreArgs& a, int nb, const RingShared& r, const int* ids, int cn) {
+  for (int k = threadIdx.x; k < nb; k += ST) {
+    const int64_t ph = (a.head + r.slot[r.perm[k]]) % a.S;
+    const int L = a.lens[ph];
+    const int* row = a.items + ph * a.W;
+    unsigned long long m = 0;
+    for (int kk = 0; kk < L; ++kk) {
+      const int d = find_sorted(ids, cn, abs(row[kk]));
+      if (d >= 0) m |= 1ull << d;
+    }
+    r.acc[k] = m;
+  }
+  __syncthreads();
+}
+
+// item score of the id at mask bit `bit`: the similarities of the kept neighbours holding it, summed copy by copy in
+// neighbour order; first = the rank of the first of them (-1: none, the id is not admissible)
+__device__ __forceinline__ void item_score(int nb, const RingShared& r, int bit, double& score, int& first) {
+  double sc_ = 0.0;
+  first = -1;
+  for (int k = 0; k < nb; ++k) {
+    if (!((r.acc[k] >> bit) & 1ull)) continue;
+    if (first < 0) first = k;
+    const int j = r.perm[k];
+    const double v = r.sim[j];
+    for (int c = 0; c < r.cnt[j]; ++c) sc_ = __dadd_rn(sc_, v);
+  }
+  score = sc_;
+}
+
+// one CTA per query (b, t) with label != 0
+__global__ void __launch_bounds__(ST) score_kernel(ScoreArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const RingShared ring(smem, (int)a.count);
+  __shared__ int s_q[MAX_CAND], s_qf[MAX_CAND], s_qfirst[MAX_CAND];
+  __shared__ double s_qs[MAX_CAND];
+  const int tid = threadIdx.x;
+  const int64_t q = blockIdx.x;
+  const int64_t label = a.label_next[q];
+  if (label == 0) return;                                            // block-uniform
+  const int64_t b = q / a.T, t = q % a.T;
+  {
+    const int64_t item = a.item_clicked[q];
+    if (item <= 0 || item >= a.num_items || label < 0 || label >= a.num_items) {
+      if (tid == 0) atomicExch(a.err, 1);
+      return;
+    }
+  }
+  // ---- the query's candidates: label + K negatives, distinct nonzero ids, sorted
+  const int nc = (int)a.K + 1;
+  for (int j = tid; j < nc; j += ST) {
+    int64_t id = j == 0 ? label : a.negatives[q * a.K + (j - 1)];
+    if (id < 0 || id >= a.num_items) { atomicExch(a.err, 1); id = 0; }
+    s_qf[j] = (int)id;
+  }
+  __syncthreads();
+  for (int j = tid; j < nc; j += ST) {
+    const int x = s_qf[j];
+    int first = x != 0;
+    for (int k = 0; k < j && first; ++k) first = s_qf[k] != x;
+    s_qfirst[j] = first;
+  }
+  __syncthreads();
+  for (int j = tid; j < nc; j += ST) {
+    if (!s_qfirst[j]) continue;
+    const int x = s_qf[j];
+    int rank = 0;
+    for (int k = 0; k < nc; ++k) rank += s_qfirst[k] && s_qf[k] < x;
+    s_q[rank] = x;
+  }
+  int nq = 0;
+  for (int j = 0; j < nc; ++j) nq += s_qfirst[j];
+  const int nb = select_neighbours(a, b, (int)t + 1, ring);
   // ---- item scores of the query's candidates, 64 at a time: neighbour masks, then sums copy by copy in order
   for (int c0 = 0; c0 < nq; c0 += 64) {
     const int cn = min(64, nq - c0);
-    for (int r = tid; r < nb; r += ST) {
-      const int64_t ph = (a.head + s_slot[s_perm[r]]) % a.S;
-      const int L = a.lens[ph];
-      const int* row = a.items + ph * a.W;
-      unsigned long long m = 0;
-      for (int kk = 0; kk < L; ++kk) {
-        const int d = find_sorted(s_q + c0, cn, abs(row[kk]));
-        if (d >= 0) m |= 1ull << d;
-      }
-      s_acc[r] = m;
-    }
-    __syncthreads();
+    neighbour_masks(a, nb, ring, s_q + c0, cn);
     if (tid < cn) {
-      double sc_ = 0.0;
-      int first = -1;
-      for (int r = 0; r < nb; ++r) {
-        if (!((s_acc[r] >> tid) & 1ull)) continue;
-        if (first < 0) first = r;
-        const int k = s_perm[r];
-        const double v = s_sim[k];
-        for (int c = 0; c < s_cnt[k]; ++c) sc_ = __dadd_rn(sc_, v);
-      }
+      double sc_; int first;
+      item_score(nb, ring, tid, sc_, first);
       s_qs[c0 + tid] = sc_; s_qf[c0 + tid] = first;
     }
     __syncthreads();
@@ -401,6 +445,87 @@ __global__ void __launch_bounds__(ST) score_kernel(ScoreArgs a) {
     }
   }
   if (tid == 0) atomicAdd(a.rank_hist + a.top_n, 1ull);
+}
+
+constexpr int MISS = 0x7fffffff;           // rank of a label no kept neighbour holds: a miss at every n
+
+// Unsampled ranking (DESIGN.md section 14), one CTA per query (b, t) with label != 0 (grid-stride over the queries when
+// the grid is capped): the neighbours of the sampled kernel, the label's key (score, first neighbour, id) from a one-id
+// chunk, then the pool 64 ids at a time as step (5) walks the query's candidates: an id is a competitor when it is not
+// the label and not in the session row all_items[b]; rank = the admissible competitors before the label.
+__global__ void __launch_bounds__(ST) rank_unsampled_kernel(ScoreArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const RingShared ring(smem, (int)a.count);
+  __shared__ int s_chunk[64];
+  __shared__ int64_t s_row[MAX_T + 1];
+  __shared__ double s_lsc;
+  __shared__ int s_lfirst;
+  __shared__ int s_red[NW][2];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int64_t nq = a.B * a.T, T1 = a.T + 1;
+  for (int64_t q = blockIdx.x; q < nq; q += gridDim.x) {
+    const int64_t label = a.label_next[q];
+    const int64_t item = a.item_clicked[q];
+    const bool bad = label != 0 && (item <= 0 || item >= a.num_items || label < 0 || label >= a.num_items);
+    if (label == 0 || bad) {                                         // block-uniform
+      if (tid == 0) {
+        if (bad) atomicExch(a.err, 1);
+        if (a.rank) a.rank[q] = -1;
+      }
+      continue;
+    }
+    const int64_t b = q / a.T, t = q % a.T;
+    __syncthreads();                                                 // the previous query is done with shared memory
+    if (tid < T1) s_row[tid] = a.all_items[b * T1 + tid];
+    if (tid == 0) s_chunk[0] = (int)label;
+    const int nb = select_neighbours(a, b, (int)t + 1, ring);
+    neighbour_masks(a, nb, ring, s_chunk, 1);
+    if (tid == 0) item_score(nb, ring, 0, s_lsc, s_lfirst);
+    __syncthreads();
+    const double lsc = s_lsc;
+    const int lf = s_lfirst;
+    int above = 0, comp = 0;
+    for (int64_t c0 = 0; c0 < a.n_pool; c0 += 64) {
+      const int cn = (int)min((int64_t)64, a.n_pool - c0);
+      if (tid < cn) {
+        int64_t id = a.pool[c0 + tid];
+        if (id <= 0 || id >= a.num_items) { atomicExch(a.err, 1); id = 0; }
+        s_chunk[tid] = (int)id;
+      }
+      __syncthreads();
+      if (lf >= 0) neighbour_masks(a, nb, ring, s_chunk, cn);     // block-uniform; a miss only counts competitors
+      if (tid < cn) {
+        const int id = s_chunk[tid];
+        bool is_comp = id != 0 && id != label;
+        for (int i = 0; i < T1 && is_comp; ++i) is_comp = s_row[i] != id;
+        if (is_comp) {
+          ++comp;
+          if (lf >= 0) {
+            double sc_; int f;
+            item_score(nb, ring, tid, sc_, f);
+            above += f >= 0 && (sc_ > lsc || (sc_ == lsc && (f < lf || (f == lf && id < label))));
+          }
+        }
+      }
+      __syncthreads();                                               // before the next chunk overwrites s_chunk / acc
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      above += __shfl_xor_sync(0xffffffffu, above, o);
+      comp += __shfl_xor_sync(0xffffffffu, comp, o);
+    }
+    if (lane == 0) { s_red[w][0] = above; s_red[w][1] = comp; }
+    __syncthreads();
+    if (tid == 0) {
+      int ab = 0, cm = 0;
+      for (int i = 0; i < NW; ++i) { ab += s_red[i][0]; cm += s_red[i][1]; }
+      const int r = lf >= 0 ? ab : MISS;
+      if (a.rank) a.rank[q] = r;
+      if (r < a.top_n) atomicAdd(a.rank_hist + r, 1ull);
+      atomicAdd(a.rank_hist + a.top_n, 1ull);
+      atomicAdd(a.rank_hist + a.top_n + 1, (unsigned long long)cm);
+    }
+  }
 }
 
 // metrics += {hits, sum of reciprocal ranks, queries}, summed over the rank histogram in a fixed order
@@ -472,6 +597,38 @@ extern "C" int nar_sknn_score(const int64_t* ids, const int32_t* lens, const int
     NAR_LAUNCH_CHECK();
   }
   finalize_kernel<<<1, 1, 0, s>>>(a.rank_hist, top_n, metrics);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_sknn_rank_unsampled(const int64_t* ids, const int32_t* lens, const int32_t* items, int64_t S, int64_t W,
+                                       int64_t head, int64_t count, const int64_t* item_clicked, const int64_t* label_next,
+                                       const int64_t* all_items, int64_t B, int64_t T, const int64_t* pool, int64_t N,
+                                       int64_t num_items, int64_t sample_size, int64_t nn, int32_t decay_div,
+                                       int32_t jaccard, int32_t top_n, int64_t max_blocks, int32_t* rank, int64_t* hist,
+                                       int* err, void* stream) {
+  if (!ids || !lens || !items || !item_clicked || !label_next || !all_items || (!pool && N > 0) || !hist || !err || S <= 0 ||
+      W <= 0 || head < 0 || head >= S || count < 0 || count > S || B < 0 || T <= 0 || N < 0 || top_n < 1 ||
+      num_items <= 0 || num_items > 0x7fffffffLL || sample_size < 0 || nn < 0)
+    return NAR_ERR_INVALID;
+  if (S > MAX_SESSIONS || T > MAX_T || B * T > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
+  cudaStream_t s = as_stream(stream);
+  static bool attr = false;
+  if (!attr) {
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(rank_unsampled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)score_smem(MAX_SESSIONS)));
+    attr = true;
+  }
+  const int64_t nq = B * T;
+  if (nq == 0) return NAR_OK;
+  ScoreArgs a = {};
+  a.ids = ids; a.lens = lens; a.items = items; a.S = S; a.W = (int)W; a.head = head; a.count = count;
+  a.item_clicked = item_clicked; a.label_next = label_next; a.B = B; a.T = T;
+  a.num_items = num_items; a.sample_size = sample_size; a.nn = nn; a.decay_div = decay_div; a.jaccard = jaccard;
+  a.top_n = top_n; a.rank_hist = reinterpret_cast<unsigned long long*>(hist); a.err = err;
+  a.all_items = all_items; a.pool = pool; a.n_pool = N; a.rank = rank;
+  const int64_t grid = max_blocks > 0 && max_blocks < nq ? max_blocks : nq;
+  rank_unsampled_kernel<<<(unsigned)grid, ST, score_smem(count), s>>>(a);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

@@ -105,7 +105,8 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
                                    eval_extended_metrics=bool(params.get('eval_extended_metrics', False)),
                                    eval_metrics_by_session_position=bool(
                                        params.get('eval_metrics_by_session_position', False)),
-                                   eval_unsampled_metrics=bool(params.get('eval_unsampled_metrics', False)))]
+                                   eval_unsampled_metrics=bool(params.get('eval_unsampled_metrics', False)),
+                                   eval_unsampled_benchmarks=bool(params.get('eval_unsampled_benchmarks', False)))]
     if mode == ModeKeys.TRAIN:
         def train_op(feats, labs, feed, sync=True):
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
@@ -336,7 +337,9 @@ class Estimator:
         session position PP ('%02d', from 01) that had a query (none without input).  With ``eval_unsampled_metrics``
         also ``unsampled_hitrate_at_n``, ``unsampled_mrr_at_n``, ``unsampled_ndcg_at_n`` and
         ``unsampled_candidates_per_query``: each label ranked against every article the negative sampler could have drawn
-        for it (DESIGN.md section 13; NaN without input)."""
+        for it (DESIGN.md section 13; NaN without input).  With ``eval_unsampled_benchmarks`` also
+        ``unsampled_hitrate_at_n_<suffix>``, ``unsampled_mrr_at_n_<suffix>`` and ``unsampled_ndcg_at_n_<suffix>`` of every
+        baseline and ``unsampled_candidates_per_query``, against the same competitors (DESIGN.md section 14)."""
         import torch
         batches = _batches(input_fn(), steps)
         nxt = next(batches, None)
@@ -351,6 +354,14 @@ class Estimator:
             if self.params.get('eval_unsampled_metrics'):
                 from .eval_metrics import UNSAMPLED_KEYS
                 empty.update({k: float('nan') for k in UNSAMPLED_KEYS})
+            if self.params.get('eval_unsampled_benchmarks'):
+                from .baselines import parse_classifiers
+                from .eval_metrics import unsampled_bench_keys
+                if not self.params.get('eval_benchmarks'):
+                    raise ValueError('eval_unsampled_benchmarks ranks the baselines of eval_benchmarks, and none is set')
+                for s in parse_classifiers(self.params.get('eval_benchmarks') or ()):
+                    empty.update({k: float('nan') for k in unsampled_bench_keys(s)})
+                empty['unsampled_candidates_per_query'] = float('nan')
             return empty
         if self._eval_spec is None:
             self._eval_spec = self.model_fn(nxt[0], nxt[1], ModeKeys.EVAL, self.params)
@@ -386,6 +397,7 @@ class Estimator:
             bench.update(h.extended_results())
             bench.update(h.by_position_results())
             bench.update(h.unsampled_results())
+            bench.update(h.unsampled_benchmark_results())
             h.end()
         eng = spec.model.engine
         if eng.world > 1:                                           # data parallel: every rank ranked its own sessions

@@ -235,3 +235,23 @@ def unsampled_results(hist, top_n: int) -> Dict[str, float]:
         mrr += h[r] / (r + 1.0)
         ndcg += h[r] / float(np.log2(r + 2.0))
     return dict(zip(UNSAMPLED_KEYS, (hits / q, mrr / q, ndcg / q, h[n + 1] / q)))
+
+
+def unsampled_bench_keys(suffix: str):
+    """The per-baseline unsampled keys of ``suffix`` (switch ``eval_unsampled_benchmarks``; DESIGN.md section 14)."""
+    return tuple('%s_%s' % (k, suffix) for k in UNSAMPLED_KEYS[:3])
+
+
+def unsampled_bench_results(hist, rows) -> Dict[str, float]:
+    """The unsampled metrics of the baselines from their integer accumulator hist [n_rows, top_n + 2] (one row per baseline,
+    laid out as NarEngine.rank_labels' histogram): ``rows`` = [(suffix, row)].  -> each baseline's
+    ``unsampled_<metric>_at_n_<suffix>`` and ``unsampled_candidates_per_query``, the same for every baseline (they share the
+    queries and the competitor sets)."""
+    h = np.asarray(hist, dtype=np.int64)
+    top_n = h.shape[1] - 2
+    out: Dict[str, float] = {}
+    for sfx, row in rows:
+        r = unsampled_results(h[row], top_n)
+        out.update(zip(unsampled_bench_keys(sfx), (r[k] for k in UNSAMPLED_KEYS[:3])))
+        out['unsampled_candidates_per_query'] = r['unsampled_candidates_per_query']
+    return out

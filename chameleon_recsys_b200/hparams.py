@@ -155,6 +155,9 @@ class NARHParams:
     # hit rate, MRR and NDCG of each label ranked against every article the negative sampler could have drawn for it, in
     # Estimator.evaluate (DESIGN.md section 13; NarEngine.rank_labels)
     eval_unsampled_metrics: bool = False
+    # the same unsampled hit rate, MRR and NDCG for every baseline of eval_benchmarks, ranked against the same competitors
+    # (DESIGN.md section 14; BaselineTables.rank_unsampled)
+    eval_unsampled_benchmarks: bool = False
 
     def to_params(self, session_features_config, articles_features_config, articles_metadata,
                   content_article_embeddings_matrix) -> dict:
@@ -202,6 +205,8 @@ class NARHParams:
             params['eval_extended_metrics'] = True
         if self.eval_unsampled_metrics:
             params['eval_unsampled_metrics'] = True
+        if self.eval_unsampled_benchmarks:
+            params['eval_unsampled_benchmarks'] = True
         return params
 
     def copy(self, **kw) -> 'NARHParams':

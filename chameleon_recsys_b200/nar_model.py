@@ -154,7 +154,7 @@ class ItemsStateUpdaterHook:
                  sessions_chameleon_recommendations_log=None, content_article_embeddings_matrix=None,
                  articles_metadata=None, eval_negative_sample_relevance=None, eval_benchmark_classifiers=(),
                  eval_metrics_by_session_position=False, eval_cold_start=False, eval_extended_metrics=False,
-                 eval_unsampled_metrics=False):
+                 eval_unsampled_metrics=False, eval_unsampled_benchmarks=False):
         self.mode = mode
         self.model = model
         self.eval_metrics_top_n = eval_metrics_top_n
@@ -198,6 +198,15 @@ class ItemsStateUpdaterHook:
         if self.unsampled_on and model.engine.world > 1:
             raise NotImplementedError('the unsampled evaluation metrics run on one process; data-parallel evaluation of '
                                       'them is not implemented')
+        # the same for every baseline (BaselineTables.rank_unsampled): an int64 histogram [n_rows, top_n + 2]
+        self.unsampled_bench_on = eval_unsampled_benchmarks and mode == ModeKeys.EVAL
+        self.unsampled_bench_hist = None
+        if self.unsampled_bench_on:
+            if model.engine.world > 1:
+                raise NotImplementedError('the unsampled evaluation of the baselines runs on one process; data-parallel '
+                                          'evaluation of it is not implemented')
+            if not eval_benchmark_classifiers:
+                raise ValueError('eval_unsampled_benchmarks ranks the baselines of eval_benchmarks, and none is set')
         # baseline recommenders (nar_model.py:1399-1407): [{'recommender': <suffix>, 'params': {...}}]; their state is the
         # BaselineTables object on the ClickedItemsState, shared by the TRAIN and EVAL hooks
         self.bench_metrics = None
@@ -228,6 +237,9 @@ class ItemsStateUpdaterHook:
             if self.baselines is not None:
                 import torch
                 self.bench_metrics = torch.zeros(self.baselines.n_rows, 3, dtype=torch.float64, device=self.model.engine.dev)
+                if self.unsampled_bench_on:
+                    self.unsampled_bench_hist = torch.zeros(self.baselines.n_rows, self.eval_metrics_top_n + 2,
+                                                            dtype=torch.int64, device=self.model.engine.dev)
             if self.extended_metrics:
                 if self.extended is None:
                     from .eval_metrics import EvalMetrics
@@ -267,13 +279,15 @@ class ItemsStateUpdaterHook:
         (:1591-1603).  The hit rate by session position takes the same lists.  With a per-session log on also
         'predicted_item_probs' [L, 1+K] and 'session_ids'.  With the unsampled metrics on, every label of the staged
         batch is ranked against the sampler's whole pool: the batch's clicks and labels and the recent-clicks buffer the
-        step was fed with, before the state learns from the batch."""
+        step was fed with, before the state learns from the batch.  With the baselines' unsampled metrics on, each
+        baseline ranks the same labels against the same pool right after its sampled scoring."""
         ext, bp = self.extended, self.by_position           # set in EVAL only
+        pool = None
+        if self.unsampled_hist is not None or self.unsampled_bench_hist is not None:
+            pool = self.model.engine.unsampled_pool(run_values['clicked_items'], run_values['last_item_label'],
+                                                    self.clicked_items_state.get_recent_clicks_buffer())
         if self.unsampled_hist is not None:
-            eng = self.model.engine
-            pool = eng.unsampled_pool(run_values['clicked_items'], run_values['last_item_label'],
-                                      self.clicked_items_state.get_recent_clicks_buffer())
-            eng.rank_labels(run_values['stage'], pool, self.eval_metrics_top_n, hist=self.unsampled_hist)
+            self.model.engine.rank_labels(run_values['stage'], pool, self.eval_metrics_top_n, hist=self.unsampled_hist)
         if self.session_logs is not None:
             st = run_values['stage']
             t, pred = st['t'], run_values.get('predicted_item_ids')
@@ -304,6 +318,10 @@ class ItemsStateUpdaterHook:
                                  self.clicked_items_state.get_recent_clicks_buffer(),
                                  self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n, self.bench_metrics,
                                  out_ids=out_ids)
+            if self.unsampled_bench_hist is not None:
+                self.baselines.rank_unsampled(t['item_clicked'], t['label_next'], t['all_items'], pool,
+                                              self.clicked_items_state.get_articles_pop(), self.eval_metrics_top_n,
+                                              self.unsampled_bench_hist)
             if out_ids is not None:
                 mask = sum(1 << self.baselines.row(s) for s in self.baselines.enabled)
                 if ext is not None:
@@ -352,6 +370,12 @@ class ItemsStateUpdaterHook:
             return {}
         from .eval_metrics import unsampled_results
         return unsampled_results(self.unsampled_hist.cpu().numpy(), self.eval_metrics_top_n)
+
+    def unsampled_benchmark_results(self) -> dict:
+        """The baselines' unsampled metrics of this evaluation (BaselineTables.unsampled_results; {} with them off)."""
+        if self.unsampled_bench_hist is None:
+            return {}
+        return self.baselines.unsampled_results(self.unsampled_bench_hist)
 
     def end(self, session=None):
         if self.mode == ModeKeys.EVAL:

@@ -100,6 +100,16 @@ class SessionKNN:
                                       self.decay_div, self.jaccard, int(top_n), _p(hist), _p(metrics_row), _p(out_ids),
                                       _p(self.err), C.c_void_p(stream.cuda_stream)), 'nar_sknn_score')
 
+    def rank_unsampled(self, ic, ln, all_items, pool, B, T, top_n, hist_row: torch.Tensor, rank_row, stream,
+                       max_blocks: int = 0):
+        """Unsampled ranks against ``pool`` [N] (ascending device ids; DESIGN.md section 14): ``hist_row`` [top_n + 2]
+        int64 device accumulator, ``rank_row`` [B*T] int32 or None (nar_sknn_rank_unsampled)."""
+        check(self.lib.nar_sknn_rank_unsampled(_p(self.ids), _p(self.lens), _p(self.items), self.S, WIDTH, self.head,
+                                               self.count, _p(ic), _p(ln), _p(all_items), B, T, _p(pool), pool.numel(),
+                                               self.num_items, self.sample_size, self.nn, self.decay_div, self.jaccard,
+                                               int(top_n), int(max_blocks), _p(rank_row), _p(hist_row), _p(self.err),
+                                               C.c_void_p(stream.cuda_stream)), 'nar_sknn_rank_unsampled')
+
     # ---- snapshot / restore / export / load
     def snapshot(self):
         self._chk = (self.ids.clone(), self.lens.clone(), self.items.clone(), self.head, self.count)

@@ -550,6 +550,21 @@ int nar_baselines_score(const int64_t* keys, const int64_t* cooc, const int64_t*
                         const int64_t* articles_pop, const float* acr, int64_t acr_dim, int64_t acr_ld,
                         const double* acr_norm, int64_t num_items, double knn_lambda, double knn_alpha, int32_t enabled,
                         int32_t top_n, int64_t* rank_hist, double* metrics, int64_t* out_ids, int* err, void* stream);
+/* Unsampled ranking (DESIGN.md section 14) of the enabled baselines of nar_baselines_score (same tables, buffer
+ * histogram, popularity and ACR inputs): every query (b, t) with label_next != 0 ranks its label against the pool [N]
+ * (distinct ids in [1, num_items)) minus the label and the ids of its session row all_items[b*(T+1) + 0..T]
+ * (T + 1 <= 1024, else NAR_ERR_UNSUPPORTED), each id scored as nar_baselines_score scores a candidate.  rank = the
+ * admissible competitors before the label in the baseline's order, 0x7fffffff when the baseline does not admit the label.
+ * hist [5, top_n + 2] int64 (accumulated): per baseline [r] += 1 for rank r < top_n, [top_n] += 1 per query,
+ * [top_n + 1] += its competitor count.  rank [5, B*T] int32 (optional; -1 where no query).  max_blocks > 0 caps the
+ * grid (one CTA per query otherwise).  One launch.                                                                   */
+int nar_baselines_rank_unsampled(const int64_t* keys, const int64_t* cooc, const int64_t* sr_w, const int64_t* sr_first,
+                                 int64_t cap, const int64_t* item_clicked, const int64_t* label_next,
+                                 const int64_t* all_items, int64_t B, int64_t T, const int64_t* pool, int64_t N,
+                                 const int32_t* buf_count, const int32_t* buf_first, const int64_t* articles_pop,
+                                 const float* acr, int64_t acr_dim, int64_t acr_ld, const double* acr_norm,
+                                 int64_t num_items, double knn_lambda, double knn_alpha, int32_t enabled, int32_t top_n,
+                                 int64_t max_blocks, int32_t* rank, int64_t* hist, int* err, void* stream);
 
 /* ---- session-based kNN baseline, V-SkNN / SkNN (csrc/sknn.cu, spec oracle/sknn_ref.py) -------------------------------
  * Ring of S slots (logical index i at slot (head + i) % S, count entries, oldest first; head and count are the caller's):
@@ -570,6 +585,17 @@ int nar_sknn_score(const int64_t* ids, const int32_t* lens, const int32_t* items
                    int64_t B, int64_t T, int64_t K, int64_t num_items, int64_t sample_size, int64_t nn, int32_t decay_div,
                    int32_t jaccard, int32_t top_n, int64_t* rank_hist, double* metrics, int64_t* out_ids, int* err,
                    void* stream);
+/* Unsampled ranking (DESIGN.md section 14) with the neighbours of nar_sknn_score: every query (b, t) with label_next != 0
+ * ranks its label against the pool [N] (ascending distinct ids in [1, num_items)) minus the label and the ids of its
+ * session row all_items[b*(T+1) + 0..T], by (item score desc, first neighbour asc, id asc) over the ids some kept
+ * neighbour holds.  rank [B*T] int32 (optional): the competitors before the label, 0x7fffffff when no kept neighbour
+ * holds it, -1 where no query.  hist [top_n + 2] int64 accumulated as in nar_baselines_rank_unsampled.  max_blocks > 0
+ * caps the grid.  NAR_ERR_UNSUPPORTED for S > 4096 or T > 64.                                                        */
+int nar_sknn_rank_unsampled(const int64_t* ids, const int32_t* lens, const int32_t* items, int64_t S, int64_t W, int64_t head,
+                            int64_t count, const int64_t* item_clicked, const int64_t* label_next, const int64_t* all_items,
+                            int64_t B, int64_t T, const int64_t* pool, int64_t N, int64_t num_items, int64_t sample_size,
+                            int64_t nn, int32_t decay_div, int32_t jaccard, int32_t top_n, int64_t max_blocks,
+                            int32_t* rank, int64_t* hist, int* err, void* stream);
 
 /* ---- NDCG, item coverage, ESI-R / ESI-RR and EILD-R / EILD-RR of top-n lists (csrc/eval_metrics.cu, spec
  *      oracle/eval_metrics_ref.py; the reference's metrics.py).  Coverage sets are bitmaps of (num_items + 31) / 32
