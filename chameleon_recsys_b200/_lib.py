@@ -63,6 +63,7 @@ class ModelCfg(C.Structure):
                 ('off_M', C.c_int64 * 4), ('off_c', C.c_int64 * 4), ('ld_M', C.c_int64 * 4),
                 ('off_Wx', C.c_int64 * NAR_MAX_LAYERS), ('off_Wh', C.c_int64 * NAR_MAX_LAYERS), ('off_rb', C.c_int64 * NAR_MAX_LAYERS),
                 ('off_Whc', C.c_int64 * NAR_MAX_LAYERS),
+                ('rnn_residual', C.c_int32), ('off_Wp', C.c_int64), ('off_bp', C.c_int64),
                 ('plan', FeaturePlanC)]
 
 
@@ -156,6 +157,7 @@ _SIGNATURES = {
     'nar_state_update': (C.c_int, [vp, vp, i64, vp, vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, i64, C.c_double, vp, vp]),
     'nar_colsum_add': (C.c_int, [vp, i64, i64, i64, vp, vp]),
     'nar_act_bwd': (C.c_int, [vp, vp, i64, C.c_int, vp, vp]),
+    'nar_residual_add': (C.c_int, [vp, vp, i64, i64, i64, vp, vp]),
     'nar_l2_loss_add': (C.c_int, [vp, i64, f32, vp, vp]),
     'nar_transpose_f32': (C.c_int, [vp, i64, i64, i64, vp, i64, vp]),
     'nar_adam_tf': (C.c_int, [vp, vp, vp, vp, i64, i64, f32, f32, f32, f32, f32, i64, vp, vp]),

@@ -60,6 +60,7 @@ struct StepBufs {
         *UO[NAR_MAX_LAYERS], *RH[NAR_MAX_LAYERS];
   // per cell: GT = UGRNN gate / GRU r (LSTM: none); CD = UGRNN and GRU candidate / LSTM cell state; UO = GRU u;
   // RH = GRU r * previous state.  The LSTM's activated gates replace its pre-activations in GX.
+  float *P, *HR[NAR_MAX_LAYERS];   // residual stack: layer 0's input projection, each layer's output HO + its input
   float *PP, *PI, *PC, *DB;        // dedup: layer-1 pre-activations and their gradients
   float* H1cT; int64_t ldr;        // dedup: the candidate rows of H1 transposed, [C, ldr], ldr >= L_cap * n_cand
 };
@@ -146,6 +147,10 @@ void session_carve(const nar_model_cfg& c, int64_t L, Carver& cv, StepBufs* sb) 
   }
   sb->F1 = cv.take<float>(L * 512);
   sb->PR = cv.take<float>(L * c.C);
+  if (c.rnn_residual) {
+    sb->P = cv.take<float>(L * Hp);
+    for (int i = 0; i < c.layers; ++i) sb->HR[i] = cv.take<float>(L * Hp);
+  }
 }
 
 int64_t step_carve(const nar_engine* e, int64_t L_cap, int train, void* base, StepBufs* sb) {
@@ -326,7 +331,8 @@ struct Seq {
 // :1308-1342) + FC1 / FC2 (:410-438) -> sb.PR - forked onto the auxiliary stream, so that it runs under whatever the
 // caller queues next on main (the candidate rows); the caller joins before reading sb.PR.  (Moving the two CAR GEMMs
 // into the session branch as well was measured neutral and is not used: DESIGN.md section 6.)  `drop`: training-step
-// dropout on the RNN outputs and FC1.
+// dropout on the RNN outputs and FC1.  Residual stack (c.rnn_residual, DESIGN.md section 15): layer 0 reads P = E Wp + bp,
+// and each layer's output HR = HO + its input feeds dropout, the next layer and FC1; HO stays the cell's own state.
 void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
   const nar_model_cfg& c = s.c;
   const nar_step_io* io = s.io;
@@ -335,10 +341,14 @@ void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
   s.fwd(sb.H1, C, c.off_W2, C, c.off_b2, sb.E, C, L, C, C, NAR_ACT_TANH, s.main);
   cudaStream_t st = s.fork();
   const float* rnn_in = sb.E; int64_t n_in = C;
+  if (c.rnn_residual) {            // InputProjectionWrapper: no activation
+    s.fwd(sb.E, C, c.off_Wp, Hp, c.off_bp, sb.P, Hp, L, Hp, C, NAR_ACT_NONE, st);
+    rnn_in = sb.P; n_in = Hp;
+  }
   const int64_t gw = gate_blocks(c) * Hp;
   for (int i = 0; i < c.layers; ++i) {
     // input projection gx = x Wx + b, then the recurrence (csrc/rnn.cu)
-    s.fwd(rnn_in, i == 0 ? C : Hp, c.off_Wx[i], gw, c.off_rb[i], sb.GX[i], gw, L, gw, n_in, NAR_ACT_NONE, st);
+    s.fwd(rnn_in, n_in, c.off_Wx[i], gw, c.off_rb[i], sb.GX[i], gw, L, gw, n_in, NAR_ACT_NONE, st);
     if (c.rnn_cell == NAR_CELL_GRU) {
       s.chk(nar_gru_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), s.W(c.off_Whc[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.UO[i],
                         sb.CD[i], sb.RH[i], st));
@@ -348,9 +358,12 @@ void clicked_rows_forward(Seq& s, const StepBufs& sb, int64_t L, bool drop) {
     } else {
       s.chk(nar_ugrnn_fwd(s.e->ctx, sb.GX[i], s.W(c.off_Wh[i]), io->sess_off, B, Hp, sb.HO[i], sb.GT[i], sb.CD[i], st));
     }
+    // ResidualWrapper: the output is cell(x) + x, the state the cell carries is its own
+    const float* out = sb.HO[i];
+    if (c.rnn_residual) { s.chk(nar_residual_add(sb.HO[i], rnn_in, L, Hp, Hp, sb.HR[i], st)); out = sb.HR[i]; }
     // DropoutWrapper(output_keep_prob) (nar_model.py:1330-1333): the cell's OUTPUT is dropped, its state is not
-    if (drop) s.dropout(sb.HO[i], sb.HOd[i], L, Hp, io->pos_idx, 8 + i, st);
-    rnn_in = drop ? sb.HOd[i] : sb.HO[i]; n_in = Hp;
+    if (drop) s.dropout(out, sb.HOd[i], L, Hp, io->pos_idx, 8 + i, st);
+    rnn_in = drop ? sb.HOd[i] : out; n_in = Hp;
   }
   s.fwd(rnn_in, Hp, c.off_W3, 512, c.off_b3, sb.F1, 512, L, 512, Hp, NAR_ACT_LEAKY_RELU, st);
   if (drop) s.dropout(sb.F1, sb.F1, L, 512, io->pos_idx, 4, st);                                // nar_model.py:417-419
@@ -454,14 +467,16 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
     { cudaStream_t st = s.fork(); s.wgrad(sb.F1, 512, sb.dPR, C, c.off_W4, C, 512, C, L, st); s.bgrad(sb.dPR, C, L, C, c.off_b4, st); }
     s.dgrad(sb.dPR, C, c.off_W4, C, sb.dF1, 512, L, 512, C, NAR_ACT_LEAKY_RELU, sb.F1, 512, 0, main);
     if (drop) s.dropout(sb.dF1, sb.dF1, L, 512, io->pos_idx, 4, main); // F1 holds the dropped activations: re-apply the mask to the gradient
-    const float* rnn_out = drop ? sb.HOd[c.layers - 1] : sb.HO[c.layers - 1];
+    const float* rnn_out = drop ? sb.HOd[c.layers - 1] : (c.rnn_residual ? sb.HR[c.layers - 1] : sb.HO[c.layers - 1]);
     { cudaStream_t st = s.fork(); s.wgrad(rnn_out, Hp, sb.dF1, 512, c.off_W3, 512, Hp, 512, L, st); s.bgrad(sb.dF1, 512, L, 512, c.off_b3, st); }
     s.dgrad(sb.dF1, 512, c.off_W3, 512, sb.dHO, Hp, L, Hp, 512, NAR_ACT_NONE, nullptr, 0, 0, main);
     float* dho = sb.dHO;
     for (int i = c.layers - 1; i >= 0; --i) {
       if (drop) s.dropout(dho, dho, L, Hp, io->pos_idx, 8 + i, main);   // gradient of the dropped cell output
-      const float* x_in = i == 0 ? sb.E : (drop ? sb.HOd[i - 1] : sb.HO[i - 1]);
-      const int64_t n_in = i == 0 ? C : Hp;
+      // dho now holds the gradient of the layer's output before dropout: the cell's d_hout and, with residual
+      // connections, also the gradient of the layer's input through the skip path
+      const float* x_in = i == 0 ? (c.rnn_residual ? sb.P : sb.E) : (drop ? sb.HOd[i - 1] : (c.rnn_residual ? sb.HR[i - 1] : sb.HO[i - 1]));
+      const int64_t n_in = (i == 0 && !c.rnn_residual) ? C : Hp;
       // gx, Wx and the bias are gw wide; the recurrent blocks differ per cell
       const int64_t gw = gate_blocks(c) * Hp;
       if (c.rnn_cell == NAR_CELL_GRU) {
@@ -488,7 +503,14 @@ int run_step(nar_engine* e, const nar_step_io* io, cudaStream_t main) {
         }
         s.bgrad(sb.dGX[i], gw, L, gw, c.off_rb[i], st);
       }
-      if (i == 0) {
+      if (c.rnn_residual) {
+        // d(input) = dGX Wx^T + dho: accumulated onto dho once the cell's backward has read it (layer 0: dP)
+        s.dgrad(sb.dGX[i], gw, c.off_Wx[i], gw, dho, Hp, L, Hp, gw, NAR_ACT_NONE, nullptr, 0, 1, main);
+        if (i == 0) {
+          { cudaStream_t st = s.fork(); s.wgrad(sb.E, C, dho, Hp, c.off_Wp, Hp, C, Hp, L, st); s.bgrad(dho, Hp, L, Hp, c.off_bp, st); }
+          s.dgrad(dho, Hp, c.off_Wp, Hp, sb.dE, C, L, C, Hp, NAR_ACT_TANH, sb.E, C, 0, main);      // clicked rows of dE (pre-tanh)
+        }
+      } else if (i == 0) {
         s.dgrad(sb.dGX[0], gw, c.off_Wx[0], gw, sb.dE, C, L, C, gw, NAR_ACT_TANH, sb.E, C, 0, main);   // clicked rows of dE (pre-tanh)
       } else {
         s.dgrad(sb.dGX[i], gw, c.off_Wx[i], gw, sb.dHOb[i], Hp, L, Hp, gw, NAR_ACT_NONE, nullptr, 0, 0, main);
@@ -694,8 +716,9 @@ int planes_build(nar_engine* e) {
   add(c.off_M[0], C, 128, c.ld_M[0]); add(c.off_M[1], 128, 64, c.ld_M[1]); add(c.off_M[2], 64, 32, c.ld_M[2]);
   for (int i = 0; i < c.layers; ++i) {
     const int64_t gw = gate_blocks(c) * Hp;
-    add(c.off_Wx[i], i == 0 ? C : Hp, gw, gw);
+    add(c.off_Wx[i], (i == 0 && !c.rnn_residual) ? C : Hp, gw, gw);
   }
+  if (c.rnn_residual) add(c.off_Wp, C, Hp, Hp);
   if (overflow) return NAR_ERR_INVALID;
   if (!ps.buf) {
     cudaMalloc(&ps.buf, (size_t)total * sizeof(uint16_t));
@@ -761,7 +784,8 @@ extern "C" int nar_engine_destroy(nar_engine* e) {
 extern "C" int nar_engine_update_cfg(nar_engine* e, const nar_model_cfg* cfg) {
   if (!e || !cfg) return NAR_ERR_INVALID;
   if (cfg->layers != e->cfg.layers || cfg->Hp != e->cfg.Hp || cfg->C != e->cfg.C || cfg->Fp != e->cfg.Fp ||
-      cfg->rnn_cell != e->cfg.rnn_cell) return NAR_ERR_INVALID;        // structural changes need a new engine
+      cfg->rnn_cell != e->cfg.rnn_cell || cfg->rnn_residual != e->cfg.rnn_residual)
+    return NAR_ERR_INVALID;        // structural changes need a new engine
   e->cfg = *cfg;
   return planes_build(e);               // the parameter buffer may have changed (share_params)
 }
@@ -872,7 +896,9 @@ extern "C" int nar_engine_buffer(const nar_engine* e, const nar_step_io* io, con
       {"logits", sb.logits, L, n_cand}, {"PD", sb.PD, Rc, c.C}, {"Z1", sb.Z1, Rc, 128}, {"Z2", sb.Z2, Rc, 64}, {"Z3", sb.Z3, Rc, 32}, {"PP", sb.PP, L, c.C},
       {"PI", sb.PI, pb.U, c.C}, {"PC", sb.PC, L, c.C}, {"DB", sb.DB, 3 * L + pb.U, c.C},
       {"HO0", sb.HO[0], L, c.Hp}, {"HO1", sb.HO[1], L, c.Hp}, {"HO2", sb.HO[2], L, c.Hp}, {"HO3", sb.HO[3], L, c.Hp},
-      {"HOd0", sb.HOd[0], L, c.Hp}, {"HOd1", sb.HOd[1], L, c.Hp}, {"HOd2", sb.HOd[2], L, c.Hp}, {"HOd3", sb.HOd[3], L, c.Hp}};
+      {"HOd0", sb.HOd[0], L, c.Hp}, {"HOd1", sb.HOd[1], L, c.Hp}, {"HOd2", sb.HOd[2], L, c.Hp}, {"HOd3", sb.HOd[3], L, c.Hp},
+      {"P", sb.P, L, c.Hp}, {"HR0", sb.HR[0], L, c.Hp}, {"HR1", sb.HR[1], L, c.Hp}, {"HR2", sb.HR[2], L, c.Hp},
+      {"HR3", sb.HR[3], L, c.Hp}};
   for (const Ent& t : tab)
     if (strcmp(t.n, name) == 0) {
       *ptr = t.p;

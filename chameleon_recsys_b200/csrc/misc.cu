@@ -116,6 +116,18 @@ dropout_rows_kernel(const float* __restrict__ src, float* __restrict__ dst, int6
   }
 }
 
+// the residual session stack's layer output: out = h + res, 4 columns per thread (out may alias h or res)
+__global__ void __launch_bounds__(256)
+residual_add_kernel(const float* h, const float* res, int64_t rows, int cols4, int64_t ld, float* out) {
+  const int64_t total = rows * cols4;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / cols4; const int64_t o = r * ld + 4 * (i - r * cols4);
+    const float4 a = *reinterpret_cast<const float4*>(h + o);
+    const float4 b = *reinterpret_cast<const float4*>(res + o);
+    *reinterpret_cast<float4*>(out + o) = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+}
+
 static unsigned grid_for(int64_t n, int per_block) {
   int64_t g = (n + per_block - 1) / per_block;
   const int64_t cap = NAR_GRID_SMS * 8;
@@ -240,6 +252,16 @@ extern "C" int nar_act_bwd(const float* dy, const float* y, int64_t n, int act, 
   if (!dy || !y || !dx) return NAR_ERR_INVALID;
   if (n <= 0) return NAR_OK;
   nar::misc::act_bwd_kernel<<<nar::misc::grid_for(n, 1024), 256, 0, as_stream(stream)>>>(dy, y, n, act, dx);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_residual_add(const float* h, const float* res, int64_t rows, int64_t cols, int64_t ld, float* out,
+                                void* stream) {
+  if (!h || !res || !out || cols < 0 || (cols & 3) || (ld & 3) || ld < cols) return NAR_ERR_INVALID;
+  if (rows <= 0 || cols == 0) return NAR_OK;
+  nar::misc::residual_add_kernel<<<nar::misc::grid_for(rows * (cols / 4), 256), 256, 0, as_stream(stream)>>>(
+      h, res, rows, (int)(cols / 4), ld, out);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

@@ -61,7 +61,7 @@ class NarEngine:
                  ranking: str = 'mlp', rnn_cell: str = 'ugrnn', sampler_seed: int = 42, device: Optional[int] = None,
                  fwd_precision: int = 4, bwd_precision: int = 1, process_group=None, max_batch: int = 0,
                  dedup: bool = True, keep_prob: float = 1.0, novelty_reg_factor: float = 0.0,
-                 dropout_seed: Optional[int] = None):
+                 dropout_seed: Optional[int] = None, rnn_residual: bool = False):
         if not torch.cuda.is_available():
             raise NarError('NarEngine needs a CUDA (sm_90a) device; there is no CPU fallback')
         if rnn_cell not in ('ugrnn', 'gru', 'lstm'):
@@ -70,6 +70,10 @@ class NarEngine:
         if rnn_cell != getattr(layout, 'rnn_cell', 'ugrnn'):
             raise ValueError('ParamLayout was built for rnn_cell=%r' % getattr(layout, 'rnn_cell', 'ugrnn'))
         self.rnn_cell = rnn_cell
+        # residual session stack (DESIGN.md section 15): the layout holds the projection and a wider layer-0 kernel
+        self.rnn_residual = bool(rnn_residual)
+        if self.rnn_residual != getattr(layout, 'residual', False):
+            raise ValueError('ParamLayout was built for rnn_residual=%r' % getattr(layout, 'residual', False))
         if ranking not in ('mlp', 'cosine'):
             raise ValueError(ranking)
         self.dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
@@ -195,6 +199,8 @@ class NarEngine:
             c.off_Wx[i], c.off_Wh[i], c.off_rb[i] = off('rnn%d/Wx' % i), off('rnn%d/Wh' % i), off('rnn%d/b' % i)
             if self.rnn_cell == 'gru':
                 c.off_Whc[i] = off('rnn%d/Whc' % i)
+        if self.rnn_residual:
+            c.rnn_residual, c.off_Wp, c.off_bp = 1, off('rnn0/Wp'), off('rnn0/bp')
         c.plan = self._plan_c_static()
         return c
 
@@ -250,6 +256,12 @@ class NarEngine:
         self.load_state_dict({'params': params, 'adam_m': adam_m, 'adam_v': adam_v, 'global_step': global_step})
 
     def load_state_dict(self, sd: dict):
+        # every variable of this layout in every group before anything is written: a checkpoint of another model (e.g.
+        # the other rnn_residual_connections setting) raises instead of loading part of a model
+        for group in ('params', 'adam_m', 'adam_v'):
+            missing = [n for n in self.layout.logical_names() if n not in sd[group]]
+            if missing:
+                raise KeyError('%s: no variable %s (%d of this model\'s variables missing)' % (group, missing[0], len(missing)))
         self.params.copy_(torch.from_numpy(self.layout.to_internal(sd['params'])))
         self.adam_m.copy_(torch.from_numpy(self.layout.to_internal(sd['adam_m'])))
         self.adam_v.copy_(torch.from_numpy(self.layout.to_internal(sd['adam_v'])))
@@ -562,8 +574,9 @@ class NarEngine:
             xin, xpos, xu = X[:L], X[L:2 * L], X[2 * L:]
             xneg = torch.cat([xu[uidx][..., :c0], xin[:, None, c0:].expand(L, K, X.shape[1] - c0)], dim=2)
             X = torch.cat([xin, torch.cat([xpos[:, None, :], xneg], dim=1).reshape(L * n_cand, -1)], dim=0)
-        # with dropout the RNN OUTPUT the reference exposes is the dropped one (DropoutWrapper); the state is HO<i>
-        ho = 'HOd%d' if (self.keep_prob < 1.0 and train) else 'HO%d'
+        # with dropout the RNN OUTPUT the reference exposes is the dropped one (DropoutWrapper); the state is HO<i>.  A
+        # residual stack's output is HR<i> = HO<i> + the layer's input
+        ho = 'HOd%d' if (self.keep_prob < 1.0 and train) else ('HR%d' if self.rnn_residual else 'HO%d')
         extra = {n: b(n) for n in ('Z1', 'Z2', 'Z3')} if self.ranking == 'mlp' else {}
         return dict(X=X.clone(), H1=H1, E=b('E'), **extra, HO=[b(ho % i) for i in range(self.layers)], F1=b('F1'), PR=b('PR'),
                     logits=b('logits'), row_pos=b('row_pos').view(-1), row_item=b('row_item').view(-1),

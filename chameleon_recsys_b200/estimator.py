@@ -85,6 +85,7 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
                            popularity_smooth_log_base=params.get('popularity_smooth_log_base', 2.0),
                            max_cardinality_for_ohe=params.get('max_cardinality_for_ohe', 10),
                            rnn_cell=params.get('rnn_cell', 'ugrnn'), ranking=params.get('ranking', 'mlp'),
+                           rnn_residual_connections=bool(params.get('rnn_residual_connections', False)),
                            sampler_seed=params.get('sampler_seed', 42), init_seed=params.get('init_seed', 42),
                            process_group=params.get('process_group'), device=params.get('device'))
 

@@ -54,7 +54,8 @@ def make_problem(name_or_wl, profile=None, session_len=None, seed: int = 42, sta
     icfg = get_internal_enabled_features_config(hp.enabled_internal_features)
     acr, meta = make_catalog(V, E, acfg, hp.content_embedding_scale_factor, seed=seed)
     plan = FeaturePlan(scfg, acfg, icfg, hp.max_cardinality_for_ohe, E, V)
-    layout = ParamLayout(plan, hp.CAR_embedding_size, hp.rnn_units, hp.rnn_num_layers, rnn_cell=hp.rnn_cell)
+    layout = ParamLayout(plan, hp.CAR_embedding_size, hp.rnn_units, hp.rnn_num_layers, rnn_cell=hp.rnn_cell,
+                         residual=hp.rnn_residual_connections)
     state = (state_cls or ClickedItemsState)(hp.recent_clicks_buffer_hours, hp.recent_clicks_buffer_max_size,
                               hp.recent_clicks_for_normalization, V)
     stream = SessionStream(V, scfg, hp.truncate_session_length, wl.session_len, seed=seed,

@@ -138,6 +138,9 @@ class NARHParams:
     max_cardinality_for_ohe: int = 10
     # --- extensions (documented in DESIGN.md) ---
     rnn_cell: str = 'ugrnn'          # 'ugrnn' = reference code (nar_model.py:1317)
+    # build_rnn's residual_connections (nar_model.py:1319-1323; the reference calls it with the default False): layer 0
+    # projects its input to rnn_units and adds it to the cell's output, layers > 0 add their input (DESIGN.md section 15)
+    rnn_residual_connections: bool = False
     ranking: str = 'mlp'             # 'mlp' = reference code (nar_model.py:447-500); 'cosine' = north_star wording
     sampler_seed: int = 42           # RANDOM_SEED, nar_trainer_gcom.py:33
     init_seed: int = 42
@@ -207,6 +210,8 @@ class NARHParams:
             params['eval_unsampled_metrics'] = True
         if self.eval_unsampled_benchmarks:
             params['eval_unsampled_benchmarks'] = True
+        if self.rnn_residual_connections:
+            params['rnn_residual_connections'] = True
         return params
 
     def copy(self, **kw) -> 'NARHParams':

@@ -50,7 +50,7 @@ class NARModuleModel:
                  eval_cold_start=False,
                  # --- extensions (not in the reference signature) ---
                  rnn_cell='ugrnn', ranking='mlp', sampler_seed=42, init_seed=42, device=None,
-                 process_group=None, fwd_precision=4, bwd_precision=1):
+                 process_group=None, fwd_precision=4, bwd_precision=1, rnn_residual_connections=False):
         from .engine import NarEngine          # imports torch + the CUDA library; fails loudly without them
         self.mode = mode
         self.lr = lr
@@ -71,7 +71,8 @@ class NARModuleModel:
         self.plan = FeaturePlan(session_features_config, articles_features_config, internal_features_config,
                                 max_cardinality_for_ohe, content_article_embeddings_matrix.shape[1],
                                 self.items_vocab_size)
-        self.layout = ParamLayout(self.plan, CAR_embedding_size, rnn_units, rnn_num_layers, rnn_cell=rnn_cell)
+        self.layout = ParamLayout(self.plan, CAR_embedding_size, rnn_units, rnn_num_layers, rnn_cell=rnn_cell,
+                                  residual=rnn_residual_connections)
         self.engine = NarEngine(self.plan, self.layout, content_article_embeddings_matrix, articles_metadata,
                                 negative_samples=negative_samples,
                                 negative_sample_from_buffer=negative_sample_from_buffer,
@@ -80,7 +81,8 @@ class NARModuleModel:
                                 recent_clicks_for_normalization=recent_clicks_for_normalization,
                                 elapsed_days_smooth_log_base=elapsed_days_smooth_log_base,
                                 popularity_smooth_log_base=popularity_smooth_log_base, ranking=ranking,
-                                rnn_cell=rnn_cell, sampler_seed=sampler_seed, device=device,
+                                rnn_cell=rnn_cell, rnn_residual=rnn_residual_connections,
+                                sampler_seed=sampler_seed, device=device,
                                 process_group=process_group, fwd_precision=fwd_precision,
                                 bwd_precision=bwd_precision,
                                 keep_prob=keep_prob if mode == ModeKeys.TRAIN else 1.0,

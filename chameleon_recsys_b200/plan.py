@@ -213,9 +213,10 @@ class ParamLayout:
     """Flat-buffer layout.  ``tensors`` in buffer order; regularised ones first."""
 
     def __init__(self, plan: FeaturePlan, CAR_embedding_size: int, rnn_units: int, rnn_num_layers: int,
-                 rnn_cell: str = 'ugrnn'):
+                 rnn_cell: str = 'ugrnn', residual: bool = False):
         self.plan = plan
         self.rnn_cell = rnn_cell
+        self.residual = bool(residual)
         C = int(CAR_embedding_size)
         H = int(rnn_units)
         self.C, self.H, self.layers = C, H, int(rnn_num_layers)
@@ -272,10 +273,19 @@ class ParamLayout:
             raise ValueError('rnn_cell=%r: one of %s' % (rnn_cell, sorted(cells)))
         scope, kernels = cells[rnn_cell]
         G = sum(n for _, n, _, _ in kernels)
+        if self.residual:
+            # build_rnn(residual_connections=True) (nar_model.py:1319-1323): layer 0 is InputProjectionWrapper(ResidualWrapper(
+            # cell), H), whose scope holds the projection's _Linear kernel [C, H] (the scope's xavier) and bias [H] (zeros)
+            # and the cell's variables; layers > 0 keep their names (ResidualWrapper opens no scope).  DESIGN.md section 15
+            proj = 'main/RNN/rnn/multi_rnn_cell/cell_0/input_projection_wrapper/'
+            noreg.append(ParamTensor('rnn0/Wp', proj + 'kernel', (C, H), INIT_XAVIER, False, rows=C, ld=Hp,
+                                     col_map=np.arange(H)))
+            noreg.append(ParamTensor('rnn0/bp', proj + 'bias', (H,), INIT_ZEROS, False, rows=1, ld=Hp, col_map=np.arange(H)))
         for i in range(self.layers):
-            n_in = C if i == 0 else H
-            n_in_p = C if i == 0 else Hp
-            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/'.format(i) + scope
+            n_in = C if (i == 0 and not self.residual) else H
+            n_in_p = C if (i == 0 and not self.residual) else Hp
+            base = 'main/RNN/rnn/multi_rnn_cell/cell_{}/'.format(i) + \
+                ('input_projection_wrapper/' if (i == 0 and self.residual) else '') + scope
             wx, b = 'rnn%d/Wx' % i, 'rnn%d/b' % i
             g0 = 0
             for prefix, n, b_init, wh in kernels:

@@ -407,6 +407,9 @@ int nar_act_bwd(const float* dy, const float* y, int64_t n, int act, float* dx, 
 /* out[0] += scale * sum(x^2) / 2  (l2_regularizer, nar_model.py:655)                       */
 int nar_l2_loss_add(const float* x, int64_t n, float scale, float* out, void* stream);
 int nar_transpose_f32(const float* src, int64_t rows, int64_t cols, int64_t ld_src, float* dst, int64_t ld_dst, void* stream);
+/* out[r, c] = h[r, c] + res[r, c] over rows x cols, all three with leading dimension ld (the residual session stack's
+ * layer output: the cell's h plus the layer input).  cols and ld multiples of 4; out may be h or res.                */
+int nar_residual_add(const float* h, const float* res, int64_t rows, int64_t cols, int64_t ld, float* out, void* stream);
 
 /* ---- optimiser (replaces tf.train.AdamOptimizer(lr,.9,.999,1e-8) nar_model.py:708-722;
  *      TF form: lr_t = lr*sqrt(1-b2^t)/(1-b1^t); w -= lr_t*m/(sqrt(v)+eps); the gradient of
@@ -454,6 +457,10 @@ typedef struct {
   /* per layer: Wx [in, G*Hp] and b [G*Hp], G gate blocks: UGRNN (gate | candidate), GRU (r | u | candidate), LSTM (i | j | f | o);
    * Wh [Hp, G*Hp], except the GRU's Wh [Hp, 2Hp] (r | u) and Whc [Hp, Hp] (candidate: a product with r*h) */
   int64_t off_Wx[NAR_MAX_LAYERS], off_Wh[NAR_MAX_LAYERS], off_rb[NAR_MAX_LAYERS], off_Whc[NAR_MAX_LAYERS];
+  /* residual session stack (build_rnn(residual_connections=True), nar_model.py:1319-1323): layer 0 reads the projection
+   * P = E*Wp + bp (Wp [C, Hp], bp [Hp]) and outputs cell(P) + P, layer i > 0 outputs cell(x) + x; 0 = plain stack */
+  int32_t rnn_residual;
+  int64_t off_Wp, off_bp;
   /* feature plan: static part (segments, tables, metadata, created_at_ts, gamma / beta, column map) */
   nar_feature_plan plan;
 } nar_model_cfg;

@@ -19,11 +19,16 @@ from chameleon_recsys_b200.harness import make_problem, warm_state  # noqa: E402
 from oracle import sampler_ref  # noqa: E402
 from oracle.lstm_ref import LstmOracle  # noqa: E402
 from oracle.nar_oracle import NarOracle  # noqa: E402
+from oracle.residual_ref import ResidualOracle  # noqa: E402
 
 
-def make_oracle(pb, dtype=torch.float64):
+def make_oracle(pb, dtype=torch.float64, residual=None):
+    """The oracle of ``pb``'s model; ``residual`` (default: hp.rnn_residual_connections) builds the residual session
+    stack of oracle/residual_ref.py."""
     hp = pb.hp
-    return (LstmOracle if hp.rnn_cell == 'lstm' else NarOracle)(pb.session_features_config, pb.articles_features_config, pb.internal_features_config,
+    residual = hp.rnn_residual_connections if residual is None else residual
+    cls = ResidualOracle if residual else (LstmOracle if hp.rnn_cell == 'lstm' else NarOracle)
+    return cls(pb.session_features_config, pb.articles_features_config, pb.internal_features_config,
                      pb.content_article_embeddings_matrix, pb.articles_metadata,
                      negative_samples=hp.train_total_negative_samples, softmax_temperature=hp.softmax_temperature,
                      reg_weight_decay=hp.reg_l2, recent_clicks_for_normalization=hp.recent_clicks_for_normalization,
@@ -46,7 +51,7 @@ def make_engine(pb, **kw):
                      elapsed_days_smooth_log_base=hp.elapsed_days_smooth_log_base,
                      popularity_smooth_log_base=hp.popularity_smooth_log_base, ranking=hp.ranking, rnn_cell=hp.rnn_cell,
                      sampler_seed=hp.sampler_seed, keep_prob=hp.dropout_keep_prob, novelty_reg_factor=hp.novelty_reg_factor,
-                     **kw)
+                     rnn_residual=hp.rnn_residual_connections, **kw)
 
 
 def rel(a, b):

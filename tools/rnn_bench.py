@@ -5,7 +5,9 @@ process, median of the rounds), the recurrence kernels' device time per training
 after the timing), and the recurrent weight bytes the kernels stream per session-step (from the shapes: the recurrent
 matrices are read once per CTA step and shared by the SB = 4 sessions of a CTA).  Prints one JSON line with the GPU
 name, power limit and max SM clock.  Writes nothing.
-Usage: python tools/rnn_bench.py [--rounds 3] [--steps 20] [--profile-steps 5]"""
+--residual: per cell, the plain stack and the residual stack (rnn_residual_connections, DESIGN.md section 15) instead,
+alternated in one process, one pair of engines per cell; interactions/s of each round and their medians.
+Usage: python tools/rnn_bench.py [--rounds 3] [--steps 20] [--profile-steps 5] [--residual]"""
 from __future__ import annotations
 
 import argparse
@@ -33,8 +35,8 @@ WH_COLS = {'ugrnn': 2, 'gru': 3, 'lstm': 4}
 SB = 4
 
 
-def make_engine(cell, n_batches):
-    pb = make_problem('g1', profile='B', rnn_cell=cell)
+def make_engine(cell, n_batches, residual=False):
+    pb = make_problem('g1', profile='B', rnn_cell=cell, rnn_residual_connections=residual)
     warm_state(pb, 3)
     batches = make_batches(pb, n_batches, pb.hp.batch_size)
     est = build_estimator(None, pb.content_article_embeddings_matrix, pb.articles_metadata, pb.articles_features_config,
@@ -81,15 +83,39 @@ def kernel_us_per_step(eng, staged, cell):
     return out
 
 
+def residual_main(args, res, warmup):
+    """Plain and residual stack of each cell, alternated round by round."""
+    res['train_interactions_per_s'], res['train_interactions_per_s_rounds'], res['launches_per_step'] = {}, {}, {}
+    for c in CELLS:
+        engs = {r: make_engine(c, warmup + args.steps, residual=r) for r in (False, True)}
+        rates = {False: [], True: []}
+        for _ in range(args.rounds):
+            for r in (False, True):
+                n0 = engs[r][0].launches
+                rates[r].append(train_rate(*engs[r], warmup)[0])
+                res['launches_per_step'].setdefault(c, {})[('on' if r else 'off')] = \
+                    (engs[r][0].launches - n0) // (warmup + args.steps)
+        for r in (False, True):
+            k = '%s_%s' % (c, 'on' if r else 'off')
+            res['train_interactions_per_s'][k] = round(float(np.median(rates[r])), 1)
+            res['train_interactions_per_s_rounds'][k] = [round(v, 1) for v in rates[r]]
+        del engs
+        torch.cuda.empty_cache()
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--rounds', type=int, default=3)
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--profile-steps', type=int, default=5)
+    ap.add_argument('--residual', action='store_true', help='plain vs residual session stack per cell')
     args = ap.parse_args()
     name, limit = gpu_info()
     res = {'gpu': name, 'power_limit_and_max_sm_clock': limit, 'workload': 'g1', 'batch': 256}
     warmup = 5
+    if args.residual:
+        return residual_main(args, res, warmup)
     engs = {c: make_engine(c, warmup + args.steps) for c in CELLS}
     Hp = engs['lstm'][0].Hp
     res['Hp'] = Hp
