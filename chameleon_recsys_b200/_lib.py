@@ -76,7 +76,7 @@ class StepIO(C.Structure):
                 ('ctx_int', C.c_void_p * NAR_MAX_SRC), ('ctx_float', C.c_void_p * NAR_MAX_SRC),
                 ('pos_idx', C.c_void_p), ('sess_off', C.c_void_p),
                 ('prep_ws', C.c_void_p), ('prep_ws_bytes', C.c_int64), ('ws', C.c_void_p), ('ws_bytes', C.c_int64),
-                ('loss', C.c_void_p)]
+                ('loss', C.c_void_p), ('stats', C.c_void_p)]
 
 
 class NoveltyReg(C.Structure):

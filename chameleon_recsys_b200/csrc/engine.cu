@@ -629,12 +629,14 @@ int run_candidate_blocks(nar_engine* e, const nar_step_io* io, const int64_t* q_
   StepBufs& sb = rb.sb;
   Seq s(e, io, main);
 
-  // ---- rows, statistics (empty buffer: the candidate rows are group 2, like the negatives), one gather
+  // ---- rows, statistics (empty buffer: the candidate rows are group 2, like the negatives), one gather.  io->stats:
+  // statistics the caller computed instead (a data-parallel rank's, over the global batch's rows)
   s.chk(nar::recommend_rows(io->pos_idx, L, io->item_clicked, cand_ids, N, rb.row_pos, rb.row_item, main));
-  s.chk(nar_feature_stats(e->ctx, io->buffer, c.buf_len, c.n_norm, c.plan.created_at_ts, io->pop_norm, io->max_ts,
-                          c.plan.log_base_recency, c.plan.log_base_novelty, rb.row_pos, rb.row_item, L + N, L, 0, io->event_ts,
-                          rb.stats, main));
-  const nar_feature_plan plan = call_plan(c, io, rb.stats);
+  if (!io->stats)
+    s.chk(nar_feature_stats(e->ctx, io->buffer, c.buf_len, c.n_norm, c.plan.created_at_ts, io->pop_norm, io->max_ts,
+                            c.plan.log_base_recency, c.plan.log_base_novelty, rb.row_pos, rb.row_item, L + N, L, 0, io->event_ts,
+                            rb.stats, main));
+  const nar_feature_plan plan = call_plan(c, io, io->stats ? io->stats : rb.stats);
   nar_row_layout rl;
   rl.n_rows = L + N; rl.n_input = L; rl.n_cand = 0; rl.n_positive = 0; rl.n_full = L; rl.ctx_col0 = c0;
   s.chk(nar_gather_features(e->ctx, &plan, rb.row_pos, rb.row_item, &rl, io->event_ts, io->max_ts, sb.X, main));

@@ -23,7 +23,7 @@ import torch
 
 from . import ops
 from ._lib import FeaturePlanC, ModelCfg, NarError, StepIO, check
-from .dp import shard_sessions
+from .dp import gather_query_rows, query_counts, query_weights, session_lengths, shard_bounds, shard_sessions
 from .plan import (SEG_ACR, SEG_CTX_EMBED, SEG_ITEM_EMB, SEG_META_EMBED, FeaturePlan, ParamLayout, round_up)
 
 _NP2T = {np.int64: torch.int64, np.float32: torch.float32, np.int32: torch.int32}
@@ -352,10 +352,12 @@ class NarEngine:
 
     # ------------------------------------------------------------------ staging (host -> HBM, one copy)
     def stage(self, features: Dict[str, np.ndarray], labels: Dict[str, np.ndarray], buffer: Optional[np.ndarray],
-              pop_norm: Optional[np.ndarray], slot: str = 'stage', stream: Optional[torch.cuda.Stream] = None) -> dict:
+              pop_norm: Optional[np.ndarray], slot: str = 'stage', stream: Optional[torch.cuda.Stream] = None,
+              shard_weights: Optional[np.ndarray] = None) -> dict:
         """Pack the step inputs into one pinned buffer and issue one async H2D copy.
         ``features``/``labels`` hold the GLOBAL batch (all data-parallel ranks see the same arrays).  ``buffer`` /
-        ``pop_norm`` None: the device-resident state is read instead (attach_device_state)."""
+        ``pop_norm`` None: the device-resident state is read instead (attach_device_state).  ``shard_weights``: the work
+        of each session the data-parallel shards balance (dp.shard_bounds; None: its valid positions)."""
         item_clicked = np.ascontiguousarray(features['item_clicked'], dtype=np.int64)
         Bg, T = item_clicked.shape
         use_dstate = buffer is None
@@ -367,7 +369,8 @@ class NarEngine:
             if buffer.size != self.buf_len:
                 raise ValueError('recent-clicks buffer has %d entries, engine was built for %d' % (buffer.size, self.buf_len))
         # this rank's sessions + compact valid positions (session-major; flat index into the GLOBAL [Bg*T] arrays)
-        sh = shard_sessions(np.asarray(features['session_size']), T, self.world, self.rank, balance=self.dp_balance)
+        sh = shard_sessions(np.asarray(features['session_size']), T, self.world, self.rank, balance=self.dp_balance,
+                            weights=shard_weights)
         s0, per, lens, L, L_global = sh['s0'], sh['per'], sh['lens'], sh['L'], sh['L_global']
         sess_off, pos_idx = sh['sess_off'], sh['pos_idx']
         all_items = np.concatenate([item_clicked, np.asarray(labels['label_last_item'], dtype=np.int64).reshape(Bg, 1)], axis=1)
@@ -719,9 +722,13 @@ class NarEngine:
         clicks item_clicked[b, 0..t].  Reads the weights and the given state only (one C call, csrc/engine.cu).
         ``ws_budget``: workspace bytes (default: the engine's budget); smaller budgets run more, smaller blocks with
         bit-identical results.  -> numpy dict: query_session [Q], query_position [Q], predicted_item_ids /
-        predicted_item_scores / predicted_item_probs [Q, top_n], candidates [N]."""
-        if self.world > 1:
-            raise NotImplementedError('recommend runs on one process; data-parallel prediction is not implemented')
+        predicted_item_scores / predicted_item_probs [Q, top_n], candidates [N]; q_block, n_block: this process's blocks.
+        Data parallel (``world > 1``): every rank passes the same batch, state, candidates and arguments (as in
+        training) and gets the dict one process returns for them, bit for bit.  Each rank scores the queries of its
+        contiguous session shard (dp.shard_bounds balanced by queries, dp.query_weights), then ONE all_gather on the
+        engine's process group collects every rank's top n in rank order, which is session order
+        (dp.gather_query_rows).  Every argument check runs before it, so all ranks raise together; a rank without
+        queries joins it with zero rows."""
         if positions not in ('last', 'all'):
             raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
         if buffer is None or pop_norm is None:
@@ -736,51 +743,81 @@ class NarEngine:
         item_clicked = np.asarray(features['item_clicked'])
         Bg, T = item_clicked.shape
         labels = {'label_next_item': np.zeros((Bg, T), dtype=np.int64), 'label_last_item': np.zeros(Bg, dtype=np.int64)}
-        st = self.stage(features, labels, buffer, pop_norm, slot='predict')
-        L, lens = st['L'], st['lens']
-        ends = np.cumsum(lens)
+        # the queries of the global batch, session-major; each rank's shard holds a contiguous run of them
+        lens_g = session_lengths(features['session_size'], T)
+        weights = query_weights(lens_g, positions)
+        st = self.stage(features, labels, buffer, pop_norm, slot='predict', shard_weights=weights)
         if positions == 'last':
-            q_rows = (ends - 1)[lens > 0].astype(np.int64)
-            q_sess = np.flatnonzero(lens > 0).astype(np.int64)
-            q_t = (lens[lens > 0] - 1).astype(np.int64)
+            q_sess = np.flatnonzero(lens_g > 0).astype(np.int64)
+            q_t = (lens_g[lens_g > 0] - 1).astype(np.int64)
         else:
-            q_rows = np.arange(L, dtype=np.int64)
-            q_sess = np.repeat(np.arange(Bg, dtype=np.int64), lens)
-            q_t = np.arange(L, dtype=np.int64) - np.repeat(ends - lens, lens)
-        Q = int(q_rows.size)
+            q_sess = np.repeat(np.arange(Bg, dtype=np.int64), lens_g)
+            q_t = np.arange(q_sess.size, dtype=np.int64) - np.repeat(np.cumsum(lens_g) - lens_g, lens_g)
         out = {'query_session': q_sess, 'query_position': q_t, 'candidates': cand,
-               'predicted_item_ids': np.zeros((Q, top_n), np.int64), 'predicted_item_scores': np.zeros((Q, top_n), np.float32),
-               'predicted_item_probs': np.zeros((Q, top_n), np.float32)}
-        if Q == 0:
-            return out
-        gather_q = positions == 'last'
-        budget = int(self._ws_budget if ws_budget is None else ws_budget)
-        wb, qb, nb = C.c_int64(0), C.c_int64(0), C.c_int64(0)
-        check(self._lib.nar_engine_recommend_workspace_bytes(self._handle, L, Q, N, int(gather_q), budget, C.byref(wb),
-                                                             C.byref(qb), C.byref(nb)), 'nar_engine_recommend_workspace_bytes')
-        self._sync_cfg()
+               'predicted_item_ids': np.zeros((q_sess.size, top_n), np.int64),
+               'predicted_item_scores': np.zeros((q_sess.size, top_n), np.float32),
+               'predicted_item_probs': np.zeros((q_sess.size, top_n), np.float32)}
+        if q_sess.size == 0:
+            return out                                    # on every rank: no query anywhere, no collective
+        counts = query_counts(lens_g, shard_bounds(lens_g, self.world, self.dp_balance, weights), positions)
+        Q, q0 = int(counts[self.rank]), int(counts[:self.rank].sum())
+        L, lens = st['L'], st['lens']
+        # this rank's queries: q_rows = their rows among the L local positions, q_pos = their flat positions b*T+t in the
+        # global [Bg*T] arrays
+        q_rows = ((np.cumsum(lens) - 1)[lens > 0] if positions == 'last' else np.arange(L)).astype(np.int64)
+        assert q_rows.size == Q
         d = self.dev
-        ws = self._buf('rec_ws', int(wb.value), 1, torch.uint8).view(-1)
-        q_pos = torch.from_numpy(q_sess * T + q_t).to(torch.int32).to(d)
-        q_rows_t = torch.from_numpy(q_rows).to(d) if gather_q else None
-        cand_t = torch.from_numpy(cand).to(d)
-        ids = torch.empty(Q, top_n, dtype=torch.int64, device=d)
-        scores = torch.empty(Q, top_n, dtype=torch.float32, device=d)
-        probs = torch.empty(Q, top_n, dtype=torch.float32, device=d)
-        io = self._staged_io(st)
-        io.L_cap, io.global_step, io.train = L, self.global_step, 0
-        io.ws, io.ws_bytes = ws.data_ptr(), ws.numel()
-        cur = torch.cuda.current_stream()
-        check(self._lib.nar_engine_recommend(self._handle, C.byref(io), C.c_void_p(0 if q_rows_t is None else q_rows_t.data_ptr()),
-                                             C.c_void_p(q_pos.data_ptr()), Q, C.c_void_p(cand_t.data_ptr()), N, top_n,
-                                             int(bool(exclude_session_clicks)), int(qb.value), int(nb.value),
-                                             C.c_void_p(ids.data_ptr()), C.c_void_p(scores.data_ptr()),
-                                             C.c_void_p(probs.data_ptr()), C.c_void_p(cur.cuda_stream)), 'nar_engine_recommend')
+        ids = torch.zeros(Q, top_n, dtype=torch.int64, device=d)
+        scores = torch.zeros(Q, top_n, dtype=torch.float32, device=d)
+        probs = torch.zeros(Q, top_n, dtype=torch.float32, device=d)
+        qb, nb = C.c_int64(0), C.c_int64(0)
+        if Q > 0:
+            gather_q = positions == 'last'
+            budget = int(self._ws_budget if ws_budget is None else ws_budget)
+            wb = C.c_int64(0)
+            check(self._lib.nar_engine_recommend_workspace_bytes(self._handle, L, Q, N, int(gather_q), budget, C.byref(wb),
+                                                                 C.byref(qb), C.byref(nb)), 'nar_engine_recommend_workspace_bytes')
+            self._sync_cfg()
+            ws = self._buf('rec_ws', int(wb.value), 1, torch.uint8).view(-1)
+            q_pos = torch.from_numpy(q_sess[q0:q0 + Q] * T + q_t[q0:q0 + Q]).to(torch.int32).to(d)
+            q_rows_t = torch.from_numpy(q_rows).to(d) if gather_q else None
+            cand_t = torch.from_numpy(cand).to(d)
+            io = self._staged_io(st)
+            io.L_cap, io.global_step, io.train = L, self.global_step, 0
+            io.ws, io.ws_bytes = ws.data_ptr(), ws.numel()
+            stats = None
+            if self.world > 1 and not np.any(np.asarray(buffer) != 0):
+                stats = self._batch_row_stats(st, item_clicked, lens_g, cand)
+                io.stats = stats.data_ptr()
+            cur = torch.cuda.current_stream()
+            check(self._lib.nar_engine_recommend(self._handle, C.byref(io), C.c_void_p(0 if q_rows_t is None else q_rows_t.data_ptr()),
+                                                 C.c_void_p(q_pos.data_ptr()), Q, C.c_void_p(cand_t.data_ptr()), N, top_n,
+                                                 int(bool(exclude_session_clicks)), int(qb.value), int(nb.value),
+                                                 C.c_void_p(ids.data_ptr()), C.c_void_p(scores.data_ptr()),
+                                                 C.c_void_p(probs.data_ptr()), C.c_void_p(cur.cuda_stream)), 'nar_engine_recommend')
+        if self.world > 1:
+            ids, scores, probs = gather_query_rows([ids, scores, probs], counts, self.pg)
         out['predicted_item_ids'] = ids.cpu().numpy()
         out['predicted_item_scores'] = scores.cpu().numpy()
         out['predicted_item_probs'] = probs.cpu().numpy()
         out['q_block'], out['n_block'] = int(qb.value), int(nb.value)
         return out
+
+    def _batch_row_stats(self, st: dict, item_clicked: np.ndarray, lens_g: np.ndarray, cand: np.ndarray) -> torch.Tensor:
+        """[24] device: the feature-normalisation statistics of a recommend call over the rows of the GLOBAL batch (its
+        valid positions, then the candidates), as one process computes them.  They depend on the rows only when the
+        recent-clicks buffer is empty: then the clicked rows' recency / novelty are normalised over the clicked rows
+        themselves (csrc/features.cu, feature_stats_kernel), and a rank's own rows would give other numbers."""
+        T = item_clicked.shape[1]
+        pos = np.flatnonzero((np.arange(T)[None, :] < lens_g[:, None]).reshape(-1))
+        row_pos = np.concatenate([pos, np.zeros(cand.size, np.int64)]).astype(np.int32)
+        row_item = np.concatenate([np.asarray(item_clicked, dtype=np.int64).reshape(-1)[pos], cand])
+        t, d = st['t'], self.dev
+        stats = torch.empty(24, device=d)
+        ops.feature_stats(t['buffer'], self.n_norm, self.created_at, t['pop_norm'], t['max_ts'], self.lb_rec, self.lb_nov,
+                          torch.from_numpy(row_pos).to(d), torch.from_numpy(row_item).to(d), row_pos.size, pos.size, 0,
+                          t['event_ts'], stats)
+        return stats
 
     # ---- unsampled evaluation (DESIGN.md section 13): rank each label against every candidate the sampler could draw
     MAX_RANK_SESSION = 1023           # positions T of a batch: the session row of T + 1 ids is the kernel's exclusion list

@@ -297,7 +297,9 @@ class Estimator:
         [n_positions, top_n] with ``positions='all'``).  The recommendation is for the article after the session's last
         valid position (``label_last_item`` on an input_fn batch).  ``top_n`` defaults to eval_metrics_top_n;
         ``candidates``: None = the distinct ids of the current recent-clicks buffer, 'catalog' = every article, or an array
-        of ids.  Weights as ``evaluate`` gets them; ClickedItemsState, weights, Adam slots and global_step are only read."""
+        of ids.  Weights as ``evaluate`` gets them; ClickedItemsState, weights, Adam slots and global_step are only read.
+        Data parallel (``params['process_group']``): every rank runs the same ``input_fn`` and arguments, scores its share
+        of each batch's sessions (NarEngine.recommend) and yields the same dicts as one process."""
         import torch
         if positions not in ('last', 'all'):
             raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
@@ -305,8 +307,6 @@ class Estimator:
             if getattr(self, '_predict_spec', None) is None:
                 self._predict_spec = self.model_fn(features, labels, ModeKeys.PREDICT, self.params)
             spec = self._predict_spec
-            if spec.model.engine.world > 1:
-                raise NotImplementedError('Estimator.predict runs on one process; data-parallel prediction is not implemented')
             if n == 0:
                 self._use_trained_weights(spec, 'predict')
             state = self._state()

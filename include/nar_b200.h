@@ -483,6 +483,11 @@ typedef struct {
   void* prep_ws;  int64_t prep_ws_bytes;      /* results of nar_engine_prepare (one slot per step in flight) */
   void* ws;       int64_t ws_bytes;           /* activations / activation gradients of the step */
   float* loss;                                /* [4] device: {cross-entropy (mean over L_global), l2 regulariser, -, -} */
+  /* optional [24] device, read by nar_engine_recommend / nar_engine_rank_labels (steps ignore it): the call's
+   * feature-normalisation statistics, computed by the caller; NULL: computed from the call's rows.  With an empty
+   * recent-clicks buffer the statistics of the clicked rows are taken over those rows, so a data-parallel rank passes
+   * the statistics of the global batch's rows here */
+  const float* stats;
 } nar_step_io;
 
 typedef struct nar_engine nar_engine;

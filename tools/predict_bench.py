@@ -6,7 +6,15 @@ Per set it prints one JSON line: ms per batch (CUDA events around whole calls af
 sessions/s, candidate pairs/s, model FLOP/s at 2*(C^2 + 128*C + 128*64 + 64*32) per pair, the achieved rate of the CAR
 layer-2 GEMM (2*pairs*C^2 over its own time, timed standalone at the chunk shape the call used, bf16x3 like the engine),
 the top-n kernel time on a [Q, N] logits matrix, and the GPU name and power limit.  Writes nothing.
-Usage: python tools/predict_bench.py [--repeats 5] [--warm-batches 30] [--top-n 10]"""
+Usage: python tools/predict_bench.py [--repeats 5] [--warm-batches 30] [--top-n 10]
+
+--dp: data-parallel prediction (DESIGN.md section 8), one rank per GPU, launched by torchrun over NCCL:
+  torchrun --nproc-per-node N tools/predict_bench.py --dp
+Per candidate set, rank 0 prints one JSON line: sessions/s of a one-process engine at batch 256 (the other GPUs idle) and
+of the data-parallel engine at the global batch 256 * N, the scaling between them, and every rank's GPU name and power
+limit.  Host clock around whole calls (each ends with the results on the host), median of the repeats.  Without
+torchrun, or with one GPU, only the one-process rate is measured and the scaling is reported as not measured; ranks
+sharing a GPU are refused, since their rate says nothing about N GPUs."""
 from __future__ import annotations
 
 import argparse
@@ -52,14 +60,93 @@ def time_ms(fn, repeats, warmup=2):
     return float(np.median(ts)), [round(t, 3) for t in ts]
 
 
+def host_ms(fn, repeats, warmup=2):
+    """Median wall time of whole calls that end with their results on the host (recommend copies them back)."""
+    import time
+    for _ in range(warmup):
+        fn()
+    ts = []
+    for _ in range(repeats):
+        t0 = time.perf_counter()
+        fn()
+        ts.append((time.perf_counter() - t0) * 1e3)
+    return float(np.median(ts)), [round(t, 3) for t in ts]
+
+
+def dp_main(args):
+    import torch.distributed as dist
+    world = int(os.environ.get('WORLD_SIZE', '1'))
+    rank, local = int(os.environ.get('RANK', '0')), int(os.environ.get('LOCAL_RANK', '0'))
+    if world > torch.cuda.device_count():
+        raise SystemExit('--dp runs one rank per GPU: %d ranks, %d GPUs' % (world, torch.cuda.device_count()))
+    torch.cuda.set_device(local)
+    pg = None
+    if world > 1:
+        dist.init_process_group('nccl', device_id=torch.device('cuda', local))
+        pg = dist.group.WORLD
+    per = 256
+    pb = make_problem('g1', profile='B', batch_size=per * world)
+    warm_state(pb, args.warm_batches)
+    logical = pb.layout.init_logical(pb.hp.init_seed)
+    feats, _ = pb.input_fn().get_next()
+    buf = pb.clicked_items_state.get_recent_clicks_buffer().copy()
+    pop = pb.clicked_items_state.get_articles_recent_pop_norm().copy()
+    one_feats = {k: np.asarray(v)[:per] for k, v in feats.items()}       # one GPU's share: the first 256 sessions
+    gpus = [None] * world
+    if world > 1:
+        dist.all_gather_object(gpus, gpu_info())
+    else:
+        gpus = [gpu_info()]
+    eng1 = None
+    if rank == 0:
+        eng1 = make_engine(pb)
+        eng1.set_params(logical)
+    engn = make_engine(pb, process_group=pg) if world > 1 else None
+    if engn is not None:
+        engn.set_params(logical)
+    for cands in (None, 'catalog'):
+        res = {'candidates': 'buffer' if cands is None else cands, 'batch_per_gpu': per, 'world': world, 'top_n': args.top_n,
+               'gpus': [{'name': n, 'power_limit_max_sm_clock': lim} for n, lim in gpus]}
+        if rank == 0:
+            last = {}
+
+            def one():
+                last['out'] = eng1.recommend(one_feats, buf, pop, args.top_n, candidates=cands)
+            ms1, all1 = host_ms(one, args.repeats)
+            q1 = last['out']['query_session'].size
+            res.update(world1_ms=round(ms1, 3), world1_ms_repeats=all1, world1_sessions_per_s=round(q1 / ms1 * 1e3, 1))
+        if world > 1:
+            dist.barrier()
+            last = {}
+
+            def dp():
+                last['out'] = engn.recommend(feats, buf, pop, args.top_n, candidates=cands)
+            msn, alln = host_ms(dp, args.repeats)
+            qn = last['out']['query_session'].size
+            res.update(worldN_ms=round(msn, 3), worldN_ms_repeats=alln, worldN_sessions_per_s=round(qn / msn * 1e3, 1))
+            if rank == 0:
+                res['scaling'] = round(res['worldN_sessions_per_s'] / res['world1_sessions_per_s'], 3)
+        else:
+            res['scaling'] = 'not measured (one GPU: data-parallel prediction needs one GPU per rank)'
+        if rank == 0:
+            print(json.dumps(res))
+            sys.stdout.flush()
+    if world > 1:
+        dist.barrier()
+        dist.destroy_process_group()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--repeats', type=int, default=5)
     ap.add_argument('--warm-batches', type=int, default=30)
     ap.add_argument('--top-n', type=int, default=10)
+    ap.add_argument('--dp', action='store_true', help='data-parallel mode (torchrun, one rank per GPU)')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('predict_bench needs a CUDA device')
+    if args.dp:
+        return dp_main(args)
     name, limit = gpu_info()
     pb = make_problem('g1', profile='B')
     warm_state(pb, args.warm_batches)
