@@ -171,11 +171,15 @@ _SIGNATURES = {
                                       C.c_double, C.c_double, i32, i32, vp, vp, vp, vp, vp]),
     'nar_baselines_rank_unsampled': (C.c_int, [vp, vp, vp, vp, i64, vp, vp, vp, i64, i64, vp, i64, vp, vp, vp, vp, i64,
                                                i64, vp, i64, C.c_double, C.c_double, i32, i32, i64, vp, vp, vp, vp]),
+    'nar_baselines_recommend': (C.c_int, [vp, vp, vp, vp, i64, vp, i64, i64, vp, i64, vp, i64, i32, vp, vp, vp, vp, i64,
+                                          i64, vp, i64, C.c_double, C.c_double, i32, i32, i64, vp, vp, vp, vp]),
     'nar_sknn_update': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, i64, i64, i64, vp, vp]),
     'nar_sknn_score': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, i64, i64, i64, i64, i64, i64, i32, i32, i32,
                                  vp, vp, vp, vp, vp]),
     'nar_sknn_rank_unsampled': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, i64, i64, vp, i64, i64, i64, i64,
                                           i32, i32, i32, i64, vp, vp, vp, vp]),
+    'nar_sknn_recommend': (C.c_int, [vp, vp, vp, i64, i64, i64, i64, vp, i64, i64, vp, i64, vp, i64, i32, i64, i64, i64,
+                                     i32, i32, i32, i64, vp, vp, vp, vp]),
     'nar_eval_metrics_mark': (C.c_int, [vp, i64, i64, i32, vp, vp, vp]),
     'nar_eval_metrics_lists': (C.c_int, [vp, i64, i64, i64, i64, i64, i64, i32, vp, i64, vp, vp, i64, i64, vp, i64,
                                          C.c_double, vp, vp, vp, vp]),

@@ -25,7 +25,7 @@ import torch
 
 from . import _lib
 from ._lib import check
-from .sknn import KNN_SUFFIXES, SessionKNN, parse_params as _knn_params
+from .sknn import KNN_SUFFIXES, MAX_T as MAX_KNN_T, SessionKNN, parse_params as _knn_params
 
 SUFFIXES = ('pop_recent', 'coocurrent', 'item_knn', 'cb', 'sr')
 DEFAULT_PARAMS = {'pop_recent': {}, 'coocurrent': {}, 'item_knn': {'reg_lambda': 20, 'alpha': 0.75}, 'cb': {},
@@ -298,6 +298,69 @@ class BaselineTables:
             self.alpha, self.mask, int(top_n), int(max_blocks), _p(None if rank is None else rank[:len(SUFFIXES)]),
             _p(hist), _p(self.err), stream), 'nar_baselines_rank_unsampled')
 
+    MAX_TOP_N = 1024                  # list entries the recommendation kernels keep per query
+    MAX_T = 1024                      # positions of a batch the table baselines' exclusion list holds
+
+    def recommend(self, suffix: str, item_clicked: torch.Tensor, q_pos: torch.Tensor, candidates: torch.Tensor,
+                  buffer_ids, articles_pop, top_n: int, exclude_session_clicks: bool = True, max_blocks: int = 0):
+        """Recommendations of baseline ``suffix`` (DESIGN.md section 16): for every query at flat position ``q_pos`` [Q]
+        (int32 device, b*T + t) of ``item_clicked`` [B, T] (int64 device), the first ``top_n`` ids of ``candidates`` [N]
+        (ascending distinct int64 device ids in [1, num_items)) in the baseline's order among the ids it admits, without
+        the query's clicks item_clicked[b, 0..t] when ``exclude_session_clicks``.  ``buffer_ids``: the recent-clicks buffer
+        the popularity baseline counts (its histogram is rebuilt, as ``score`` does); ``articles_pop``: the popularity
+        item_knn normalises with.  Reads the tables and rings; writes nothing else.  Queues work on the current stream,
+        no host synchronisation.  -> (ids [Q, top_n] int64, scores [Q, top_n] float64) device tensors: the baseline's own
+        scores, then id 0 with score NaN where fewer ids are admissible.  ``max_blocks`` > 0 caps the kernel's grid.
+        The kernel checks the candidates' order on the device: ids that are not strictly ascending set the error flag,
+        and ``check_errors`` (the next synchronising call) raises ValueError."""
+        if suffix not in self.enabled:
+            raise ValueError('baseline %r is not enabled here (enabled: %s)' % (suffix, ', '.join(self.enabled)))
+        if isinstance(top_n, (bool, np.bool_)) or not isinstance(top_n, (int, np.integer)) or \
+                not 1 <= int(top_n) <= self.MAX_TOP_N:
+            raise ValueError('top_n must be an integer in [1, %d], not %r' % (self.MAX_TOP_N, top_n))
+        top_n = int(top_n)
+        B, T = item_clicked.shape
+        limit = MAX_KNN_T if suffix in KNN_SUFFIXES else self.MAX_T
+        if T > limit:
+            raise ValueError('baseline %r recommends for sessions of at most %d positions, not %d' % (suffix, limit, T))
+        for name, x, dt in (('item_clicked', item_clicked, torch.int64), ('q_pos', q_pos, torch.int32),
+                            ('candidates', candidates, torch.int64)):
+            if not torch.is_tensor(x) or x.device != self.dev or x.dtype != dt or not x.is_contiguous():
+                raise ValueError('%s must be a contiguous %s tensor on %s' % (name, dt, self.dev))
+        s = torch.cuda.current_stream(self.dev)
+        self._wait(s)
+        d = self.dev
+        Q = q_pos.numel()
+        ids = torch.empty(Q, top_n, dtype=torch.int64, device=d)
+        scores = torch.empty(Q, top_n, dtype=torch.float64, device=d)
+        if Q == 0:
+            return ids, scores
+        stream = C.c_void_p(s.cuda_stream)
+        if suffix in self.knn:
+            self.knn[suffix].recommend(item_clicked, B, T, q_pos, candidates, exclude_session_clicks, top_n, ids, scores,
+                                       s, max_blocks)
+            return ids, scores
+
+        def up(x):                    # host arrays go up through a pinned copy on the stream: no host synchronisation
+            if torch.is_tensor(x) and x.is_cuda:
+                return x.to(d, torch.int64).contiguous().view(-1)
+            host = torch.as_tensor(np.ascontiguousarray(np.asarray(x, dtype=np.int64).reshape(-1)))
+            with torch.cuda.stream(s):
+                return host.pin_memory().to(d, non_blocking=True)
+        if suffix == 'pop_recent':
+            buf = up(buffer_ids)
+            check(self.lib.nar_baselines_buffer_hist(_p(buf), buf.numel(), self.num_items, _p(self.hist_count),
+                                                     _p(self.hist_first), _p(self.err), stream), 'nar_baselines_buffer_hist')
+        pop = up(articles_pop) if suffix == 'item_knn' else None
+        check(self.lib.nar_baselines_recommend(
+            *[_p(x) for x in self._tables()], self.cap, _p(item_clicked), B, T, _p(q_pos), Q, _p(candidates),
+            candidates.numel(), int(bool(exclude_session_clicks)), _p(getattr(self, 'hist_count', None)),
+            _p(getattr(self, 'hist_first', None)), _p(pop), _p(self.acr), self.acr_dim,
+            0 if self.acr is None else self.acr.shape[1], _p(self.acr_norm), self.num_items, self.reg_lambda, self.alpha,
+            SUFFIXES.index(suffix), top_n, int(max_blocks), _p(ids), _p(scores), _p(self.err), stream),
+            'nar_baselines_recommend')
+        return ids, scores
+
     def unsampled_results(self, hist) -> Dict[str, float]:
         """{'unsampled_hitrate_at_n_<suffix>', 'unsampled_mrr_at_n_<suffix>', 'unsampled_ndcg_at_n_<suffix>'} of the
         enabled baselines and 'unsampled_candidates_per_query' from an [n_rows, top_n + 2] accumulator
@@ -356,6 +419,9 @@ class BaselineTables:
             raise ValueError('baselines: an article id lies outside [0, num_items)')
         if e == 2:
             raise RuntimeError('baselines: pair table overflow')
+        if e == 3:
+            self.err.zero_()                  # an argument error: the tables are intact, later calls may proceed
+            raise ValueError('baselines: recommendation candidates must be strictly ascending (distinct, sorted) ids')
 
     def export(self) -> Dict[str, np.ndarray]:
         s = torch.cuda.current_stream(self.dev)

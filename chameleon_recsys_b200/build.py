@@ -32,7 +32,7 @@ def _stale(target: str, deps) -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    hdrs = [os.path.join(CSRC, 'common.cuh'), os.path.join(HERE, '..', 'include', 'nar_b200.h')]
+    hdrs = [os.path.join(CSRC, 'common.cuh'), os.path.join(CSRC, 'select_topn.cuh'), os.path.join(HERE, '..', 'include', 'nar_b200.h')]
     objdir = os.path.join(HERE, '..', 'build', 'obj')
     os.makedirs(objdir, exist_ok=True)
     nvcc = _nvcc()

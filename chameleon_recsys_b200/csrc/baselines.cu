@@ -10,6 +10,7 @@
 //            running over (session, i, j) in the reference's loop order
 // Integer atomics only: the table contents do not depend on thread scheduling (slot placement does; exports sort).
 #include "common.cuh"
+#include "select_topn.cuh"
 
 namespace nar {
 namespace bl {
@@ -410,6 +411,84 @@ __global__ void __launch_bounds__(RANK_NT) rank_unsampled_kernel(ScoreArgs a) {
   }
 }
 
+// ---- recommendations (DESIGN.md section 16): the top n of one baseline's order over a candidate set
+constexpr int REC_NT = 256;
+
+struct RecArgs {
+  const int32_t* q_pos; int64_t n_q;     // queries: flat positions b*T + t of item_clicked [B, T]
+  const int64_t* cand; int64_t N;        // distinct candidate ids in [1, num_items)
+  int exclude;                           // drop the query's clicks item_clicked[b, 0..t]
+  int bl;                                // baseline: 0 pop_recent, 1 coocurrent, 2 item_knn, 3 cb, 4 sr
+  int top_n;
+  int64_t* out_ids; double* out_scores;  // [n_q, top_n]
+};
+
+// One CTA per query (grid-stride over the queries when the grid is capped).  The query's clicks sit behind the Bloom
+// filter of rank_unsampled_kernel; the candidates are walked in tiles of REC_NT, each id scored as pair_score / cb_score
+// score it (cb: one warp per id, 32 ids per warp and tile), and the admissible ones go through sel::offer.
+__global__ void __launch_bounds__(REC_NT) recommend_kernel(ScoreArgs a, RecArgs r) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  sel::KeySel& S = *reinterpret_cast<sel::KeySel*>(smem);
+  __shared__ int64_t s_excl[MAX_SESSION];
+  __shared__ uint32_t s_bloom[BLOOM_WORDS];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int bl = r.bl;
+  for (int64_t q = blockIdx.x; q < r.n_q; q += gridDim.x) {
+    const int64_t pos = r.q_pos[q];
+    const int64_t b = pos / a.T, t = pos - b * a.T;
+    const int64_t item = pos >= 0 && b < a.B ? a.item_clicked[pos] : 0;
+    __syncthreads();                                            // the previous query is done with shared memory
+    if (item <= 0 || item >= a.num_items) {                     // block-uniform
+      if (tid == 0) atomicExch(a.err, 1);
+      for (int i = tid; i < r.top_n; i += REC_NT) {
+        r.out_ids[q * r.top_n + i] = 0;
+        r.out_scores[q * r.top_n + i] = __longlong_as_double(0x7ff8000000000000LL);
+      }
+      continue;
+    }
+    for (int i = tid; i < BLOOM_WORDS; i += REC_NT) s_bloom[i] = 0u;
+    sel::begin<REC_NT>(S);
+    const int n_excl = r.exclude ? (int)(t + 1) : 0;
+    for (int i = tid; i < n_excl; i += REC_NT) {
+      const int64_t id = a.item_clicked[b * a.T + i];
+      s_excl[i] = id;
+      const uint32_t h = bloom_slot(id);
+      atomicOr(&s_bloom[h >> 5], 1u << (h & 31));
+    }
+    __syncthreads();
+    auto excluded = [&](int64_t c) -> bool {
+      const uint32_t h = bloom_slot(c);
+      if (s_bloom[h >> 5] & (1u << (h & 31)))
+        for (int i = 0; i < n_excl; ++i)
+          if (s_excl[i] == c) return true;
+      return false;
+    };
+    if (q == 0)                                                 // the selection's key is strict only over distinct ids
+      for (int64_t j = tid + 1; j < r.N; j += REC_NT)
+        if (r.cand[j] <= r.cand[j - 1]) atomicExch(a.err, 3);
+    for (int64_t j0 = 0; j0 < r.N; j0 += REC_NT) {
+      bool ok = false; double sc = 0.0; long long tie = 0; int64_t c = 0;
+      if (bl == 3) {                                            // block-uniform
+        for (int k = 0; k < 32; ++k) {
+          const int64_t j = j0 + w * 32 + k;
+          if (j >= r.N) break;                                  // warp-uniform
+          const int64_t cc = r.cand[j];
+          if (cc <= 0 || cc >= a.num_items) { if (lane == 0) atomicExch(a.err, 1); continue; }
+          if (excluded(cc)) continue;
+          const double s = cb_score(a, item, cc, lane);
+          if (lane == k) { sc = s; tie = -(long long)cc; ok = true; c = cc; }
+        }
+      } else if (j0 + tid < r.N) {
+        c = r.cand[j0 + tid];
+        if (c <= 0 || c >= a.num_items) atomicExch(a.err, 1);
+        else if (!excluded(c)) { int o; pair_score(a, bl, item, c, sc, tie, o); ok = o; }
+      }
+      sel::offer<REC_NT, REC_NT>(S, r.top_n, ok, sc, tie, (int)c);
+    }
+    sel::finish<REC_NT>(S, r.top_n, r.out_ids + q * r.top_n, r.out_scores + q * r.top_n);
+  }
+}
+
 static inline bool pow2(int64_t x) { return x > 0 && (x & (x - 1)) == 0; }
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
@@ -559,6 +638,47 @@ extern "C" int nar_baselines_rank_unsampled(const int64_t* keys, const int64_t* 
   a.all_items = all_items; a.pool = pool; a.n_pool = N; a.rank = rank;
   const int64_t grid = max_blocks > 0 && max_blocks < nq ? max_blocks : nq;
   rank_unsampled_kernel<<<(unsigned)grid, RANK_NT, 0, s>>>(a);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_baselines_recommend(const int64_t* keys, const int64_t* cooc, const int64_t* sr_w,
+                                       const int64_t* sr_first, int64_t cap, const int64_t* item_clicked, int64_t B,
+                                       int64_t T, const int32_t* q_pos, int64_t Q, const int64_t* cand, int64_t N,
+                                       int32_t exclude, const int32_t* buf_count, const int32_t* buf_first,
+                                       const int64_t* articles_pop, const float* acr, int64_t acr_dim, int64_t acr_ld,
+                                       const double* acr_norm, int64_t num_items, double knn_lambda, double knn_alpha,
+                                       int32_t baseline, int32_t top_n, int64_t max_blocks, int64_t* out_ids,
+                                       double* out_scores, int* err, void* stream) {
+  if (!item_clicked || (!q_pos && Q > 0) || (!cand && N > 0) || !out_ids || !out_scores || !err || B < 0 || T <= 0 ||
+      Q < 0 || N < 0 || top_n < 1 || num_items <= 0 || num_items > 0x7fffffffLL || baseline < 0 || baseline >= N_BASELINES)
+    return NAR_ERR_INVALID;
+  if (baseline == 0 && (!buf_count || !buf_first)) return NAR_ERR_INVALID;
+  if ((baseline == 1 || baseline == 2 || baseline == 4) && (!keys || !cooc || !sr_w || !sr_first || !pow2(cap)))
+    return NAR_ERR_INVALID;
+  if (baseline == 2 && !articles_pop) return NAR_ERR_INVALID;
+  if (baseline == 3 && (!acr || !acr_norm || acr_dim <= 0 || acr_ld < acr_dim)) return NAR_ERR_INVALID;
+  if (top_n > nar::sel::MAX_TOP || T > MAX_SESSION || Q > 0x7fffffffLL || B * T > 0x7fffffffLL) return NAR_ERR_UNSUPPORTED;
+  if (Q == 0) return NAR_OK;
+  cudaStream_t s = as_stream(stream);
+  constexpr size_t smem = sizeof(nar::sel::KeySel);
+  static bool attr = false;
+  if (!attr) {
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(recommend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr = true;
+  }
+  ScoreArgs a = {};
+  a.keys = reinterpret_cast<const unsigned long long*>(keys); a.cooc = (const long long*)cooc;
+  a.sr_w = (const long long*)sr_w; a.sr_first = (const long long*)sr_first; a.cap = cap;
+  a.item_clicked = item_clicked; a.B = B; a.T = T;
+  a.buf_count = buf_count; a.buf_first = buf_first; a.articles_pop = articles_pop;
+  a.acr = acr; a.acr_dim = acr_dim; a.acr_ld = acr_ld; a.acr_norm = acr_norm; a.num_items = num_items;
+  a.knn_lambda = knn_lambda; a.knn_alpha = knn_alpha; a.enabled = 1 << baseline; a.top_n = top_n; a.err = err;
+  RecArgs r;
+  r.q_pos = q_pos; r.n_q = Q; r.cand = cand; r.N = N; r.exclude = exclude != 0; r.bl = baseline; r.top_n = top_n;
+  r.out_ids = out_ids; r.out_scores = out_scores;
+  const int64_t grid = max_blocks > 0 && max_blocks < Q ? max_blocks : Q;
+  recommend_kernel<<<(unsigned)grid, REC_NT, smem, s>>>(a, r);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

@@ -15,6 +15,7 @@
 // ring in insertion order, the 'recent' cut, fp64 similarities in the reference's association, the neighbour cut, item
 // scores of the query's own candidates summed copy by copy, exact ranking and an integer rank histogram.
 #include "common.cuh"
+#include "select_topn.cuh"
 
 namespace nar {
 namespace sknn {
@@ -528,6 +529,78 @@ __global__ void __launch_bounds__(ST) rank_unsampled_kernel(ScoreArgs a) {
   }
 }
 
+// ---- recommendations (DESIGN.md section 16): the top n of the kNN order over a candidate set
+struct RecArgs {
+  const int32_t* q_pos; int64_t n_q;     // queries: flat positions b*T + t of item_clicked [B, T]
+  const int64_t* cand; int64_t N;        // ascending distinct candidate ids in [1, num_items)
+  int exclude;                           // drop the query's clicks item_clicked[b, 0..t]
+  int top_n;
+  int64_t* out_ids; double* out_scores;  // [n_q, top_n]
+};
+
+// dynamic shared memory of recommend_kernel: the ring's arrays, then the selection state
+__host__ __device__ __forceinline__ size_t rec_sel_offset(int64_t count) {
+  const int64_t sc = count > 0 ? count : 1;
+  int64_t n2 = 1;
+  while (n2 < sc) n2 <<= 1;
+  return (size_t)((28 * sc + 2 * n2 + 15) & ~15LL);     // score_smem(count), 16-byte aligned
+}
+
+// One CTA per query (grid-stride over the queries when the grid is capped): the neighbours of the sampled kernel, then
+// the candidates 64 ids at a time as rank_unsampled_kernel walks its pool (neighbour masks, item sums copy by copy); an
+// id a kept neighbour holds is admissible with key (score desc, first neighbour asc, id asc) and goes through
+// sel::offer.  No kept neighbour: every entry is padding.
+__global__ void __launch_bounds__(ST) recommend_kernel(ScoreArgs a, RecArgs r) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const RingShared ring(smem, (int)a.count);
+  sel::KeySel& S = *reinterpret_cast<sel::KeySel*>(smem + rec_sel_offset(a.count));
+  __shared__ int s_chunk[64];
+  __shared__ int64_t s_row[MAX_T];
+  const int tid = threadIdx.x;
+  for (int64_t q = blockIdx.x; q < r.n_q; q += gridDim.x) {
+    const int64_t pos = r.q_pos[q];
+    const int64_t b = pos / a.T, t = pos - b * a.T;
+    const int64_t item = pos >= 0 && b < a.B ? a.item_clicked[pos] : 0;
+    __syncthreads();                                                 // the previous query is done with shared memory
+    sel::begin<ST>(S);
+    if (item <= 0 || item >= a.num_items) {                          // block-uniform
+      if (tid == 0) atomicExch(a.err, 1);
+      sel::finish<ST>(S, r.top_n, r.out_ids + q * r.top_n, r.out_scores + q * r.top_n);
+      continue;
+    }
+    const int n_excl = r.exclude ? (int)(t + 1) : 0;
+    if (tid < n_excl) s_row[tid] = a.item_clicked[b * a.T + tid];
+    if (q == 0)                                  // neighbour_masks' search and the selection's key need ascending ids
+      for (int64_t j = tid + 1; j < r.N; j += ST)
+        if (r.cand[j] <= r.cand[j - 1]) atomicExch(a.err, 3);
+    const int nb = select_neighbours(a, b, (int)t + 1, ring);
+    for (int64_t c0 = 0; nb > 0 && c0 < r.N; c0 += 64) {            // block-uniform
+      const int cn = (int)min((int64_t)64, r.N - c0);
+      if (tid < cn) {
+        int64_t id = r.cand[c0 + tid];
+        if (id <= 0 || id >= a.num_items) { atomicExch(a.err, 1); id = 0; }
+        s_chunk[tid] = (int)id;
+      }
+      __syncthreads();
+      neighbour_masks(a, nb, ring, s_chunk, cn);
+      bool ok = false; double sc_ = 0.0; long long tie = 0; int id = 0;
+      if (tid < cn) {
+        id = s_chunk[tid];
+        bool keep = id != 0;
+        for (int i = 0; i < n_excl && keep; ++i) keep = s_row[i] != id;
+        if (keep) {
+          int f;
+          item_score(nb, ring, tid, sc_, f);
+          ok = f >= 0;
+          tie = ((long long)f << 32) | (unsigned)id;
+        }
+      }
+      sel::offer<ST, 64>(S, r.top_n, ok, sc_, tie, id);            // its barrier: s_chunk / acc are free again
+    }
+    sel::finish<ST>(S, r.top_n, r.out_ids + q * r.top_n, r.out_scores + q * r.top_n);
+  }
+}
+
 // metrics += {hits, sum of reciprocal ranks, queries}, summed over the rank histogram in a fixed order
 __global__ void finalize_kernel(const unsigned long long* h, int top_n, double* metrics) {
   unsigned long long hits = 0; double rr = 0.0;
@@ -629,6 +702,40 @@ extern "C" int nar_sknn_rank_unsampled(const int64_t* ids, const int32_t* lens, 
   a.all_items = all_items; a.pool = pool; a.n_pool = N; a.rank = rank;
   const int64_t grid = max_blocks > 0 && max_blocks < nq ? max_blocks : nq;
   rank_unsampled_kernel<<<(unsigned)grid, ST, score_smem(count), s>>>(a);
+  NAR_LAUNCH_CHECK();
+  return NAR_OK;
+}
+
+extern "C" int nar_sknn_recommend(const int64_t* ids, const int32_t* lens, const int32_t* items, int64_t S, int64_t W,
+                                  int64_t head, int64_t count, const int64_t* item_clicked, int64_t B, int64_t T,
+                                  const int32_t* q_pos, int64_t Q, const int64_t* cand, int64_t N, int32_t exclude,
+                                  int64_t num_items, int64_t sample_size, int64_t nn, int32_t decay_div, int32_t jaccard,
+                                  int32_t top_n, int64_t max_blocks, int64_t* out_ids, double* out_scores, int* err,
+                                  void* stream) {
+  if (!ids || !lens || !items || !item_clicked || (!q_pos && Q > 0) || (!cand && N > 0) || !out_ids || !out_scores ||
+      !err || S <= 0 || W <= 0 || head < 0 || head >= S || count < 0 || count > S || B < 0 || T <= 0 || Q < 0 || N < 0 ||
+      top_n < 1 || num_items <= 0 || num_items > 0x7fffffffLL || sample_size < 0 || nn < 0)
+    return NAR_ERR_INVALID;
+  if (S > MAX_SESSIONS || T > MAX_T || top_n > nar::sel::MAX_TOP || Q > 0x7fffffffLL || B * T > 0x7fffffffLL)
+    return NAR_ERR_UNSUPPORTED;
+  if (Q == 0) return NAR_OK;
+  cudaStream_t s = as_stream(stream);
+  static bool attr = false;
+  if (!attr) {
+    NAR_CHECK_CUDA(cudaFuncSetAttribute(recommend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)(rec_sel_offset(MAX_SESSIONS) + sizeof(nar::sel::KeySel))));
+    attr = true;
+  }
+  ScoreArgs a = {};
+  a.ids = ids; a.lens = lens; a.items = items; a.S = S; a.W = (int)W; a.head = head; a.count = count;
+  a.item_clicked = item_clicked; a.B = B; a.T = T;
+  a.num_items = num_items; a.sample_size = sample_size; a.nn = nn; a.decay_div = decay_div; a.jaccard = jaccard;
+  a.top_n = top_n; a.err = err;
+  RecArgs r;
+  r.q_pos = q_pos; r.n_q = Q; r.cand = cand; r.N = N; r.exclude = exclude != 0; r.top_n = top_n;
+  r.out_ids = out_ids; r.out_scores = out_scores;
+  const int64_t grid = max_blocks > 0 && max_blocks < Q ? max_blocks : Q;
+  recommend_kernel<<<(unsigned)grid, ST, rec_sel_offset(count) + sizeof(nar::sel::KeySel), s>>>(a, r);
   NAR_LAUNCH_CHECK();
   return NAR_OK;
 }

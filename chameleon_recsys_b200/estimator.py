@@ -113,8 +113,15 @@ def nar_module_model_fn(features, labels, mode, params) -> EstimatorSpec:
             return model.train(feats, labs, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], sync=sync)
         return EstimatorSpec(mode, loss=None, train_op=train_op, training_chief_hooks=hooks, model=model)
     if mode == ModeKeys.PREDICT:
-        # one call per batch: the state arrays are read, never updated (no hook runs in PREDICT)
-        def predict(feats, feed, top_n=None, candidates=None, positions='last', exclude_session_clicks=True):
+        # one call per batch: the state arrays are read, never updated (no hook runs in PREDICT).  ``recommender``: a
+        # baseline's suffix recommends with the tables on the ClickedItemsState instead of the model
+        def predict(feats, feed, top_n=None, candidates=None, positions='last', exclude_session_clicks=True,
+                    recommender=None):
+            if recommender is not None:
+                return model.recommend(feats, feed['pop_recent_items_buffer'], None, top_n=top_n, candidates=candidates,
+                                       positions=positions, exclude_session_clicks=exclude_session_clicks,
+                                       recommender=recommender, baselines=hooks[0].baselines,
+                                       articles_pop=feed.get('articles_pop'))
             return model.recommend(feats, feed['pop_recent_items_buffer'], feed['articles_recent_pop_norm'], top_n=top_n,
                                    candidates=candidates, positions=positions, exclude_session_clicks=exclude_session_clicks)
         return EstimatorSpec(mode, loss=None, predictions=predict, model=model)
@@ -291,7 +298,7 @@ class Estimator:
             self._restored = restored
 
     def predict(self, input_fn, steps: Optional[int] = None, top_n: Optional[int] = None, candidates=None,
-                exclude_session_clicks: bool = True, positions: str = 'last'):
+                exclude_session_clicks: bool = True, positions: str = 'last', recommender: Optional[str] = None):
         """tf.estimator.Estimator.predict: a generator over the batches of ``input_fn`` that yields one dict per session -
         ``session_id``, ``predicted_item_ids`` / ``predicted_item_scores`` / ``predicted_item_probs`` [top_n] (arrays
         [n_positions, top_n] with ``positions='all'``).  The recommendation is for the article after the session's last
@@ -299,10 +306,29 @@ class Estimator:
         ``candidates``: None = the distinct ids of the current recent-clicks buffer, 'catalog' = every article, or an array
         of ids.  Weights as ``evaluate`` gets them; ClickedItemsState, weights, Adam slots and global_step are only read.
         Data parallel (``params['process_group']``): every rank runs the same ``input_fn`` and arguments, scores its share
-        of each batch's sessions (NarEngine.recommend) and yields the same dicts as one process."""
+        of each batch's sessions (NarEngine.recommend) and yields the same dicts as one process.
+        ``recommender``: the suffix of one baseline of ``params['eval_benchmarks']`` recommends instead of the model
+        (DESIGN.md section 16), with what it learnt in this Estimator's training or, without one, in the latest
+        checkpoint: the first top_n ids of the valid set it admits, in its own order; ``predicted_item_scores`` are float64
+        and its own scores, id 0 and NaN pad past the admissible ids, and there is no ``predicted_item_probs``.  One
+        process only (NotImplementedError data parallel)."""
         import torch
         if positions not in ('last', 'all'):
             raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
+        if recommender is not None:
+            from .baselines import SUFFIXES, parse_classifiers
+            from .sknn import KNN_SUFFIXES
+            if recommender not in SUFFIXES + KNN_SUFFIXES:
+                raise ValueError('unknown baseline recommender %r (expected one of %s)'
+                                 % (recommender, ', '.join(SUFFIXES + KNN_SUFFIXES)))
+            enabled = list(parse_classifiers(self.params.get('eval_benchmarks') or ()))
+            if recommender not in enabled:
+                raise ValueError('baseline %r is not one of eval_benchmarks (%s)'
+                                 % (recommender, ', '.join(enabled) if enabled else 'none'))
+            pg = self.params.get('process_group')
+            if pg is not None and torch.distributed.get_world_size(pg) > 1:
+                raise NotImplementedError('baseline recommenders run on one process; data-parallel prediction with a '
+                                          'baseline is not implemented')
         for n, (features, labels) in enumerate(_batches(input_fn(), steps)):
             if getattr(self, '_predict_spec', None) is None:
                 self._predict_spec = self.model_fn(features, labels, ModeKeys.PREDICT, self.params)
@@ -312,18 +338,25 @@ class Estimator:
             state = self._state()
             feed = {'pop_recent_items_buffer': state.get_recent_clicks_buffer(),
                     'articles_recent_pop_norm': state.get_articles_recent_pop_norm()}
-            out = spec.predictions(features, feed, top_n=top_n, candidates=candidates, positions=positions,
-                                   exclude_session_clicks=exclude_session_clicks)
+            if recommender is not None:
+                feed['articles_pop'] = state.get_articles_pop()
+                out = spec.predictions(features, feed, top_n=top_n, candidates=candidates, positions=positions,
+                                       exclude_session_clicks=exclude_session_clicks, recommender=recommender)
+            else:
+                out = spec.predictions(features, feed, top_n=top_n, candidates=candidates, positions=positions,
+                                       exclude_session_clicks=exclude_session_clicks)
             sids = features.get('session_id')
             Bg = np.asarray(features['item_clicked']).shape[0]
             qs = out['query_session']
             for b in range(Bg):
                 rows = np.flatnonzero(qs == b)
                 sel = rows[0] if (positions == 'last' and rows.size) else rows
-                yield {'session_id': None if sids is None else np.asarray(sids)[b],
+                row = {'session_id': None if sids is None else np.asarray(sids)[b],
                        'predicted_item_ids': out['predicted_item_ids'][sel],
-                       'predicted_item_scores': out['predicted_item_scores'][sel],
-                       'predicted_item_probs': out['predicted_item_probs'][sel]}
+                       'predicted_item_scores': out['predicted_item_scores'][sel]}
+                if recommender is None:
+                    row['predicted_item_probs'] = out['predicted_item_probs'][sel]
+                yield row
         torch.cuda.synchronize()
 
     def evaluate(self, input_fn, steps: Optional[int] = None, hooks=None, name=None) -> dict:

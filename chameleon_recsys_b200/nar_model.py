@@ -123,13 +123,84 @@ class NARModuleModel:
 
     def recommend(self, features: Dict[str, np.ndarray], pop_recent_items_buffer: np.ndarray,
                   articles_recent_pop_norm: np.ndarray, top_n: Optional[int] = None, candidates=None, positions: str = 'last',
-                  exclude_session_clicks: bool = True) -> dict:
+                  exclude_session_clicks: bool = True, recommender: Optional[str] = None, baselines=None,
+                  articles_pop=None) -> dict:
         """Top-n next-article recommendations for the batch ``features`` (NarEngine.recommend): ``top_n`` defaults to
         ``metrics_top_n``; ``candidates`` None = the recent-clicks buffer's distinct ids, 'catalog' = every article, or an
-        array of ids.  Reads the weights and the given state; changes neither."""
+        array of ids.  Reads the weights and the given state; changes neither.  ``recommender``: the suffix of one
+        baseline of ``baselines`` (the BaselineTables of the ClickedItemsState) recommends instead of the model
+        (recommend_baseline)."""
+        if recommender is not None:
+            return self.recommend_baseline(recommender, baselines, features, pop_recent_items_buffer, articles_pop,
+                                           top_n=top_n, candidates=candidates, positions=positions,
+                                           exclude_session_clicks=exclude_session_clicks)
         return self.engine.recommend(features, pop_recent_items_buffer, articles_recent_pop_norm,
                                      self.metrics_top_n if top_n is None else top_n, candidates=candidates,
                                      positions=positions, exclude_session_clicks=exclude_session_clicks)
+
+    def recommend_baseline(self, recommender: str, baselines, features: Dict[str, np.ndarray],
+                           pop_recent_items_buffer: np.ndarray, articles_pop: Optional[np.ndarray], top_n: Optional[int] = None,
+                           candidates=None, positions: str = 'last', exclude_session_clicks: bool = True) -> dict:
+        """Top-n recommendations of the baseline ``recommender`` (DESIGN.md section 16) for the queries and candidates
+        ``recommend`` would use: the first ``top_n`` admissible ids of each query's valid set in the baseline's order
+        (BaselineTables.recommend), with the popularity baseline counting ``pop_recent_items_buffer`` and item_knn
+        normalising with ``articles_pop``.  Every argument is checked before any launch.  Reads the tables; changes
+        nothing.  -> numpy dict: query_session [Q], query_position [Q], predicted_item_ids [Q, top_n] int64,
+        predicted_item_scores [Q, top_n] float64 (the baseline's own scores; id 0 and NaN past the admissible ids),
+        candidates [N] (ascending)."""
+        import torch
+        from .baselines import SUFFIXES, BaselineTables
+        from .dp import session_lengths
+        from .sknn import KNN_SUFFIXES, MAX_T as MAX_KNN_T
+        if recommender not in SUFFIXES + KNN_SUFFIXES:
+            raise ValueError('unknown baseline recommender %r (expected one of %s)'
+                             % (recommender, ', '.join(SUFFIXES + KNN_SUFFIXES)))
+        if baselines is None or recommender not in baselines.enabled:
+            raise ValueError('baseline %r is not one of eval_benchmarks (%s)'
+                             % (recommender, ', '.join(baselines.enabled) if baselines is not None else 'none'))
+        if self.engine.world > 1:
+            raise NotImplementedError('baseline recommenders run on one process; data-parallel prediction with a baseline '
+                                      'is not implemented')
+        if positions not in ('last', 'all'):
+            raise ValueError("positions must be 'last' or 'all', not %r" % (positions,))
+        if pop_recent_items_buffer is None:
+            raise ValueError('recommend needs the host recent-clicks buffer')
+        if recommender == 'item_knn' and articles_pop is None:
+            raise ValueError("the 'item_knn' baseline needs the articles' popularity")
+        cand = np.sort(self.engine.resolve_candidates(candidates, pop_recent_items_buffer))
+        N = int(cand.size)
+        top_n = self.metrics_top_n if top_n is None else top_n
+        if isinstance(top_n, (bool, np.bool_)) or not isinstance(top_n, (int, np.integer)):
+            raise ValueError('top_n must be an integer')
+        top_n = int(top_n)
+        if not 1 <= top_n <= min(N, BaselineTables.MAX_TOP_N):
+            raise ValueError('top_n=%d outside [1, min(N=%d, %d)]' % (top_n, N, BaselineTables.MAX_TOP_N))
+        item_clicked = np.asarray(features['item_clicked'], dtype=np.int64)
+        Bg, T = item_clicked.shape
+        limit = MAX_KNN_T if recommender in KNN_SUFFIXES else BaselineTables.MAX_T
+        if T > limit:
+            raise ValueError('baseline %r recommends for sessions of at most %d positions, not %d' % (recommender, limit, T))
+        lens_g = session_lengths(features['session_size'], T)
+        if positions == 'last':
+            q_sess = np.flatnonzero(lens_g > 0).astype(np.int64)
+            q_t = (lens_g[lens_g > 0] - 1).astype(np.int64)
+        else:
+            q_sess = np.repeat(np.arange(Bg, dtype=np.int64), lens_g)
+            q_t = np.arange(q_sess.size, dtype=np.int64) - np.repeat(np.cumsum(lens_g) - lens_g, lens_g)
+        out = {'query_session': q_sess, 'query_position': q_t, 'candidates': cand,
+               'predicted_item_ids': np.zeros((q_sess.size, top_n), np.int64),
+               'predicted_item_scores': np.full((q_sess.size, top_n), np.nan)}
+        if q_sess.size == 0:
+            return out
+        d = baselines.dev
+        ids, scores = baselines.recommend(recommender, torch.from_numpy(item_clicked).to(d),
+                                          torch.from_numpy((q_sess * T + q_t).astype(np.int32)).to(d),
+                                          torch.from_numpy(cand).to(d), pop_recent_items_buffer, articles_pop, top_n,
+                                          exclude_session_clicks=exclude_session_clicks)
+        baselines.check_errors()
+        out['predicted_item_ids'] = ids.cpu().numpy()
+        out['predicted_item_scores'] = scores.cpu().numpy()
+        return out
 
     def _publish(self, features, labels, out):
         self.item_clicked = features['item_clicked']

@@ -110,6 +110,15 @@ class SessionKNN:
                                                int(top_n), int(max_blocks), _p(rank_row), _p(hist_row), _p(self.err),
                                                C.c_void_p(stream.cuda_stream)), 'nar_sknn_rank_unsampled')
 
+    def recommend(self, ic, B, T, q_pos, cand, exclude, top_n, out_ids, out_scores, stream, max_blocks: int = 0):
+        """Top-n recommendations against ``cand`` [N] (ascending device ids; DESIGN.md section 16) for the queries at flat
+        positions ``q_pos`` [Q] int32 of ``ic`` [B, T]: ``out_ids`` / ``out_scores`` [Q, top_n] (nar_sknn_recommend)."""
+        check(self.lib.nar_sknn_recommend(_p(self.ids), _p(self.lens), _p(self.items), self.S, WIDTH, self.head, self.count,
+                                          _p(ic), B, T, _p(q_pos), q_pos.numel(), _p(cand), cand.numel(), int(bool(exclude)),
+                                          self.num_items, self.sample_size, self.nn, self.decay_div, self.jaccard, int(top_n),
+                                          int(max_blocks), _p(out_ids), _p(out_scores), _p(self.err),
+                                          C.c_void_p(stream.cuda_stream)), 'nar_sknn_recommend')
+
     # ---- snapshot / restore / export / load
     def snapshot(self):
         self._chk = (self.ids.clone(), self.lens.clone(), self.items.clone(), self.head, self.count)

@@ -577,6 +577,20 @@ int nar_baselines_rank_unsampled(const int64_t* keys, const int64_t* cooc, const
                                  const float* acr, int64_t acr_dim, int64_t acr_ld, const double* acr_norm,
                                  int64_t num_items, double knn_lambda, double knn_alpha, int32_t enabled, int32_t top_n,
                                  int64_t max_blocks, int32_t* rank, int64_t* hist, int* err, void* stream);
+/* Recommendations of one table baseline (DESIGN.md section 16): for every query q < Q at flat position q_pos[q] = b*T + t
+ * of item_clicked [B, T] (T <= 1024), the first top_n ids of cand [N] (distinct ids in [1, num_items)) in the order of
+ * baseline (0 pop_recent, 1 coocurrent, 2 item_knn, 3 cb, 4 sr; inputs as in nar_baselines_score) among the admissible
+ * ones, without item_clicked[b*T + 0..t] when exclude != 0.  out_ids [Q, top_n] int64 and out_scores [Q, top_n] float64
+ * (the baseline's own score), then id 0 and NaN when fewer ids are admissible.  1 <= top_n <= 1024, else
+ * NAR_ERR_UNSUPPORTED above.  max_blocks > 0 caps the grid (one CTA per query otherwise).  Any grid gives the same
+ * bits.  *err = 1 for an id outside [1, num_items), 3 when cand is not strictly ascending.  One launch.          */
+int nar_baselines_recommend(const int64_t* keys, const int64_t* cooc, const int64_t* sr_w, const int64_t* sr_first,
+                            int64_t cap, const int64_t* item_clicked, int64_t B, int64_t T, const int32_t* q_pos, int64_t Q,
+                            const int64_t* cand, int64_t N, int32_t exclude, const int32_t* buf_count,
+                            const int32_t* buf_first, const int64_t* articles_pop, const float* acr, int64_t acr_dim,
+                            int64_t acr_ld, const double* acr_norm, int64_t num_items, double knn_lambda, double knn_alpha,
+                            int32_t baseline, int32_t top_n, int64_t max_blocks, int64_t* out_ids, double* out_scores,
+                            int* err, void* stream);
 
 /* ---- session-based kNN baseline, V-SkNN / SkNN (csrc/sknn.cu, spec oracle/sknn_ref.py) -------------------------------
  * Ring of S slots (logical index i at slot (head + i) % S, count entries, oldest first; head and count are the caller's):
@@ -608,6 +622,15 @@ int nar_sknn_rank_unsampled(const int64_t* ids, const int32_t* lens, const int32
                             int64_t B, int64_t T, const int64_t* pool, int64_t N, int64_t num_items, int64_t sample_size,
                             int64_t nn, int32_t decay_div, int32_t jaccard, int32_t top_n, int64_t max_blocks,
                             int32_t* rank, int64_t* hist, int* err, void* stream);
+/* Recommendations of the kNN baseline (DESIGN.md section 16) with the neighbours of nar_sknn_score: queries, exclusion,
+ * top_n and outputs as in nar_baselines_recommend, over cand [N] (ascending distinct ids in [1, num_items)), in the
+ * order (item score desc, first neighbour asc, id asc) of the ids some kept neighbour holds.  NAR_ERR_UNSUPPORTED for
+ * S > 4096, T > 64 or top_n > 1024.  *err as in nar_baselines_recommend.  One launch.                           */
+int nar_sknn_recommend(const int64_t* ids, const int32_t* lens, const int32_t* items, int64_t S, int64_t W, int64_t head,
+                       int64_t count, const int64_t* item_clicked, int64_t B, int64_t T, const int32_t* q_pos, int64_t Q,
+                       const int64_t* cand, int64_t N, int32_t exclude, int64_t num_items, int64_t sample_size, int64_t nn,
+                       int32_t decay_div, int32_t jaccard, int32_t top_n, int64_t max_blocks, int64_t* out_ids,
+                       double* out_scores, int* err, void* stream);
 
 /* ---- NDCG, item coverage, ESI-R / ESI-RR and EILD-R / EILD-RR of top-n lists (csrc/eval_metrics.cu, spec
  *      oracle/eval_metrics_ref.py; the reference's metrics.py).  Coverage sets are bitmaps of (num_items + 31) / 32
