@@ -219,6 +219,7 @@ extern "C" int nar_dropout_rows(const float* src, float* dst, int64_t rows, int6
                                 int64_t n_input, int64_t n_cand, int64_t K, int tensor_id, float keep_prob, uint64_t seed,
                                 uint32_t step, void* stream) {
   if (!src || !dst || !row_pos || (cols & 3) || (ld & 3) || tensor_id < 0 || tensor_id > 255) return NAR_ERR_INVALID;
+  if ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) return NAR_ERR_INVALID;   // float4 rows
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NAR_ERR_INVALID;
   if (tensor_id == 0 && (n_cand <= 0 || K != n_cand - 1)) return NAR_ERR_INVALID;
   if (rows <= 0 || cols <= 0) return NAR_OK;
@@ -259,6 +260,8 @@ extern "C" int nar_act_bwd(const float* dy, const float* y, int64_t n, int act, 
 extern "C" int nar_residual_add(const float* h, const float* res, int64_t rows, int64_t cols, int64_t ld, float* out,
                                 void* stream) {
   if (!h || !res || !out || cols < 0 || (cols & 3) || (ld & 3) || ld < cols) return NAR_ERR_INVALID;
+  if ((reinterpret_cast<uintptr_t>(h) | reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(out)) & 15u)
+    return NAR_ERR_INVALID;                                                                        // float4 accesses
   if (rows <= 0 || cols == 0) return NAR_OK;
   nar::misc::residual_add_kernel<<<nar::misc::grid_for(rows * (cols / 4), 256), 256, 0, as_stream(stream)>>>(
       h, res, rows, (int)(cols / 4), ld, out);

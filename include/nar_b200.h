@@ -394,7 +394,8 @@ int nar_state_update(const int64_t* old_items, const int64_t* old_ts, int64_t ca
  *      tensor_id > 0: every row belongs to that tensor, row key = row_pos[r] (flat position b*T+t).
  *      tensor_id == 0: feature rows in the n_cand > 0 layout of nar_row_layout: rows [0,n_input) tensor 1 (key =
  *      position), then per position the positive (tensor 2, key = position) and K negatives (tensor 3, key =
- *      position*K + k).  In place (dst == src) is allowed.                                                        */
+ *      position*K + k).  In place (dst == src) is allowed.  cols and ld multiples of 4, src and dst 16-byte aligned
+ *      (float4 accesses; checked even when there is nothing to do): NAR_ERR_INVALID otherwise.                      */
 int nar_dropout_rows(const float* src, float* dst, int64_t rows, int64_t cols, int64_t ld, const int32_t* row_pos,
                      int64_t n_input, int64_t n_cand, int64_t K, int tensor_id, float keep_prob, uint64_t seed,
                      uint32_t step, void* stream);
@@ -408,7 +409,9 @@ int nar_act_bwd(const float* dy, const float* y, int64_t n, int act, float* dx, 
 int nar_l2_loss_add(const float* x, int64_t n, float scale, float* out, void* stream);
 int nar_transpose_f32(const float* src, int64_t rows, int64_t cols, int64_t ld_src, float* dst, int64_t ld_dst, void* stream);
 /* out[r, c] = h[r, c] + res[r, c] over rows x cols, all three with leading dimension ld (the residual session stack's
- * layer output: the cell's h plus the layer input).  cols and ld multiples of 4; out may be h or res.                */
+ * layer output: the cell's h plus the layer input).  cols and ld multiples of 4, ld >= cols, h, res and out 16-byte
+ * aligned (float4 accesses; checked even when rows or cols is 0): NAR_ERR_INVALID otherwise.
+ * out may be h or res.                                                                                                */
 int nar_residual_add(const float* h, const float* res, int64_t rows, int64_t cols, int64_t ld, float* out, void* stream);
 
 /* ---- optimiser (replaces tf.train.AdamOptimizer(lr,.9,.999,1e-8) nar_model.py:708-722;

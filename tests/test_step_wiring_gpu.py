@@ -123,11 +123,12 @@ def _adam_ref(layout, regularised, raw, reg, lr):
     return (p1, m1, v1), (b1 * np.abs(m0) + (1 - b1) * ag, b2 * v0 + (1 - b2) * ag * ag)
 
 
-def measure(case):
-    """Run one case of CASES -> the worst value of every measured quantity over its steps."""
+def measure(case, cases=CASES):
+    """Run one case of `cases` (CASES, or another dict of the same form) -> the worst value of every measured quantity
+    over its steps."""
     import torch
     from tools import gpu_step_check as g
-    cfg = CASES[case]
+    cfg = cases[case]
     fwd, bwd = cfg.get('prec', (3, 3))
     ekw = dict(fwd_precision=fwd, bwd_precision=bwd, **cfg.get('ekw', {}))
     res = g.run_case(cfg.get('name', 'tiny'), cfg.get('profile', 'B'), cfg.get('warm', 5), cfg.get('steps', 2),
